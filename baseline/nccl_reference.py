@@ -1,7 +1,7 @@
 """Same-box baseline: the reference's *algorithm* on stock libraries.
 
 The reference stack (TF 1.11 fork + Horovod 0.16.3 + OpenMPI) cannot be built
-for sm_100 offline, so BASELINE.md defines the same-box comparison as a
+for sm_90 offline, so BASELINE.md defines the same-box comparison as a
 reference-equivalent path written against `torch.distributed` with Horovod
 semantics, using none of parallax_b200's kernels or engine:
 

@@ -1,4 +1,4 @@
-"""parallax_b200 — a Blackwell-native sparsity-aware data-parallel training
+"""parallax_b200 — a Hopper-native sparsity-aware data-parallel training
 engine with the capabilities and API of snuspl/parallax.
 
 Public surface (parity with `parallax/parallax/__init__.py:16-26`):

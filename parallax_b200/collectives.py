@@ -62,8 +62,8 @@ class _State(object):
             self.oneshot_bytes = int(oneshot_bytes)
             self.stage = heap.alloc(2 * self.oneshot_bytes, "oneshot_stage")
             self.user_bufs = {}
-            # NVLS workspace: measured best from 256 KB up at >= 4 GPUs
-            # (profiles/allreduce_sweep_8gpu.json)
+            # NVLS workspace from 256 KB up at >= 4 GPUs (tools/allreduce_sweep.py measures
+            # the crossover)
             self.ws_mc = None
             self.nvls_min_bytes = 256 << 10
             if comm.world >= 4:
@@ -301,7 +301,7 @@ def _allreduce_cuda(x, out, scale):
 
 class Compression(object):
     """Gradient compression for all-reduce (`horovod/tensorflow/compression.py:46-64`:
-    ``Compression.none`` / ``Compression.fp16``).  bf16 is the Blackwell-native
+    ``Compression.none`` / ``Compression.fp16``).  bf16 is the Hopper-native
     16-bit wire format; fp16 is kept for parity."""
 
     class none(object):

@@ -103,6 +103,9 @@ REMOTE_PARALLAX_ROOT = os.path.join("/tmp", "parallax-%s" % _user())
 NUM_ITERATIONS_FOR_WARMUP = 50
 NUM_ITERATIONS_FOR_TEST = 100
 
+# streaming multiprocessors of the target GPU (H100 SXM); grid sizes of the native kernels
+NUM_SMS = 132
+
 RUN_OPTIONS = ("PS", "MPI", "HYBRID")
 # "AR" is accepted as a modern alias of the reference's "MPI" run option.
 RUN_OPTION_ALIASES = {"AR": "MPI", "ALLREDUCE": "MPI"}

@@ -6,7 +6,7 @@ with exported env), `mpi/runner.py:36-131` (mpirun, one process per GPU),
 redirect files ``log_worker<i>_{stdout,stderr}`` — `ps/runner.py:34-46`,
 SIGINT kills all process groups `:186-192`).
 
-B200 design: every run option uses the same shape — one worker process per
+Design: every run option uses the same shape — one worker process per
 GPU re-executing the user's script, rendezvousing through `torch.distributed`
 (MASTER_ADDR = first host).  There are no separate parameter-server
 processes: a variable's "server" is the GPU that owns it.  Local workers are

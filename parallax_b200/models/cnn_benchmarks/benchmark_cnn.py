@@ -54,7 +54,7 @@ _DEFAULT_PARAMS = collections.OrderedDict([
     ("rmsprop_epsilon", ParamSpec(float, 1.0, "RMSProp epsilon")),
     ("gradient_clip", ParamSpec(float, None, "clip gradients to [-x, x] element-wise")),
     ("weight_decay", ParamSpec(float, 0.00004, "L2 weight decay")),
-    ("use_fp16", ParamSpec(bool, False, "reduced-precision compute (bf16 on Blackwell)")),
+    ("use_fp16", ParamSpec(bool, False, "reduced-precision compute (bf16 on Hopper)")),
     ("fp16_loss_scale", ParamSpec(float, None, "loss scale (default 1: bf16 needs none)")),
     ("tf_random_seed", ParamSpec(int, 1234, "random seed")),
     ("num_batches_for_eval", ParamSpec(int, 0, "evaluation batches (0 = one epoch)")),

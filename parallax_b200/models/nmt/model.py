@@ -19,7 +19,7 @@ Parity (behaviour, not structure):
   layer_norm_lstm; dropout on every cell's input; residual wrappers on the
   top `num_*_residual_layers` layers.
 
-B200-first structure: there is no per-step cell graph.  Every layer is one
+GPU-first structure: there is no per-step cell graph.  Every layer is one
 cuDNN sequence call wherever the data dependence allows it — whole encoder
 stacks (packed by length), and in the GNMT decoder every layer above the
 attention layer (those depend on the *contexts*, which the bottom layer

@@ -1,12 +1,11 @@
-"""In-tree build of the native library (sm_100a only).
+"""In-tree build of the native library (sm_90a only).
 
     python -m parallax_b200.ops.build            # incremental
     python -m parallax_b200.ops.build --force
 
-Produces `parallax_b200/ops/libparallax_b200.so` (git-ignored, travels to the
-GPU box with the snapshot).  Every translation unit is compiled with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo``; there is no other
-target.  The reference's build (`horovod/setup.py`, TF bazel with
+Produces `parallax_b200/ops/libparallax_b200.so` (git-ignored).  Every
+translation unit is compiled with ``-gencode arch=compute_90a,code=sm_90a
+-lineinfo``; there is no other target.  The reference's build (`horovod/setup.py`, TF bazel with
 compute 3.5/7.0 — `tensorflow/configure.py:36-39`) has no counterpart here:
 one nvcc invocation per file, one link.
 """
@@ -22,7 +21,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libparallax_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
           "-Xcompiler", "-fvisibility=default", "--expt-relaxed-constexpr"]
 

@@ -88,7 +88,7 @@ px_allreduce_twoshot_kernel(PeerPtrs rot, uint32_t* const* pads, uint32_t* epoch
 // double-buffered shared-memory stage of W x PX_BULK_BYTES, the CTA sums the W tiles out of shared
 // memory in fp32 and stores the reduced tile into every peer (all-gather by store).  Same
 // barriers, same bytes over NVLink as `px_allreduce_twoshot_kernel`; only the load path differs
-// (TMA engine + SMEM instead of ld.global.v4 into registers).  Result in profiles/README.md.
+// (TMA engine + SMEM instead of ld.global.v4 into registers).
 #define PX_BULK_BYTES 8192
 __device__ __forceinline__ uint32_t cvta_smem(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);

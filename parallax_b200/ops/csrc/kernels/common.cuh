@@ -1,4 +1,4 @@
-// Shared device helpers for the parallax_b200 sm_100a kernels.
+// Shared device helpers for the parallax_b200 sm_90a kernels.
 //
 // Conventions
 //  * A "world" is up to PX_MAX_RANKS GPUs on one NVSwitch domain.  Peer
@@ -20,6 +20,7 @@
 #include <stdint.h>
 
 #define PX_MAX_RANKS 16
+#define PX_NUM_SMS 132            // H100 SXM: grid caps of the grid-stride kernels
 #define PX_MAX_BLOCKS 128          // max CTAs of a communicating kernel
 #define PX_NUM_CHANNELS 8          // independent barrier channels per pad
 

@@ -347,7 +347,7 @@ int px_dense_step(const void* const* grads, const void* const* params, float* ma
   const int threads = 512;
   // rank-level barriers: the grid is sized for HBM bandwidth, not by barrier slots
   size_t b = (n / world / vn + threads - 1) / threads;
-  const size_t cap = world == 1 ? 148 * 4 : (size_t)(max_blocks > 0 ? max_blocks : 148);
+  const size_t cap = world == 1 ? PX_NUM_SMS * 4 : (size_t)(max_blocks > 0 ? max_blocks : PX_NUM_SMS);
   int blocks = (int)(b < 1 ? 1 : (b > cap ? cap : b));
 #define LAUNCH(T, W)                                                                       \
   do {                                                                                     \
@@ -408,7 +408,7 @@ int px_dense_async(const void* my_grads, void* my_params, const void* const* mas
 
 int px_sumsq(const void* x, size_t n, int dtype, float mul, float* out, cudaStream_t stream) {
   const int vn = dtype == 0 ? 4 : 8;
-  const int blocks = px_clamp_blocks(n / vn, 512 * 4, 148 * 2);
+  const int blocks = px_clamp_blocks(n / vn, 512 * 4, PX_NUM_SMS * 2);
   if (dtype == 0) px_sumsq_kernel<float><<<blocks, 512, 0, stream>>>((const float*)x, n, mul, out);
   else px_sumsq_kernel<__nv_bfloat16><<<blocks, 512, 0, stream>>>((const __nv_bfloat16*)x, n, mul, out);
   return (int)cudaGetLastError();

@@ -64,7 +64,7 @@ px_lstm_cell_bwd_kernel(const T* __restrict__ dm, float* __restrict__ dc,
                         int interleaved) {
   const int total = B * S;
   // gate g of unit s lives at column g*S + s (plain) or, gate-interleaved in
-  // tiles of 32 units, at (s/32)*128 + g*32 + s%32 (layout of the tcgen05 path)
+  // tiles of 32 units, at (s/32)*128 + g*32 + s%32 (layout of the wgmma path)
   const int GS = interleaved ? 32 : S;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += gridDim.x * blockDim.x) {
@@ -250,7 +250,7 @@ extern "C" {
 int px_lstm_cell_fwd(const void* gates, const float* c_prev, void* act, float* c_new, void* m,
                      int B, int S, float forget_bias, int dtype, cudaStream_t stream) {
   int blocks = (B * S + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
   if (dtype == 0)
     px_lstm_cell_fwd_kernel<float><<<blocks, 256, 0, stream>>>(
         (const float*)gates, c_prev, (float*)act, c_new, (float*)m, B, S, forget_bias);
@@ -265,7 +265,7 @@ int px_lstm_cell_bwd(const void* dm, float* dc, const void* act, const float* c_
                      const float* c_new, void* dgates, int B, int S, int dtype, int interleaved,
                      cudaStream_t stream) {
   int blocks = (B * S + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
   if (dtype == 0)
     px_lstm_cell_bwd_kernel<float><<<blocks, 256, 0, stream>>>(
         (const float*)dm, dc, (const float*)act, c_prev, c_new, (float*)dgates, B, S,
@@ -327,7 +327,7 @@ int px_ssm_bwd(void* G, const void* inputs, const void* w_true, const float* g, 
   if (P % vec) return -2;
   const long long total = (long long)N * (P / vec);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
   if (dtype == 0)
     px_ssm_bwd_kernel<float><<<blocks, 256, 0, stream>>>(

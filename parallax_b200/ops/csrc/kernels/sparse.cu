@@ -909,7 +909,7 @@ int px_sparse_lookup(const void* ids, int ids_is64, int n, const PxLookupTable* 
   const int lpr = pick_lpr(maxv);
   const int threads = 256, rpb = threads / lpr;
   int blocks = (n + rpb - 1) / rpb;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
   const uint32_t* applied = reinterpret_cast<const uint32_t*>(hdr_mine) + PX_MAX_RANKS;
   if (ids_is64)
     px_sparse_lookup_kernel<long long><<<blocks, threads, 0, stream>>>(
@@ -1014,7 +1014,7 @@ int px_sparse_owner(const PxOwnerTable* tabs, int nt, int wire_dtype, const int3
   if (use_merge) {
     // one grid barrier inside: every CTA must be resident
     if (blocks > max_coop) blocks = max_coop;
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > PX_NUM_SMS * 4) blocks = PX_NUM_SMS * 4;
     e = cudaLaunchCooperativeKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
   } else {
     e = cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, 0, stream);

@@ -7,7 +7,7 @@
 // samples of bytes/µs — parameter_manager.cc:28-31,45-56,155-181,391-402,
 // 462-475) and horovod/common/optim/{bayesian_optimization,gaussian_process}.cc
 // (Eigen + L-BFGS there; a dense Cholesky and random-restart EI search here —
-// the problem is ≤ 4-D with ≤ 24 samples).  What is tuned on B200: comm-kernel
+// the problem is ≤ 4-D with ≤ 24 samples).  What is tuned: comm-kernel
 // CTA count, sparse-kernel CTA cap, bucket size, one-shot/two-shot threshold.
 #include <algorithm>
 #include <cmath>

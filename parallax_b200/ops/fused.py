@@ -69,11 +69,10 @@ _perm_cache = {}
 
 
 def _tc_forward_enabled():
-    """The fused tcgen05 forward step is opt-in (`PARALLAX_LSTM_TC_FWD=1`):
-    measured on B200 at the LM1B shape it is numerically equivalent but, with the
-    per-step weight re-layout it needs, slower than cuBLAS + the stand-alone cell
-    kernel (profiles/README.md); the tcgen05 split-K product on the backward path
-    is always on."""
+    """The fused wgmma forward step is opt-in (`PARALLAX_LSTM_TC_FWD=1`): it is
+    numerically equivalent but needs a per-step weight re-layout, and on one H100 (400 W
+    power limit) the LM1B bench step takes 1.64 ms with it against 1.42 ms without; the
+    wgmma split-K product on the backward path is always on."""
     import os
     return os.environ.get("PARALLAX_LSTM_TC_FWD", "0") == "1"
 
@@ -99,11 +98,9 @@ def _bwd_fused_w():
     ``dm_{t-1} = dH_{t-1} W_P^T + dgates_t Wc^T`` — ONE product per time step on the
     critical path instead of two (``dh = dH + dgates Wh^T`` then ``dm = dh W_P^T``); the
     per-step `dh` values (needed only for dW_P) are produced afterwards by one batched GEMM
-    off the critical path.  "tc": tcgen05 split-K kernel, "cublas": torch.addmm, "0": off.
-    Measured on B200 at the LM1B shape (tools/bench_lstm_gemms.py): the combined product
-    (128 x 2048 x 8192, 32 MB of weights per step from L2) costs 13.5 us (cuBLAS) / 16.2 us
-    (tcgen05 split-K) against 2.8 + 11.7 us for the two it replaces — no gain (1.46 / 1.52
-    vs 1.43 ms per training step), so it stays OFF by default."""
+    off the critical path.  "tc": wgmma split-K kernel, "cublas": torch.addmm, "0": off
+    (the default).  The combined product (128 x 2048 x 8192) reads 32 MB of weights per step
+    where the two it replaces read 10 MB; tools/bench_lstm_gemms.py times both."""
     import os
     return os.environ.get("PARALLAX_LSTM_BWD_FUSEDW", "0")
 
@@ -124,8 +121,8 @@ def _dbias_stream():
 def _wgrad_chunks(T):
     """How many pieces the weight-gradient GEMMs are cut into along time so that the
     earlier pieces run on the side stream underneath the (latency-bound) recurrent
-    backward chain.  Default 1 (all after the loop, still on the side stream): measured on
-    B200, 2 chunks cost 1.253 vs 1.239 ms/step — the big GEMMs slow the chain they overlap."""
+    backward chain.  Default 1 (all after the loop, still on the side stream): the big
+    GEMMs compete for SMs with the latency-bound chain they would overlap."""
     import os
     n = int(os.environ.get("PARALLAX_LSTM_WGRAD_CHUNKS", "1"))
     return max(1, min(n, T // 2 if T >= 4 else 1))
@@ -151,7 +148,7 @@ class _LSTMLayerFn(torch.autograd.Function):
             Wx, Wh = W.detach()[:E], W.detach()[E:]
         else:
             Wx = W
-        # tcgen05 path: recurrent GEMM with the LSTM cell fused into its epilogue
+        # wgmma path: recurrent GEMM with the LSTM cell fused into its epilogue
         # (gate-interleaved column layout, see gemm_tc.cu)
         tc = (dt == torch.bfloat16 and Bsz % 128 == 0 and P % 64 == 0 and S % 32 == 0 and
               _tc_forward_enabled())
@@ -244,12 +241,12 @@ class _LSTMLayerFn(torch.autograd.Function):
             WPT = W_P.t().contiguous()
         # dh_{t-1} = dH_{t-1} + dgates_t @ Wh^T : Wh [P, 4S] is already the
         # K-contiguous "B^T" operand, so this skinny product (M=B, N=P, K=4S)
-        # goes to our tcgen05 split-K kernel with the +dH addend fused in.
+        # goes to our wgmma split-K kernel with the +dH addend fused in.
         from . import gemm as _gemm
         use_tc = (dt == torch.bfloat16 and Bsz % 128 == 0 and P % 64 == 0 and
                   (4 * S) % 1024 == 0 and Wh.is_contiguous())
         # K-splits of the dh product: 8 CTAs per tile reducing through DSMEM in a cluster
-        # (8.7 us at the LM1B shape) or 16 through the L2 workspace (11.5 us)
+        # or 16 through the L2 workspace (LM1B bench step on one H100: 1.42 vs 1.45 ms)
         ksp = 8 if _gemm.cluster_default() else 16
         WhT = None if use_tc else Wh.t().contiguous()
         st = _stream()

@@ -1,8 +1,8 @@
-"""Python face of the tcgen05/TMEM/TMA GEMM (`csrc/kernels/gemm_tc.cu`).
+"""Python face of the wgmma/TMA GEMM (`csrc/kernels/gemm_tc.cu`).
 
 `gemm_tn(A, Bt, addend=None, splits=None)` computes ``A @ Bt.T (+ addend)`` in
 bf16 with fp32 accumulation, where both operands are K-contiguous
-(A: [M, K], Bt: [N, K]) — the layout tcgen05 consumes directly through
+(A: [M, K], Bt: [N, K]) — the layout wgmma consumes directly through
 128B-swizzled TMA tiles.  `splits` > 1 spreads the reduction over that many
 CTAs per output tile (skinny products: M = batch, K or N huge).
 """
@@ -10,6 +10,7 @@ import ctypes
 
 import torch
 
+from .. import consts
 from . import lib as _lib, check as _check, register_signatures
 
 _vp, _i = ctypes.c_void_p, ctypes.c_int
@@ -30,7 +31,7 @@ def _workspace(M, N, device):
     return w
 
 
-def pick_splits(M, N, K, bn=128, sms=148):
+def pick_splits(M, N, K, bn=128, sms=consts.NUM_SMS):
     """Enough K-splits to put ~one CTA on every SM, each split ≥ 256 deep."""
     tiles = (M // 128) * (N // bn)
     s = max(1, min(K // 256, sms // max(tiles, 1)))

@@ -8,7 +8,7 @@ variables, SparseApplyAdagrad / Scatter*) and runs TF's kernels
 `training_ops.cc:1276-1382`).  Here an optimizer is a *spec* (kind +
 hyper-parameters); the math is executed by
 
-* the fused sm_100a kernels (`ops/csrc/kernels/dense_step.cu`,
+* the fused sm_90a kernels (`ops/csrc/kernels/dense_step.cu`,
   `sparse_apply.cu`) on the NVLink fabric, or
 * the pure-torch fp32 functions in this file on the host fabric — which are
   also the numerics oracle for the kernel tests.
@@ -29,7 +29,7 @@ import math
 
 import torch
 
-# Every kind has a fused sm_100a rule (`ops/csrc/kernels/optim_rules.cuh`), split in two
+# Every kind has a fused sm_90a rule (`ops/csrc/kernels/optim_rules.cuh`), split in two
 # template families so the five hot rules keep their register budget: KINDS (family 0)
 # and EXT_KINDS (family 1: the rest of the reference's recognised update ops,
 # `graph_transform_lib.py:56-75` — ApplyAdadelta, ApplyFtrl, ApplyProximalGradientDescent,

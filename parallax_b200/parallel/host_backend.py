@@ -5,7 +5,7 @@ NCCL — the path for jobs that span several NVLink domains, where peer memory
 cannot be addressed).
 
 Purpose: (1) BASELINE config 1 — plumbing and dense/sparse routing tests with
-``world_size=2`` and no GPU; (2) the semantic oracle the sm_100a kernels are
+``world_size=2`` and no GPU; (2) the semantic oracle the sm_90a kernels are
 checked against.  It is *not* a second production path: on a GPU box the
 engine refuses to fall back to it unless explicitly asked (tests, baseline).
 

@@ -29,7 +29,7 @@ import math
 
 import torch
 
-from .. import optim as _optim
+from .. import consts, optim as _optim
 from ..log import parallax_log
 from . import modes
 from .layout import TableLayout
@@ -344,7 +344,7 @@ class NVSparseGroup(object):
         # kernels for the optimizer, but every byte that crosses GPUs goes through NCCL
         # collectives (Horovod's IndexedSlices path: all-gather of ids and rows)
         self.protocol = opts.get("_protocol", "nvlink")
-        self.max_blocks = int(opts.get("sparse_blocks", 148 * 2))
+        self.max_blocks = int(opts.get("sparse_blocks", consts.NUM_SMS * 2))
         self.early_push = bool(opts.get("sparse_early_push", True))
         hints = [t.capacity_hint for t in tables if t.capacity_hint]
         self.capacity_hint = max(hints) if hints else None
@@ -729,7 +729,8 @@ class NVSparseGroup(object):
         nt = len(self.tables)
         # 16 half-warps per CTA, one entry per half-warp: as many CTAs as fit on the device at once
         # (4 per SM at 64 registers; the merge variant is a cooperative launch)
-        blocks = max(1, min(max(self.max_blocks, 148 * 4) if self.max_blocks >= 148
+        blocks = max(1, min(max(self.max_blocks, consts.NUM_SMS * 4)
+                            if self.max_blocks >= consts.NUM_SMS
                             else self.max_blocks,
                             (n * (self.world if self.replicated else 1) + 15) // 16))
         use_merge = self.world > 1 or not self.local_aggregation

@@ -1,4 +1,4 @@
-"""NVLink fabric backend: the engine's production path on B200.
+"""NVLink fabric backend: the engine's production path on H100.
 
 Dense variables → `NVDenseGroup` (buckets in symmetric memory, fused
 reduce-scatter + optimizer + parameter all-gather kernel per bucket, launched
@@ -19,7 +19,7 @@ import math
 
 import torch
 
-from .. import optim as _optim
+from .. import consts, optim as _optim
 from ..log import parallax_log
 from ..ops import sinks as _sinks
 from . import modes, nvops
@@ -59,7 +59,7 @@ class NVFabric(object):
         # a second wave behind the first one's system-scope fence); an explicit comm_blocks
         # (tests simulating several ranks on one GPU need small grids) applies to it as well
         self.dense_blocks = int(self.options.get(
-            "dense_blocks", self.options.get("comm_blocks", 148)))
+            "dense_blocks", self.options.get("comm_blocks", consts.NUM_SMS)))
         if isinstance(ex, IpcExchange):
             self.heap.pads_dev()        # eager: no lazy H2D inside a step
         if comm.distributed:
@@ -155,10 +155,9 @@ class NVDenseGroup(object):
         heap = self.heap
         # NVLS: bucket buffers bound to an NVSwitch multicast object, the fused
         # kernel then reduces with multimem.ld_reduce and broadcasts parameters
-        # with multimem.st.  Measured (profiles/allreduce_sweep_8gpu.json): wins
-        # from 256 KB up at 8 GPUs, loses at 2.  "auto" enables it on the
-        # configuration it was validated and measured on (a full 8-GPU box; the
-        # end-to-end gain there is ~1 %); `dense_nvls=True` forces it for 4..7.
+        # with multimem.st.  It pays off on large buckets across many GPUs and not at
+        # 2 (tools/allreduce_sweep.py measures the crossover).  "auto" enables it on a
+        # full 8-GPU box; `dense_nvls=True` forces it for 4..7.
         want = self.options.get("dense_nvls", "auto")
         self.nvls = False
         if W > 1 and self.update == "sharded" and not self.pull_mirrors and want:

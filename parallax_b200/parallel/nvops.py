@@ -43,8 +43,8 @@ def allreduce_twoshot(heap, buf_cptrs, n, dtype, scale, channels, sumsq=None,
 
 def allreduce_twoshot_bulk(heap, buf_cptrs, n, dtype, scale, channels, max_blocks=128,
                            stream=None):
-    """TMA (cp.async.bulk) variant of the two-shot all-reduce — kept for the measurement in
-    profiles/README.md; the engine uses the ld.global / multimem kernels."""
+    """TMA (cp.async.bulk) variant of the two-shot all-reduce — kept for comparison
+    (tools/allreduce_sweep.py); the engine uses the ld.global / multimem kernels."""
     L = ops.lib()
     _count()
     ops.check(L.px_allreduce_twoshot_bulk(

@@ -10,7 +10,7 @@ Fixed relative to the reference (SURVEY §8.4): the `queue` shadowing bug
 (`partitions.py:69`) and float partitions from `/` under Python 3
 (`:105,112`).
 
-B200 meaning of P: a table with P partitions is split row-wise ("mod"
+Meaning of P here: a table with P partitions is split row-wise ("mod"
 strategy, `embedding_ops.py:151-153`: ``p = id % P, local = id // P``);
 partition p is owned by rank ``p % world``.  P therefore controls how rows
 interleave across owners and how many independent apply segments each owner

@@ -6,7 +6,7 @@ launches and exits, worker returns
 ``(sess, num_workers, worker_id, num_replicas_per_worker)``) and `:62-137`
 (`_parallax_run_master`: mode degeneration, partition-search loop, cleanup).
 
-Differences by design (B200-first):
+Differences by design (one process per GPU):
 * one worker process per GPU for every run option, so
   ``num_replicas_per_worker`` is always 1 (the reference returns the number of
   local GPUs in PS mode, `ps/runner.py:293-295`);

@@ -13,7 +13,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 

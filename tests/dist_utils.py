@@ -21,6 +21,9 @@ def _entry(rank, world, port, fn, args, outdir, env):
     os.environ.update({"RANK": str(rank), "WORLD_SIZE": str(world),
                        "LOCAL_RANK": str(rank), "MASTER_ADDR": "127.0.0.1",
                        "MASTER_PORT": str(port), "OMP_NUM_THREADS": "1"})
+    # the ranks are CPU processes on gloo: on a machine with fewer GPUs than ranks a visible
+    # GPU would make every rank pick NCCL on the same device
+    os.environ["CUDA_VISIBLE_DEVICES"] = ""
     os.environ.update(env or {})
     import torch
     torch.set_num_threads(1)

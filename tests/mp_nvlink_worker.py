@@ -187,7 +187,7 @@ def variable_rows(comm, check):
 
 
 def lm1b_flagship(comm, check):
-    """The flagship step on N ranks (the smoke() shape: tcgen05 recurrent product, fused LSTM
+    """The flagship step on N ranks (the smoke() shape: wgmma recurrent product, fused LSTM
     and loss-head nodes, co-lookup group, gradient sinks, CUDA graph, bf16): finite losses and
     bit-identical parameter replicas on every rank after 8 steps of different data per rank."""
     from parallax_b200.models.lm1b import LM1B, lm1b_graph

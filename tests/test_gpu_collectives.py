@@ -1,4 +1,4 @@
-"""sm_100a collective kernels vs plain PyTorch fp32 references.  A world of W
+"""sm_90a collective kernels vs plain PyTorch fp32 references.  A world of W
 ranks is simulated on one GPU (see tests/gpu_utils.py)."""
 import pytest
 import torch

@@ -36,8 +36,8 @@ def test_lstm_layer_matches_reference(dtype, tol):
 @pytest.mark.parametrize("tc_fwd", ["0", "1"])
 def test_lstm_layer_bf16_tcgen05_backward_path(tc_fwd, monkeypatch):
     """B=128, 4S multiple of 1024: the recurrent backward product runs on the
-    tcgen05 split-K kernel with the fused addend; with PARALLAX_LSTM_TC_FWD=1 the
-    forward step runs on the tcgen05 kernel with the LSTM cell fused in its
+    wgmma split-K kernel with the fused addend; with PARALLAX_LSTM_TC_FWD=1 the
+    forward step runs on the wgmma kernel with the LSTM cell fused in its
     epilogue (gate-interleaved layout)."""
     monkeypatch.setenv("PARALLAX_LSTM_TC_FWD", tc_fwd)
     from parallax_b200.ops.fused import lstm_layer, lstm_layer_reference

@@ -1,4 +1,4 @@
-"""tcgen05/TMEM/TMA GEMM vs a plain PyTorch fp32 reference."""
+"""wgmma/TMA GEMM vs a plain PyTorch fp32 reference."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""The example model families on the NVLink fabric (one B200): NMT (GNMT),
+"""The example model families on the NVLink fabric (one H100): NMT (GNMT),
 skip-thoughts and the CNN benchmark harness take training steps in bf16 and agree
 with the host-fabric oracle in fp32.  (Named to run after the kernel suites.)"""
 import numpy as np

@@ -1,4 +1,4 @@
-"""Time the tcgen05 GEMM against cuBLAS (torch.mm) on the LSTM's skinny shapes."""
+"""Time the wgmma GEMM against cuBLAS (torch.mm) on the LSTM's skinny shapes."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -21,7 +21,7 @@ def timeit(fn, n=40):
 
 shapes = [("dh_rec  dgates@Wh^T", 128, 512, 8192), ("proj    m@W_P", 128, 512, 2048),
           ("gates   h@Wh", 128, 8192, 512), ("dm      dh@W_P^T", 128, 2048, 512)]
-print("%-22s %6s %6s %6s | %9s | %s" % ("shape", "M", "N", "K", "cuBLAS us", "tcgen05 us (splits,bn)"))
+print("%-22s %6s %6s %6s | %9s | %s" % ("shape", "M", "N", "K", "cuBLAS us", "wgmma us (splits,bn)"))
 for name, M, N, K in shapes:
     A = torch.randn(M, K, device="cuda").bfloat16()
     Bt = torch.randn(N, K, device="cuda").bfloat16()

@@ -1,8 +1,8 @@
 """Device time of the per-time-step products of the LM1B LSTM backward chain, each captured
 in a CUDA graph of 40 back-to-back dependent launches (the regime of the real step):
-  A  today:   dm = dh @ W_P^T (cuBLAS)  then  dh' = dH + dgates @ Wh^T (tcgen05 split-K 16)
+  A  today:   dm = dh @ W_P^T (cuBLAS)  then  dh' = dH + dgates @ Wh^T (wgmma split-K 16)
   B  fused W: dm' = DMH + dgates @ (W_P Wh)^T   cuBLAS addmm
-  C  fused W: same product on the tcgen05 split-K kernel (several tilings)
+  C  fused W: same product on the wgmma split-K kernel (several tilings)
 Usage: python tools/bench_lstm_gemms.py"""
 import os
 import sys

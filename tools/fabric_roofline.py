@@ -5,8 +5,8 @@ stream, max over ranks; the push / owner kernels also stamp %globaltimer themsel
   python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 \
       --master-port 29541 tools/fabric_roofline.py --out gpurun_out/fabric_roofline_8.json
 
-Roofline (B200_PROFILING.md): bytes that must cross NVLink per GPU and direction / 770 GB/s
-(measured peer copy), or the HBM side (bytes / measured copy bandwidth) when that is slower.
+Roofline: bytes that must cross NVLink per GPU and direction / NVLink bandwidth, or the HBM side
+(bytes / HBM bandwidth) when that is slower.
 Paths: fused dense step (reduce-scatter by load + optimizer + all-gather by store; P2P and
 NVLS), remote-gather lookup, push (all-to-all of bf16 rows + ids), owner (HBM-bound)."""
 import argparse
@@ -31,7 +31,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--out", default=None)
 ap.add_argument("--iters", type=int, default=30)
 args = ap.parse_args()
-NVLINK, HBM = 770.0, 6585.4
+NVLINK, HBM = 450.0, 3350.0      # H100 SXM data sheet, GB/s: NVLink 4 per direction, HBM3
 try:
     HBM = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:

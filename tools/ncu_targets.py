@@ -20,7 +20,7 @@ from tests.gpu_utils import make_world
 torch.manual_seed(0)
 dev = "cuda"
 REP = 2
-# ---- tcgen05 split-K GEMM at the LSTM backward shape --------------------------
+# ---- wgmma split-K GEMM at the LSTM backward shape ----------------------------
 A = torch.randn(128, 8192, device=dev).bfloat16()
 Bt = torch.randn(512, 8192, device=dev).bfloat16()
 D = torch.randn(128, 512, device=dev).bfloat16()

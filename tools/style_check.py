@@ -1,7 +1,7 @@
 """Source hygiene check (the reference's `tools/style_check.py:20-27` runs
 pycodestyle): byte-compile every Python file, flag tabs / trailing whitespace /
 lines over 100 columns in the package, and make sure no CUDA source targets an
-architecture other than sm_100a."""
+architecture other than sm_90a."""
 import os
 import py_compile
 import re
@@ -34,8 +34,8 @@ for top in ("parallax_b200", "parallax", "tests", "tools", "examples", "baseline
                 for m in re.findall(r"sm_(\d+)a?", txt):
                     if m not in ("100",) and "sm_%s" % m not in ("sm_90", "sm_103"):
                         pass
-                if re.search(r"wgmma|__CUDA_ARCH__\s*[<=>]+\s*[1-9]\d{2}\b(?!0)", txt):
-                    print("ARCH  %s: non-sm_100a construct" % p)
+                if re.search(r"tcgen05|cta_group::|sm_100|compute_100", txt):
+                    print("ARCH  %s: non-sm_90a construct" % p)
                     bad += 1
 print("style check: %d issue(s)" % bad)
 sys.exit(1 if bad else 0)
