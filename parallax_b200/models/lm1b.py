@@ -193,11 +193,8 @@ class LM1B(nn.Module):
                                     row_w=row_w, adj=adj)
 
     def full_softmax_loss(self, inputs, targets):
-        ids = torch.arange(self.vocab_size, device=inputs.device)
-        w, b = pnn.lookup_many([self.softmax_w, self.softmax_b], ids)
-        w, b = w.to(inputs.dtype), b.squeeze(-1).float()
-        logits = (inputs @ w.t()).float() + b
-        return F.cross_entropy(logits, targets, reduction="none")
+        """per-row full-softmax NLL of `inputs` [T*B, P] (`parallax.nn.full_softmax_nll`)."""
+        return pnn.full_softmax_nll(inputs, targets, self.softmax_w, self.softmax_b)
 
 
 def lm1b_graph(model, batch_size=128, learning_rate=0.2, max_grad_norm=10.0):

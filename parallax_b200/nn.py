@@ -124,3 +124,33 @@ def lookup_many(modules, ids, defer=False):
     early (e.g. on a side stream) and call ``.rows()`` where the rows are consumed."""
     from .parallel.engine import lookup_many as _lm
     return _lm(list(modules), ids, defer=defer)
+
+
+def full_softmax_nll(inputs, targets, weight, bias):
+    """Full-softmax cross entropy of every row of `inputs` against every row of a partitioned
+    output table: per-row NLL ``[N]`` fp32, i.e. ``reduction="none"`` of ::
+
+        cross_entropy(inputs @ weight.weight.T + bias.weight.T, targets)
+
+    `inputs` is ``[N, K]``, `targets` ``[N]`` integer ids, `weight` / `bias` are the two
+    embedding modules (``[V, K]`` and ``[V, 1]``) — the arguments `lookup_many` takes.  When
+    they form a co-lookup group on the NVLink fabric with a bf16 weight shadow, inputs are bf16
+    with K % 8 == 0 and K <= 512, and no gradient is wanted, one fused kernel evaluates the
+    softmax where the rows live (no gathered table, no [N, V] logits, fp32 logits; a target
+    outside [0, V) gives NaN in its row).  Otherwise the table is gathered and the logits
+    materialised, which also carries gradients to the tables."""
+    if inputs.dim() != 2:
+        raise ValueError("inputs must be [N, K], got shape %s" % (tuple(inputs.shape),))
+    if targets.dim() != 1 or targets.shape[0] != inputs.shape[0]:
+        raise ValueError("targets must be [N] = [%d], got shape %s"
+                         % (inputs.shape[0], tuple(targets.shape)))
+    if targets.dtype.is_floating_point or targets.dtype == torch.bool:
+        raise ValueError("targets must be integer ids, got %s" % targets.dtype)
+    if weight.embedding_dim != inputs.shape[1]:
+        raise ValueError("weight rows have %d columns, inputs have %d"
+                         % (weight.embedding_dim, inputs.shape[1]))
+    if bias.embedding_dim != 1 or bias.num_embeddings != weight.num_embeddings:
+        raise ValueError("bias must be a [%d, 1] embedding, got [%d, %d]"
+                         % (weight.num_embeddings, bias.num_embeddings, bias.embedding_dim))
+    from .parallel.engine import full_softmax_nll as _fs
+    return _fs(inputs, targets, weight, bias)

@@ -87,6 +87,10 @@ _SIGS = {
     "px_sparse_lookup": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(PxLookupTable),
                                  c_int, c_void_p, ctypes.POINTER(PxGroupGeom), c_void_p,
                                  c_void_p, c_int, c_void_p]),
+    "px_full_softmax_nll": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                    c_void_p, c_int, ctypes.POINTER(PxGroupGeom), c_int,
+                                    c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p]),
     "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PxPushTable), c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_int,
                                ctypes.POINTER(PxGroupGeom), c_void_p, c_int, c_int, c_int,

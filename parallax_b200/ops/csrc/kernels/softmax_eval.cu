@@ -1,0 +1,301 @@
+// Full-softmax cross entropy over a partitioned (weight, bias) co-lookup group, evaluated where
+// the rows live — no gather of the table, no [N, V] logits buffer, fp32 logits:
+//
+//   nll[i] = logsumexp_v(x_i · w_v + b_v) − (x_i · w_t + b_t),   t = targets[i]
+//
+//   px_full_softmax_lse_kernel      wgmma GEMM with a log-sum-exp epilogue.  Work items are
+//                                   blocks of BV local rows of one owner, walked in owner order
+//                                   rotated by rank; a CTA loads its block (bf16 shadow rows,
+//                                   K-major, 128B swizzle) into shared memory once and streams
+//                                   every 128-row tile of X through a TMA ring over it, so each
+//                                   table byte is read once per call.  The epilogue adds the fp32
+//                                   bias, masks padding rows with −inf and merges the block's
+//                                   per-row (max, Σexp) into the CTA's slice of a [grid, N]
+//                                   workspace (only that CTA touches it: no atomics).
+//   px_full_softmax_combine_kernel  one row per warp: merge the grid's (max, Σexp) pairs and
+//                                   subtract the target logit, whose rows come from the group's
+//                                   lookup kernel.
+//
+// One-sided like the lookup: peers' rows are read over NVLink with 16-byte loads; nothing is
+// exchanged, so a rank may evaluate alone.  In sync mode the kernel first waits applied[o] >=
+// completed steps on the group header (the lookup's freshness rule).
+#include "common.cuh"
+#include "sparse_group.cuh"
+#include "wgmma.cuh"
+
+namespace tc {
+
+constexpr int EV_BV = 128;          // table rows per work item = wgmma N
+constexpr int EV_STAGES = 4;        // X ring depth (16 KB per stage)
+constexpr int EV_KMAX = 512;
+constexpr float EV_LOG2E = 1.4426950408889634f;
+
+struct EvalArgs {
+  const __nv_bfloat16* const* w;    // [W] bf16 shadow rows of the weight table on every rank
+  const float* const* b;            // [W] fp32 master rows of the bias table on every rank
+  const int* row_cnt;               // [owners][slots] real rows of the partition in each slot
+  const uint32_t* applied;          // this rank's group header: applied[W]
+  const SparseCtl* ctl;
+  float2* ws;                       // [grid][N] running (max, Σexp) per (CTA, row)
+  int N, K, kb;                     // kb = ceil(K / 64) K-blocks of 64 columns
+  int w_pitch, b_pitch;             // row pitch (elements) of the shadow / bias rows
+  int W, rank, replicated, owners, slots, rows_per_part, nblk;
+  int wait;
+};
+
+// (m, s) ⊕ (m2, s2) for s = Σ exp(l − m); s == 0 marks an empty pair (m = −inf)
+__device__ __forceinline__ void lse_merge(float2& c, float m2, float s2) {
+  if (s2 == 0.f) return;
+  if (c.y == 0.f) { c = make_float2(m2, s2); return; }
+  const float mx = fmaxf(c.x, m2);
+  c.y = c.y * exp2f((c.x - mx) * EV_LOG2E) + s2 * exp2f((m2 - mx) * EV_LOG2E);
+  c.x = mx;
+}
+
+__device__ __forceinline__ bool ev_row_real(const EvalArgs& a, const int* cnt, int lr) {
+  return lr < a.slots * a.rows_per_part &&
+         (lr % a.rows_per_part) < __ldg(cnt + lr / a.rows_per_part);
+}
+
+// Roles as in gemm_tc.cu: warpgroup 0 produces (thread 0 issues the X TMA loads), warpgroups
+// 1 and 2 each own 64 rows of the 128-row X tile and run wgmma m64×BV×16 against the resident
+// table block.  All 384 threads load the table block between work items.
+__global__ void __launch_bounds__(THREADS, 1)
+px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs a) {
+  constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* sB = smem;                                        // [kb][BV rows][128 B]
+  uint8_t* sX = smem + a.kb * BV * 128;                      // [STAGES][128 rows][128 B]
+  float* s_bias = reinterpret_cast<float*>(sX + EV_STAGES * X_BYTES);   // [BV], −inf = padding
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + BV);
+  uint64_t* empty_bar = full_bar + EV_STAGES;
+
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
+    for (int s = 0; s < EV_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (a.wait && threadIdx.x < a.W) {
+    const uint32_t need = a.ctl->step;
+    while ((int32_t)(ld_acquire_sys(a.applied + threadIdx.x) - need) < 0) { }
+  }
+  __syncthreads();
+
+  const int wg = threadIdx.x >> 7;
+  const int items = a.owners * a.nblk;
+  const int m_tiles = (a.N + BM - 1) / BM;
+  const int cpr = a.kb * 8;                     // 16-byte chunks per table row in shared memory
+  const int kc = a.K / 8;                       // ... of which real
+  uint32_t it = 0;                              // X stages so far: ring slot and parity
+  bool first = true;
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int oi = item / a.nblk;
+    const int owner = a.replicated ? a.rank : (a.rank + oi) % a.W;
+    const int* cnt = a.row_cnt + (a.replicated ? 0 : owner) * a.slots;
+    const int r0 = (item % a.nblk) * BV;
+    const __nv_bfloat16* src = a.w[owner];
+    __syncthreads();                            // every wgmma on the previous block has retired
+    // table block -> shared memory, 128B-swizzled K-major (chunk c of row r at c ^ (r % 8));
+    // padding rows and columns beyond K are zero.  Eight loads in flight per thread.
+    const int total = BV * cpr;
+    for (int base = threadIdx.x; base < total; base += 8 * THREADS) {
+      uint4 v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * THREADS;
+        const int r = idx / cpr, c = idx % cpr;
+        v[u] = make_uint4(0, 0, 0, 0);
+        if (idx < total && c < kc && ev_row_real(a, cnt, r0 + r))
+          v[u] = ld_v4(src + (size_t)(r0 + r) * a.w_pitch + c * 8);
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int idx = base + u * THREADS;
+        if (idx >= total) break;
+        const int r = idx / cpr, c = idx % cpr;
+        *reinterpret_cast<uint4*>(sB + (c >> 3) * (BV * 128) + r * 128 +
+                                  (((c & 7) ^ (r & 7)) << 4)) = v[u];
+      }
+    }
+    if (threadIdx.x < BV) {
+      const int lr = r0 + threadIdx.x;
+      float bv = -INFINITY;
+      if (ev_row_real(a, cnt, lr))
+        bv = __uint_as_float(ld_v4(a.b[owner] + (size_t)lr * a.b_pitch).x);
+      s_bias[threadIdx.x] = bv;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // st.shared -> wgmma reads
+    __syncthreads();
+
+    if (wg == 0) {
+      if (threadIdx.x == 0) {
+        for (int mt = 0; mt < m_tiles; ++mt)
+          for (int kb = 0; kb < a.kb; ++kb, ++it) {
+            const int s = it % EV_STAGES;
+            mbar_wait(&empty_bar[s], ((it / EV_STAGES) & 1) ^ 1);
+            mbar_expect_tx(&full_bar[s], X_BYTES);
+            tma_load_2d(sX + s * X_BYTES, &tmap_x, &full_bar[s], kb * BK, mt * BM);
+          }
+      }
+    } else {
+      const int cw = wg - 1;
+      const bool leader = (threadIdx.x & 127) == 0;
+      const int lane = threadIdx.x & 31;
+      const int cq = (lane & 3) * 2;
+      for (int mt = 0; mt < m_tiles; ++mt) {
+        float acc[BV / 2];
+        for (int kb = 0; kb < a.kb; ++kb, ++it) {
+          const int s = it % EV_STAGES;
+          mbar_wait(&full_bar[s], (it / EV_STAGES) & 1);
+          const uint64_t adesc = make_smem_desc(smem_u32(sX + s * X_BYTES + cw * 64 * BK * 2));
+          const uint64_t bdesc = make_smem_desc(smem_u32(sB + kb * BV * 128));
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / WG_K; ++k)
+            wgmma_bf16<BV>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2),
+                           (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kb > 0 && leader) mbar_arrive(&empty_bar[(it - 1) % EV_STAGES]);
+        }
+        wgmma_wait<0>();
+        if (leader) mbar_arrive(&empty_bar[(it - 1) % EV_STAGES]);
+        // epilogue: a quad of lanes holds all BV columns of 2 rows (acc[j·4 + 2h + e] is row
+        // lane/4 + 8h, column j·8 + (lane%4)·2 + e of the warp's 16 rows)
+        const int rbase = mt * BM + cw * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float mx = -INFINITY;
+#pragma unroll
+          for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float& v = acc[j * 4 + 2 * h + e];
+              v += s_bias[j * 8 + cq + e];
+              mx = fmaxf(mx, v);
+            }
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          float sum = 0.f;
+          if (mx != -INFINITY) {
+            const float ms = mx * EV_LOG2E;
+#pragma unroll
+            for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                sum += exp2f(fmaf(acc[j * 4 + 2 * h + e], EV_LOG2E, -ms));
+          }
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          const int row = rbase + 8 * h;
+          if ((lane & 3) == 0 && row < a.N) {
+            float2* p = a.ws + (size_t)blockIdx.x * a.N + row;
+            float2 c = first ? make_float2(-INFINITY, 0.f) : *p;
+            lse_merge(c, mx, sum);
+            *p = c;
+          }
+        }
+      }
+    }
+    first = false;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, int K,
+                               const __nv_bfloat16* __restrict__ X,
+                               const __nv_bfloat16* __restrict__ wt, int wt_pitch,
+                               const float* __restrict__ bt, int bt_pitch,
+                               const long long* __restrict__ targets, int V,
+                               float* __restrict__ nll) {
+  const int lane = threadIdx.x & 31;
+  for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
+    float2 c = make_float2(-INFINITY, 0.f);
+    for (int g = lane; g < grid; g += 32) {
+      const float2 p = ws[(size_t)g * N + row];
+      lse_merge(c, p.x, p.y);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, c.x, o);
+      const float s2 = __shfl_xor_sync(0xffffffffu, c.y, o);
+      lse_merge(c, m2, s2);
+    }
+    float d = 0.f;
+    for (int ch = lane; ch < K / 8; ch += 32) {
+      float xf[8], wf[8];
+      Vec16<__nv_bfloat16>::unpack(*reinterpret_cast<const uint4*>(X + (size_t)row * K + ch * 8), xf);
+      Vec16<__nv_bfloat16>::unpack(
+          *reinterpret_cast<const uint4*>(wt + (size_t)row * wt_pitch + ch * 8), wf);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) d = fmaf(xf[e], wf[e], d);
+    }
+    d = warp_sum(d);
+    if (lane == 0) {
+      const long long t = targets[row];
+      nll[row] = (t >= 0 && t < V) ? c.x + logf(c.y) - (d + bt[(size_t)row * bt_pitch])
+                                   : __int_as_float(0x7fc00000);
+    }
+  }
+}
+
+constexpr int ev_smem_bytes(int kb) {
+  return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8;
+}
+
+}  // namespace tc
+
+extern "C" {
+
+// nll[N] (fp32) of X [N, K] (bf16, K-contiguous) against a (weight, bias) co-lookup group.
+//   w_ptrs / b_ptrs: device arrays of every rank's weight shadow (bf16, row pitch w_pitch) and
+//                    bias master rows (fp32, row pitch b_pitch, a multiple of 4);
+//   row_cnt:         [owners][slots] real rows of the partition stored in each slot (owners = 1
+//                    for a replicated layout, else W);
+//   ws:              fp32 [ws_ctas][N][2] scratch, the grid is at most ws_ctas CTAs;
+//   targets:         int64 [N]; wt / bt: the targets' rows from the group lookup (same pitches).
+// Returns 0, a negative argument error, or a CUDA error code.
+int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                        const void* b_ptrs, int b_pitch, const int* row_cnt, int slots,
+                        const PxGroupGeom* g, int rank, const void* hdr_mine, const void* ctl,
+                        int wait, void* ws, int ws_ctas, const long long* targets, const void* wt,
+                        const float* bt, float* nll, cudaStream_t stream) {
+  using namespace tc;
+  if (N <= 0) return 0;
+  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % 4) return -1;
+  if (ws_ctas < 1 || slots < 1) return -2;
+  const GroupGeom G = to_geom(g);
+  EvalArgs a;
+  a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const float* const*)b_ptrs;
+  a.row_cnt = row_cnt;
+  a.applied = reinterpret_cast<const uint32_t*>(hdr_mine) + PX_MAX_RANKS;
+  a.ctl = (const SparseCtl*)ctl; a.ws = (float2*)ws;
+  a.N = N; a.K = K; a.kb = (K + BK - 1) / BK;
+  a.w_pitch = w_pitch; a.b_pitch = b_pitch;
+  a.W = G.W; a.rank = rank; a.replicated = G.replicated; a.owners = G.replicated ? 1 : G.W;
+  a.slots = slots; a.rows_per_part = G.rows_per_part;
+  a.nblk = (slots * G.rows_per_part + EV_BV - 1) / EV_BV;
+  a.wait = wait;
+  const int items = a.owners * a.nblk;
+  const int grid = items < ws_ctas ? items : ws_ctas;
+  CUtensorMap tx;
+  int rc = make_tmap(&tx, X, N, K, BM);
+  if (rc) return rc;
+  constexpr int SMEM_MAX = ev_smem_bytes(EV_KMAX / BK);
+  static bool set = false;
+  if (!set) {
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         SMEM_MAX);
+    set = true;
+  }
+  px_full_softmax_lse_kernel<<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
+  int blocks = (N + 7) / 8;
+  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
+  px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
+      (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt, w_pitch,
+      bt, b_pitch, targets, G.V, nll);
+  return (int)cudaGetLastError();
+}
+
+}  // extern "C"

@@ -35,34 +35,7 @@
 #include "common.cuh"
 #include "launch.h"
 #include "optim_rules.cuh"
-
-#define PX_GRP_MAX 4            // member tables per group
-
-struct GroupGeom {
-  int V, P, W, rows_per_part;
-  int strategy;                 // 0 mod, 1 div
-  int replicated;               // 1: every rank holds the full table (AR mode)
-  int extras, base;             // div strategy
-  const int* part_owner;        // [P] owner rank of partition p (byte-greedy placement)
-  const int* part_slot;         // [P] index of partition p among its owner's partitions
-};
-
-// per-rank control block of a group (local memory)
-struct SparseCtl {
-  uint32_t step;                // completed steps
-  uint32_t push_done;           // CTA ticket counter (push kernel)
-  uint32_t apply_done;          // CTA ticket counter (owner kernel)
-  uint32_t bar;                 // grid barrier arrivals (owner kernel)
-  int32_t n_dup;                // staging rows handed out this step
-  int32_t overflow;             // #positions that fell back to un-deduplicated entries (stat)
-  int32_t owner_cnt[PX_MAX_RANKS];
-  unsigned long long t_push[2]; // %globaltimer at push start / flag publication
-  unsigned long long t_own[3];  // owner kernel: start / all sources arrived / applied published
-  unsigned long long t_dbg[8];  // push kernel, CTA 0: end of each internal phase (profiling aid)
-};
-
-// group header (symmetric): [pushed[R] | applied[R] | cnt[R]]
-#define PX_GRP_HDR_WORDS (3 * PX_MAX_RANKS)
+#include "sparse_group.cuh"
 
 __device__ __forceinline__ unsigned long long px_globaltimer() {
   unsigned long long t;
@@ -859,16 +832,6 @@ static void launch_push(int blocks, size_t smem, cudaStream_t stream, const int3
 }
 
 extern "C" {
-
-struct PxGroupGeom {
-  int V, P, W, rows_per_part, strategy, replicated, extras, base;
-  const int* part_owner; const int* part_slot;
-};
-static inline GroupGeom to_geom(const PxGroupGeom* g) {
-  GroupGeom t; t.V = g->V; t.P = g->P; t.W = g->W; t.rows_per_part = g->rows_per_part;
-  t.strategy = g->strategy; t.replicated = g->replicated; t.extras = g->extras; t.base = g->base;
-  t.part_owner = g->part_owner; t.part_slot = g->part_slot; return t;
-}
 
 // C mirrors of the per-table descriptors (plain pointers / ints, filled from Python)
 struct PxLookupTable { const void* srcs; void* out; int D4, src_bf16, out_bf16, pad; };

@@ -123,6 +123,35 @@ def lookup_many(modules, ids, defer=False):
     return PendingLookup(outs) if defer else outs
 
 
+def full_softmax_nll(inputs, targets, weight, bias):
+    """Per-row ``cross_entropy(inputs @ W.T + b, targets, reduction="none")`` over every row
+    of the (weight, bias) embedding modules.  When the modules form a co-lookup group on the
+    NVLink fabric (protocol nvlink) whose weight table keeps a bf16 shadow, `inputs` is bf16
+    with K % 8 == 0 and K <= 512, and no gradient is wanted, the group's fused kernel computes
+    it where the rows live; everything else runs the gather + matmul + cross_entropy
+    composition (which also gives the tables their gradients in training)."""
+    tabs = [getattr(m, "table", None) for m in (weight, bias)]
+    grp = getattr(tabs[0], "group", None) if tabs[0] is not None else None
+    K = int(inputs.shape[-1])
+    if grp is not None and list(grp.tables) == tabs and grp.protocol == "nvlink" and \
+            tabs[0].use_shadow and inputs.dtype == torch.bfloat16 and \
+            inputs.device == grp.device and K % 8 == 0 and K <= 512 and \
+            (not torch.is_grad_enabled() or not (inputs.requires_grad or
+                                                 weight._anchor.requires_grad or
+                                                 bias._anchor.requires_grad)):
+        return grp.full_softmax_nll(inputs, targets)
+    return full_softmax_composition(inputs, targets, weight, bias)
+
+
+def full_softmax_composition(inputs, targets, weight, bias):
+    """The unfused full softmax: gather every row, materialise the [N, V] logits."""
+    ids = torch.arange(weight.num_embeddings, device=inputs.device)
+    w, b = lookup_many([weight, bias], ids)
+    w, b = w.to(inputs.dtype), b.squeeze(-1).float()
+    logits = (inputs @ w.t()).float() + b
+    return torch.nn.functional.cross_entropy(logits, targets, reduction="none")
+
+
 class ShardedEmbedding(tnn.Module):
     """Drop-in replacement for ``nn.Embedding(sparse=True)`` whose storage is
     a partitioned table on the fabric."""

@@ -378,6 +378,7 @@ class NVSparseGroup(object):
         self._cur_step = 0
         self._done_step = -1
         self._last_n = 1
+        self._row_cnt = None
         NVSparseGroup._seq += 1
 
     # ---------------------------------------------------------------- forward
@@ -507,6 +508,68 @@ class NVSparseGroup(object):
                 1 if (self.route.sync and self.world > 1 and not self._nccl()) else 0,
                 _sp(torch.cuda.current_stream(self.device))), "sparse_lookup")
         return outs, pend
+
+    # ------------------------------------------------------------- evaluation
+    def _row_counts(self):
+        """int32 [owners, slots] on the device: real rows of the partition held in each
+        (owner, slot) of the layout (the rest of a slot is padding).  Built once per layout."""
+        lay = self.layout
+        if self._row_cnt is None or self._row_cnt[0] is not lay:
+            cnt = torch.zeros(1 if lay.replicated else lay.world, lay.parts_per_owner,
+                              dtype=torch.int32)
+            for p in range(lay.P):
+                cnt[0 if lay.replicated else lay.owners[p], lay.slots[p]] = lay.partition_rows(p)
+            self._row_cnt = (lay, cnt.to(self.device))
+        return self._row_cnt[1]
+
+    def full_softmax_nll(self, x, targets):
+        """Per-row full-softmax NLL, fp32 [N], of bf16 inputs `x` [N, K] against this
+        group's (weight, bias) tables: ``cross_entropy(x @ W.T + b, targets)`` with fp32
+        logits, computed from the rows where their owners store them — no gather of the
+        table and no [N, V] logits (`ops/csrc/kernels/softmax_eval.cu`).  The targets' rows
+        come from one launch of the group's lookup kernel.  A target outside [0, V) gives
+        NaN in its row.  One-sided: no other rank takes part."""
+        from .. import ops
+        L = _lib()
+        tw, tb = self.tables
+        n, K = int(x.shape[0]), int(x.shape[1])
+        if not tw.use_shadow or tb.D != 1 or K != tw.D or x.dtype != torch.bfloat16:
+            raise ValueError("full_softmax_nll needs bf16 inputs [N, %d], a weight table with "
+                             "a bf16 shadow and a bias table of width 1" % tw.D)
+        out = torch.empty(n, dtype=torch.float32, device=self.device)
+        if n == 0:
+            return out
+        x = x.contiguous()
+        if x.data_ptr() % 16:                      # TMA needs a 16-byte aligned base
+            x = x.clone()
+        ids = targets.reshape(-1).to(self.device, torch.int64).contiguous()
+        wait = 1 if (self.route.sync and self.world > 1 and not self._nccl()) else 0
+        stream = _sp(torch.cuda.current_stream(self.device))
+        w_t = torch.empty((n, tw.Dps), dtype=torch.bfloat16, device=self.device)
+        b_t = torch.empty((n, tb.Dp), dtype=torch.float32, device=self.device)
+        descs = (ops.PxLookupTable * 2)()
+        descs[0].srcs, descs[0].out, descs[0].D4 = \
+            tw.dev_ptrs("shadow").data_ptr(), w_t.data_ptr(), tw.D4
+        descs[0].src_bf16, descs[0].out_bf16 = 1, 1
+        descs[1].srcs, descs[1].out, descs[1].D4 = \
+            tb.dev_ptrs("table").data_ptr(), b_t.data_ptr(), tb.D4
+        descs[1].src_bf16, descs[1].out_bf16 = 0, 0
+        _count()
+        ops.check(L.px_sparse_lookup(
+            _vp(ids.data_ptr()), 1, n, descs, 2, _vp(0), ctypes.byref(self.geom),
+            _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), wait, stream),
+            "sparse_lookup(full softmax targets)")
+        cnt = self._row_counts()
+        ws = torch.empty(consts.NUM_SMS * n * 2, dtype=torch.float32, device=self.device)
+        _count(2)
+        ops.check(L.px_full_softmax_nll(
+            _vp(x.data_ptr()), n, K, _vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps,
+            _vp(tb.dev_ptrs("table").data_ptr()), tb.Dp, _vp(cnt.data_ptr()),
+            int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
+            _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), wait, _vp(ws.data_ptr()),
+            consts.NUM_SMS, _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
+            _vp(out.data_ptr()), stream), "full_softmax_nll")
+        return out
 
     def add_pending(self, token, grads):
         gs = []
