@@ -11,35 +11,37 @@ import os
 from .build import LIB, build as _build, nvcc as _nvcc
 
 _lib = None
+_abi = None
 
 c_void_p, c_int, c_size_t, c_float = \
     ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_float
 PP = ctypes.POINTER(ctypes.c_void_p)
 
 
-class PxGroupGeom(ctypes.Structure):
+# ctypes mirrors of the sparse-group descriptors, named like their C structs (sparse_group.cuh,
+# sparse.cu); `lib()` checks their layout against the library's `px_sparse_abi()`.
+class GroupGeom(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ("V", "P", "W", "rows_per_part", "strategy",
                                      "replicated", "extras", "base")] + \
         [("part_owner", c_void_p), ("part_slot", c_void_p)]
 
 
-class PxLookupTable(ctypes.Structure):
+class LookupTable(ctypes.Structure):
     _fields_ = [("srcs", c_void_p), ("out", c_void_p), ("D4", c_int),
-                ("src_bf16", c_int), ("out_bf16", c_int), ("pad", c_int)]
+                ("src_bf16", c_int), ("out_bf16", c_int)]
 
 
-class PxPushTable(ctypes.Structure):
+class PushTable(ctypes.Structure):
     _fields_ = [("grads", c_void_p), ("staging", c_void_p), ("rings", c_void_p),
                 ("tables", c_void_p), ("slot0s", c_void_p), ("slot1s", c_void_p),
                 ("slot2s", c_void_p), ("shadows", c_void_p), ("hp", c_void_p),
-                ("D4", c_int), ("kind", c_int), ("scale", c_float), ("pad", c_int)]
+                ("D4", c_int), ("kind", c_int), ("scale", c_float)]
 
 
-class PxOwnerTable(ctypes.Structure):
+class OwnerTable(ctypes.Structure):
     _fields_ = [("ring", c_void_p), ("table", c_void_p), ("slot0", c_void_p),
                 ("slot1", c_void_p), ("slot2", c_void_p), ("shadow", c_void_p),
-                ("hp", c_void_p), ("D4", c_int), ("kind", c_int), ("avg", c_float),
-                ("pad", c_int)]
+                ("hp", c_void_p), ("D4", c_int), ("kind", c_int), ("avg", c_float)]
 
 
 _SIGS = {
@@ -79,25 +81,20 @@ _SIGS = {
                                c_size_t, c_int, c_int, c_int, c_int, c_int,
                                c_void_p]),
     "px_sumsq": (c_int, [c_void_p, c_size_t, c_int, c_float, c_void_p, c_void_p]),
-    "px_sparse_ctl_bytes": (c_size_t, []),
-    "px_sparse_hdr_words": (c_int, []),
-    "px_sparse_group_max": (c_int, []),
-    "px_sparse_ctl_time_offset": (c_int, []),
-    "px_sparse_ctl_overflow_offset": (c_int, []),
-    "px_sparse_lookup": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(PxLookupTable),
-                                 c_int, c_void_p, ctypes.POINTER(PxGroupGeom), c_void_p,
+    "px_sparse_lookup": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(LookupTable),
+                                 c_int, c_void_p, ctypes.POINTER(GroupGeom), c_void_p,
                                  c_void_p, c_int, c_void_p]),
     "px_full_softmax_nll": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
-                                    c_void_p, c_int, ctypes.POINTER(PxGroupGeom), c_int,
+                                    c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
                                     c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
-    "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PxPushTable), c_int, c_int,
+    "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PushTable), c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_int,
-                               ctypes.POINTER(PxGroupGeom), c_void_p, c_int, c_int, c_int,
+                               ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int, c_int,
                                c_void_p]),
-    "px_sparse_owner": (c_int, [ctypes.POINTER(PxOwnerTable), c_int, c_int, c_void_p,
+    "px_sparse_owner": (c_int, [ctypes.POINTER(OwnerTable), c_int, c_int, c_void_p,
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                ctypes.POINTER(PxGroupGeom), c_void_p, c_int, c_int, c_int,
+                                ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int, c_int,
                                 c_int, c_void_p]),
     "px_stamp": (c_int, [c_void_p, c_void_p]),
 }
@@ -107,8 +104,30 @@ def available():
     return os.path.exists(LIB)
 
 
+def check_struct(cls, abi):
+    """Raise RuntimeError unless ctypes class `cls` has the layout `abi` (`sparse_abi()`)
+    gives the C struct of the same name: the same fields at the same offsets, same size."""
+    name = cls.__name__
+    ours = {"%s.%s" % (name, f): getattr(cls, f).offset for f, _ in cls._fields_}
+    ours[name] = ctypes.sizeof(cls)
+    for k in [k for k in abi if k.startswith(name + ".")] + list(ours):
+        if abi.get(k) != ours.get(k):
+            raise RuntimeError(
+                "%s and parallax_b200.ops disagree on %s (%s vs %s; a bare struct name is its "
+                "size): rebuild it with `python -m parallax_b200.ops.build`"
+                % (LIB, k, abi.get(k), ours.get(k)))
+
+
+def sparse_abi():
+    """The library's `px_sparse_abi()` as a dict: ``group_max``, ``hdr_words``,
+    ``ctl_bytes``, ``ctl_time_offset``, ``ctl_overflow_offset``, and per descriptor
+    ``Struct`` (its size) and ``Struct.field`` (byte offsets)."""
+    lib()
+    return _abi
+
+
 def lib(build_if_missing=True):
-    global _lib
+    global _lib, _abi
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB):
@@ -126,7 +145,11 @@ def lib(build_if_missing=True):
             continue        # optional symbol (added by later build stages)
         fn.restype = res
         fn.argtypes = args
-    _lib = L
+    L.px_sparse_abi.restype = ctypes.c_char_p    # required: a library without it fails here
+    abi = {k: int(v) for k, v in (kv.split("=") for kv in L.px_sparse_abi().decode().split())}
+    for cls in (GroupGeom, LookupTable, PushTable, OwnerTable):
+        check_struct(cls, abi)
+    _lib, _abi = L, abi
     return L
 
 

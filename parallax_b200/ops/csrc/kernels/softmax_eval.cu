@@ -258,14 +258,14 @@ extern "C" {
 // Returns 0, a negative argument error, or a CUDA error code.
 int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
                         const void* b_ptrs, int b_pitch, const int* row_cnt, int slots,
-                        const PxGroupGeom* g, int rank, const void* hdr_mine, const void* ctl,
+                        const GroupGeom* g, int rank, const void* hdr_mine, const void* ctl,
                         int wait, void* ws, int ws_ctas, const long long* targets, const void* wt,
                         const float* bt, float* nll, cudaStream_t stream) {
   using namespace tc;
   if (N <= 0) return 0;
   if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % 4) return -1;
   if (ws_ctas < 1 || slots < 1) return -2;
-  const GroupGeom G = to_geom(g);
+  const GroupGeom G = *g;
   EvalArgs a;
   a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const float* const*)b_ptrs;
   a.row_cnt = row_cnt;

@@ -37,6 +37,8 @@
 #include "optim_rules.cuh"
 #include "sparse_group.cuh"
 
+#include <string>
+
 __device__ __forceinline__ unsigned long long px_globaltimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -833,39 +835,55 @@ static void launch_push(int blocks, size_t smem, cudaStream_t stream, const int3
 
 extern "C" {
 
-// C mirrors of the per-table descriptors (plain pointers / ints, filled from Python)
-struct PxLookupTable { const void* srcs; void* out; int D4, src_bf16, out_bf16, pad; };
-struct PxPushTable {
-  const void* grads; float* staging; void* rings; void* tables; void* slot0s; void* slot1s;
-  void* slot2s; void* shadows; const float* hp; int D4, kind; float scale; int pad;
-};
-struct PxOwnerTable {
-  void* ring; float* table; float* slot0; float* slot1; float* slot2; void* shadow;
-  const float* hp; int D4, kind; float avg; int pad;
-};
-
-size_t px_sparse_ctl_bytes() { return sizeof(SparseCtl); }
-int px_sparse_hdr_words() { return PX_GRP_HDR_WORDS; }
-int px_sparse_group_max() { return PX_GRP_MAX; }
-// byte offset of the device timestamps inside SparseCtl (t_push[2], t_own[3]: 5 x u64)
-int px_sparse_ctl_time_offset() { return (int)offsetof(SparseCtl, t_push); }
-int px_sparse_ctl_overflow_offset() { return (int)offsetof(SparseCtl, overflow); }
+// The group constants and the layout of the descriptors Python fills through ctypes, as
+// `name=value` pairs: `Struct=sizeof(Struct)`, `Struct.field=offsetof(Struct, field)`.
+// `ops.lib()` checks its ctypes mirrors against it, so a field changed on one side only fails
+// at load.
+const char* px_sparse_abi() {
+  static const std::string abi = [] {
+    std::string s;
+    auto put = [&s](const char* k, size_t v) { s += std::string(k) + '=' + std::to_string(v) + ' '; };
+#define SIZE(S) put(#S, sizeof(S))
+#define FIELD(S, f) put(#S "." #f, offsetof(S, f))
+    put("ctl_bytes", sizeof(SparseCtl)); put("hdr_words", PX_GRP_HDR_WORDS);
+    put("group_max", PX_GRP_MAX);
+    // SparseCtl byte offsets of the u64 device timestamps (t_push, t_own, t_dbg) and of `overflow`
+    put("ctl_time_offset", offsetof(SparseCtl, t_push));
+    put("ctl_overflow_offset", offsetof(SparseCtl, overflow));
+    SIZE(GroupGeom); FIELD(GroupGeom, V); FIELD(GroupGeom, P); FIELD(GroupGeom, W);
+    FIELD(GroupGeom, rows_per_part); FIELD(GroupGeom, strategy); FIELD(GroupGeom, replicated);
+    FIELD(GroupGeom, extras); FIELD(GroupGeom, base); FIELD(GroupGeom, part_owner);
+    FIELD(GroupGeom, part_slot);
+    SIZE(LookupTable); FIELD(LookupTable, srcs); FIELD(LookupTable, out); FIELD(LookupTable, D4);
+    FIELD(LookupTable, src_bf16); FIELD(LookupTable, out_bf16);
+    SIZE(PushTable); FIELD(PushTable, grads); FIELD(PushTable, staging); FIELD(PushTable, rings);
+    FIELD(PushTable, tables); FIELD(PushTable, slot0s); FIELD(PushTable, slot1s);
+    FIELD(PushTable, slot2s); FIELD(PushTable, shadows); FIELD(PushTable, hp);
+    FIELD(PushTable, D4); FIELD(PushTable, kind); FIELD(PushTable, scale);
+    SIZE(OwnerTable); FIELD(OwnerTable, ring); FIELD(OwnerTable, table); FIELD(OwnerTable, slot0);
+    FIELD(OwnerTable, slot1); FIELD(OwnerTable, slot2); FIELD(OwnerTable, shadow);
+    FIELD(OwnerTable, hp); FIELD(OwnerTable, D4); FIELD(OwnerTable, kind); FIELD(OwnerTable, avg);
+#undef SIZE
+#undef FIELD
+    return s;
+  }();
+  return abi.c_str();
+}
 
 static inline int pick_lpr(int D4) { int l = 1; while (l < D4 && l < 32) l <<= 1; return l; }
 
 // ids_is64: 1 = int64 ids, 0 = int32.
-int px_sparse_lookup(const void* ids, int ids_is64, int n, const PxLookupTable* tabs, int nt,
-                     int32_t* pend_ids, const PxGroupGeom* g, const void* hdr_mine,
+int px_sparse_lookup(const void* ids, int ids_is64, int n, const LookupTable* tabs, int nt,
+                     int32_t* pend_ids, const GroupGeom* g, const void* hdr_mine,
                      const void* ctl, int wait, cudaStream_t stream) {
   if (n <= 0) return 0;
   if (nt < 1 || nt > PX_GRP_MAX) return -4;
-  const GroupGeom G = to_geom(g);
+  const GroupGeom G = *g;
   LookupArgs a{};
   a.nt = nt;
   int maxv = 1;
   for (int t = 0; t < nt; ++t) {
-    a.t[t].srcs = (const void* const*)tabs[t].srcs; a.t[t].out = tabs[t].out;
-    a.t[t].D4 = tabs[t].D4; a.t[t].src_bf16 = tabs[t].src_bf16; a.t[t].out_bf16 = tabs[t].out_bf16;
+    a.t[t] = tabs[t];
     const int v = tabs[t].src_bf16 ? (tabs[t].D4 + 1) / 2 : tabs[t].D4;
     if (v > maxv) maxv = v;
   }
@@ -893,25 +911,19 @@ static inline int push_hbits(int n, int blocks) {
 
 // grad_dtype / wire_dtype: 0 fp32, 1 bf16.  async: 1 = remote optimizer application (Hogwild).
 // All member tables of a group use the same optimizer kind family.
-int px_sparse_push(const int32_t* pend_ids, int n, const PxPushTable* tabs, int nt,
+int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt,
                    int grad_dtype, int wire_dtype, int async, void* ring_ids_dev, void* hdrs_dev,
-                   int cap, const PxGroupGeom* g, void* ctl, int rank, int dedup, int max_blocks,
+                   int cap, const GroupGeom* g, void* ctl, int rank, int dedup, int max_blocks,
                    cudaStream_t stream) {
   if (nt < 1 || nt > PX_GRP_MAX) return -4;
-  const GroupGeom G = to_geom(g);
+  const GroupGeom G = *g;
   PushArgs a{};
   a.nt = nt; a.ring_ids = (int32_t* const*)ring_ids_dev; a.hdrs = (uint32_t* const*)hdrs_dev;
   a.cap = cap; a.rank = rank;
-  int fam = 0;
+  const int fam = PX_KIND_FAMILY(tabs[0].kind);
   for (int t = 0; t < nt; ++t) {
-    PushTable& T = a.t[t];
-    T.grads = tabs[t].grads; T.staging = tabs[t].staging; T.rings = (char* const*)tabs[t].rings;
-    T.tables = (float* const*)tabs[t].tables; T.slot0s = (float* const*)tabs[t].slot0s;
-    T.slot1s = (float* const*)tabs[t].slot1s; T.slot2s = (float* const*)tabs[t].slot2s;
-    T.shadows = (__nv_bfloat16* const*)tabs[t].shadows; T.hp = tabs[t].hp;
-    T.D4 = tabs[t].D4; T.kind = tabs[t].kind; T.scale = tabs[t].scale;
-    if (t == 0) fam = PX_KIND_FAMILY(T.kind);
-    else if (fam != PX_KIND_FAMILY(T.kind)) return -6;
+    if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
+    a.t[t] = tabs[t];
   }
   int blocks = (n + 15) / 16;
   if (blocks > max_blocks) blocks = max_blocks;
@@ -934,24 +946,20 @@ int px_sparse_push(const int32_t* pend_ids, int n, const PxPushTable* tabs, int 
   return (int)cudaGetLastError();
 }
 
-int px_sparse_owner(const PxOwnerTable* tabs, int nt, int wire_dtype, const int32_t* ring_ids,
+int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_t* ring_ids,
                     void* hdr, void* hdrs_dev, int32_t* slotmap, int32_t* next, int cap,
-                    const PxGroupGeom* g, void* ctl, int rank, int use_merge, int blocks,
+                    const GroupGeom* g, void* ctl, int rank, int use_merge, int blocks,
                     int fixed_cnt, cudaStream_t stream) {
   if (nt < 1 || nt > PX_GRP_MAX) return -4;
-  GroupGeom G = to_geom(g);
+  GroupGeom G = *g;
   OwnerArgs a{};
   a.fixed_cnt = fixed_cnt;
   a.nt = nt; a.ring_ids = ring_ids; a.hdr = (uint32_t*)hdr; a.hdrs = (uint32_t* const*)hdrs_dev;
   a.slotmap = slotmap; a.next = next; a.cap = cap; a.rank = rank; a.use_merge = use_merge;
-  int fam = 0;
+  const int fam = PX_KIND_FAMILY(tabs[0].kind);
   for (int t = 0; t < nt; ++t) {
-    OwnerTable& T = a.t[t];
-    T.ring = (char*)tabs[t].ring; T.table = tabs[t].table; T.slot0 = tabs[t].slot0;
-    T.slot1 = tabs[t].slot1; T.slot2 = tabs[t].slot2; T.shadow = (__nv_bfloat16*)tabs[t].shadow;
-    T.hp = tabs[t].hp; T.D4 = tabs[t].D4; T.kind = tabs[t].kind; T.avg = tabs[t].avg;
-    if (t == 0) fam = PX_KIND_FAMILY(T.kind);
-    else if (fam != PX_KIND_FAMILY(T.kind)) return -6;
+    if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
+    a.t[t] = tabs[t];
   }
   if (blocks < 1) blocks = 1;
   if (fixed_cnt < 0 && G.W > 1)

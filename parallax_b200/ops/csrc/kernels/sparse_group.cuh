@@ -1,5 +1,7 @@
 // Geometry and control block of a sparse co-lookup group, shared by the kernels that read
 // a group's tables (sparse.cu: lookup / push / owner; softmax_eval.cu: full-softmax eval).
+// Python fills GroupGeom through the ctypes class of the same name (`ops.GroupGeom`);
+// `px_sparse_abi` in sparse.cu publishes its layout so that `ops.lib()` can check the two agree.
 #pragma once
 #include "common.cuh"
 
@@ -30,14 +32,3 @@ struct SparseCtl {
 
 // group header (symmetric): [pushed[R] | applied[R] | cnt[R]]
 #define PX_GRP_HDR_WORDS (3 * PX_MAX_RANKS)
-
-// C mirror of GroupGeom (filled from Python, `ops.PxGroupGeom`)
-struct PxGroupGeom {
-  int V, P, W, rows_per_part, strategy, replicated, extras, base;
-  const int* part_owner; const int* part_slot;
-};
-static inline GroupGeom to_geom(const PxGroupGeom* g) {
-  GroupGeom t; t.V = g->V; t.P = g->P; t.W = g->W; t.rows_per_part = g->rows_per_part;
-  t.strategy = g->strategy; t.replicated = g->replicated; t.extras = g->extras; t.base = g->base;
-  t.part_owner = g->part_owner; t.part_slot = g->part_slot; return t;
-}

@@ -25,23 +25,23 @@ Reference semantics kept (file:line in /root/reference/parallax/parallax):
   replay shapes are static.
 """
 import ctypes
-import math
 
 import torch
 
-from .. import consts, optim as _optim
+from .. import consts, ops, optim as _optim
 from ..log import parallax_log
 from . import modes
 from .layout import TableLayout
 
 _vp = ctypes.c_void_p
-_ES = {torch.float32: 4, torch.bfloat16: 2}
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 
 
-def _lib():
-    from .. import ops
-    return ops.lib()
+def _lookup_table(t, src, out):
+    """LookupTable descriptor: table `t`'s rows, read from every rank's `src` ("shadow":
+    the bf16 copy, "table": the fp32 master), into `out`."""
+    return ops.LookupTable(t.dev_ptrs(src).data_ptr(), out.data_ptr(), t.D4,
+                           int(src == "shadow"), int(out.dtype == torch.bfloat16))
 
 
 def _count(k=1):
@@ -316,9 +316,8 @@ class NVSparseGroup(object):
     _seq = 0
 
     def __init__(self, tables, name=None):
-        from .. import ops
-        L = _lib()
-        gmax = int(L.px_sparse_group_max())
+        abi = ops.sparse_abi()
+        gmax = abi["group_max"]
         if not 1 <= len(tables) <= gmax:
             raise ValueError("a co-lookup group holds 1..%d tables" % gmax)
         t0 = tables[0]
@@ -352,7 +351,7 @@ class NVSparseGroup(object):
         lay = self.layout
         self._owners_dev = torch.tensor(lay.owners, dtype=torch.int32, device=self.device)
         self._slots_dev = torch.tensor(lay.slots, dtype=torch.int32, device=self.device)
-        g = ops.PxGroupGeom()
+        g = ops.GroupGeom()
         g.V, g.P, g.W, g.rows_per_part = lay.V, lay.P, lay.world, lay.rows_per_part
         g.strategy = 0 if lay.strategy == "mod" else 1
         g.replicated = 1 if lay.replicated else 0
@@ -360,11 +359,8 @@ class NVSparseGroup(object):
         g.part_owner = self._owners_dev.data_ptr()
         g.part_slot = self._slots_dev.data_ptr()
         self.geom = g
-        self.ctl = torch.zeros(int(L.px_sparse_ctl_bytes()) // 4, dtype=torch.int32,
-                               device=self.device)
-        self._t_off = int(L.px_sparse_ctl_time_offset())
-        self._ovf_off = int(L.px_sparse_ctl_overflow_offset())
-        self.hdr_buf = self.heap.alloc(int(L.px_sparse_hdr_words()) * 4, "hdr:" + self.name)
+        self.ctl = torch.zeros(abi["ctl_bytes"] // 4, dtype=torch.int32, device=self.device)
+        self.hdr_buf = self.heap.alloc(abi["hdr_words"] * 4, "hdr:" + self.name)
         self.ids_buf = None
         self.slotmap = torch.full((lay.rows_local,), -1, dtype=torch.int32,
                                   device=self.device)
@@ -388,23 +384,17 @@ class NVSparseGroup(object):
                 self.route.sync)
 
     def _place(self, ids):
-        """(valid, owner, local row) of global ids — device tensor arithmetic."""
+        """(valid, owner, local row) of global ids from the device-resident maps (`owner_of` /
+        `local_row_of` of TableLayout copy host maps over: illegal in a CUDA-graph capture)."""
         lay = self.layout
         valid = (ids >= 0) & (ids < lay.V)
         idc = ids.clamp(0, lay.V - 1).to(torch.int64)
         if lay.replicated:
             return valid, torch.zeros_like(idc), idc
-        if lay.strategy == "mod":
-            p, idx = idc % lay.P, idc // lay.P
-        else:
-            thr = lay._extras * (lay._base + 1)
-            p = torch.where(idc < thr, idc // (lay._base + 1),
-                            (idc - lay._extras) // max(lay._base, 1))
-            start = torch.where(p < lay._extras, p * (lay._base + 1),
-                                p * lay._base + lay._extras)
-            idx = idc - start
+        p = lay.partition_of(idc)
         owner = self._owners_dev[p].to(torch.int64)
-        local = self._slots_dev[p].to(torch.int64) * lay.rows_per_part + idx
+        local = self._slots_dev[p].to(torch.int64) * lay.rows_per_part + \
+            lay.index_in_partition(idc)
         return valid, owner, local
 
     def _lookup_nccl(self, members, ids, n, record):
@@ -435,10 +425,7 @@ class NVSparseGroup(object):
         """all-gather (ids, rows) from every rank, then the owner kernel applies the rows
         this rank owns (entries of other owners are marked -1)."""
         import torch.distributed as dist
-        from .. import ops
-        L = _lib()
         W, grp = self.world, self.comm.group
-        nt = len(self.tables)
         with torch.cuda.stream(cs):
             all_ids = torch.empty(W * n, dtype=torch.int32, device=self.device)
             dist.all_gather_into_tensor(all_ids, pend_ids, group=grp)
@@ -446,35 +433,33 @@ class NVSparseGroup(object):
             mine = valid if self.replicated else (valid & (owner == self.rank))
             ring_ids = torch.where(mine, local, torch.full_like(local, -1)).to(torch.int32)
             nxt = torch.empty(W * n, dtype=torch.int32, device=self.device)
-            descs = (ops.PxOwnerTable * nt)()
-            keep = [all_ids, ring_ids, nxt]
-            for d, t, g in zip(descs, self.tables, grads):
+            all_gs = []
+            for t, g in zip(self.tables, grads):
                 all_g = torch.empty(W * n, t.Dp, dtype=g.dtype, device=self.device)
                 dist.all_gather_into_tensor(all_g, g, group=grp)
-                keep.append(all_g)
-                d.ring, d.table = all_g.data_ptr(), t.table.data_ptr()
-                d.slot0 = t.slots[0].data_ptr() if t.nslots > 0 else 0
-                d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
-                d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
-                d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
-                d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
-                d.avg = ((1.0 / W) if t.average else 1.0) * t.scale
+                all_gs.append(all_g)
+            # the rows travel unscaled through all_gather: the owner applies the scale
+            descs = self._owner_tables([g.data_ptr() for g in all_gs], sender_scaled=False)
+            keep = [all_ids, ring_ids, nxt] + all_gs
             if not torch.cuda.is_current_stream_capturing():
                 for k_ in keep:
                     k_.record_stream(cs)
             self._keep_n = (keep, descs)
             blocks = max(1, min(self.max_blocks, (n * W + 7) // 8))
             _count()
-            ops.check(L.px_sparse_owner(
-                descs, nt, _DT[grads[0].dtype], _vp(ring_ids.data_ptr()),
+            ops.check(ops.lib().px_sparse_owner(
+                descs, len(self.tables), _DT[grads[0].dtype], _vp(ring_ids.data_ptr()),
                 _vp(self.hdr_buf.local_ptr), _vp(self.hdrs_dev.data_ptr()),
                 _vp(self.slotmap.data_ptr()), _vp(nxt.data_ptr()), n,
                 ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank, 1, blocks, n,
                 _sp(cs)), "sparse_owner(nccl)")
 
+    @property
+    def _wait(self):
+        """1: lookups and the eval first wait for every owner's `applied` flag (sync NVLink)."""
+        return 1 if (self.route.sync and self.world > 1 and not self._nccl()) else 0
+
     def lookup(self, flat_ids, record=True, members=None):
-        from .. import ops
-        L = _lib()
         members = self.tables if members is None else members
         n = int(flat_ids.numel())
         ids = flat_ids if flat_ids.is_cuda else flat_ids.to(self.device, non_blocking=True)
@@ -483,29 +468,23 @@ class NVSparseGroup(object):
         ids = ids.contiguous()
         if self._nccl() and not self.replicated and n > 0:
             return self._lookup_nccl(members, ids, n, record)
-        descs = (ops.PxLookupTable * len(members))()
-        outs = []
-        for d, t in zip(descs, members):
-            if t.use_shadow:
-                out = torch.empty((n, t.Dps), dtype=torch.bfloat16, device=self.device)
-                d.srcs, d.src_bf16, d.out_bf16 = t.dev_ptrs("shadow").data_ptr(), 1, 1
-            else:
-                out = torch.empty((n, t.Dp), dtype=t.out_dtype, device=self.device)
-                d.srcs, d.src_bf16 = t.dev_ptrs("table").data_ptr(), 0
-                d.out_bf16 = 1 if t.out_dtype == torch.bfloat16 else 0
-            d.out, d.D4 = out.data_ptr(), t.D4
+        descs, outs = (ops.LookupTable * len(members))(), []
+        for i, t in enumerate(members):
+            # a table with a shadow has bf16 outputs: rows are copied at the shadow's width
+            out = torch.empty((n, t.Dps if t.use_shadow else t.Dp), dtype=t.out_dtype,
+                              device=self.device)
+            descs[i] = _lookup_table(t, "shadow" if t.use_shadow else "table", out)
             outs.append(out if out.shape[1] == t.D else out[:, :t.D])
         pend = torch.empty(n, dtype=torch.int32, device=self.device) if record else None
         if record:
             self._fwd_calls += 1
         if n > 0:
             _count()
-            ops.check(L.px_sparse_lookup(
+            ops.check(ops.lib().px_sparse_lookup(
                 _vp(ids.data_ptr()), 1 if ids.dtype == torch.int64 else 0, n, descs,
                 len(members), _vp(pend.data_ptr()) if pend is not None else _vp(0),
                 ctypes.byref(self.geom), _vp(self.hdr_buf.local_ptr),
-                _vp(self.ctl.data_ptr()),
-                1 if (self.route.sync and self.world > 1 and not self._nccl()) else 0,
+                _vp(self.ctl.data_ptr()), self._wait,
                 _sp(torch.cuda.current_stream(self.device))), "sparse_lookup")
         return outs, pend
 
@@ -529,8 +508,7 @@ class NVSparseGroup(object):
         table and no [N, V] logits (`ops/csrc/kernels/softmax_eval.cu`).  The targets' rows
         come from one launch of the group's lookup kernel.  A target outside [0, V) gives
         NaN in its row.  One-sided: no other rank takes part."""
-        from .. import ops
-        L = _lib()
+        L = ops.lib()
         tw, tb = self.tables
         n, K = int(x.shape[0]), int(x.shape[1])
         if not tw.use_shadow or tb.D != 1 or K != tw.D or x.dtype != torch.bfloat16:
@@ -543,17 +521,13 @@ class NVSparseGroup(object):
         if x.data_ptr() % 16:                      # TMA needs a 16-byte aligned base
             x = x.clone()
         ids = targets.reshape(-1).to(self.device, torch.int64).contiguous()
-        wait = 1 if (self.route.sync and self.world > 1 and not self._nccl()) else 0
+        wait = self._wait
         stream = _sp(torch.cuda.current_stream(self.device))
         w_t = torch.empty((n, tw.Dps), dtype=torch.bfloat16, device=self.device)
         b_t = torch.empty((n, tb.Dp), dtype=torch.float32, device=self.device)
-        descs = (ops.PxLookupTable * 2)()
-        descs[0].srcs, descs[0].out, descs[0].D4 = \
-            tw.dev_ptrs("shadow").data_ptr(), w_t.data_ptr(), tw.D4
-        descs[0].src_bf16, descs[0].out_bf16 = 1, 1
-        descs[1].srcs, descs[1].out, descs[1].D4 = \
-            tb.dev_ptrs("table").data_ptr(), b_t.data_ptr(), tb.D4
-        descs[1].src_bf16, descs[1].out_bf16 = 0, 0
+        # target bias from the fp32 master like every bias row the eval kernel reads
+        descs = (ops.LookupTable * 2)(_lookup_table(tw, "shadow", w_t),
+                                      _lookup_table(tb, "table", b_t))
         _count()
         ops.check(L.px_sparse_lookup(
             _vp(ids.data_ptr()), 1, n, descs, 2, _vp(0), ctypes.byref(self.geom),
@@ -693,14 +667,10 @@ class NVSparseGroup(object):
         self._done_step = step
         if self._nccl():
             cs = stream if stream is not None else self.fabric.comm_stream
-            calls, self.calls = self.calls, []
-            if not calls:
+            pend_ids, grads = self._take_calls()
+            if pend_ids is None:
                 raise RuntimeError("protocol='nccl': every rank must look the group %s up in "
                                    "every step (collective)" % self.name)
-            nt = len(self.tables)
-            pend_ids = calls[0][0] if len(calls) == 1 else torch.cat([c[0] for c in calls])
-            grads = [calls[0][1][k] if len(calls) == 1 else
-                     torch.cat([c[1][k] for c in calls]) for k in range(nt)]
             cur = torch.cuda.current_stream(self.device)
             if cs is not cur:
                 cs.wait_stream(cur)
@@ -718,20 +688,23 @@ class NVSparseGroup(object):
             if self.route.sync:
                 self.stage_apply(step, stream)
 
+    def _take_calls(self):
+        """Pending ids and per-table gradient rows of this step's lookups, concatenated,
+        or (None, None) when there were none; the list starts empty again."""
+        calls, self.calls = self.calls, []
+        if len(calls) <= 1:
+            return calls[0] if calls else (None, None)
+        ids, grads = zip(*calls)
+        return torch.cat(ids), [torch.cat(g) for g in zip(*grads)]
+
     def stage_push(self, step, stream=None):
         """Sender side, one kernel: local aggregation + push (or remote apply in async
         mode).  Separate from `stage_apply` so that a world simulated on one GPU can
         enqueue every rank's push before any rank's (spinning) owner kernel."""
-        from .. import ops
-        L = _lib()
         cs = stream if stream is not None else self.fabric.comm_stream
-        calls, self.calls = self.calls, []
         nt = len(self.tables)
-        if calls:
-            pend_ids = calls[0][0] if len(calls) == 1 else torch.cat([c[0] for c in calls])
-            grads = [calls[0][1][k] if len(calls) == 1 else
-                     torch.cat([c[1][k] for c in calls]) for k in range(nt)]
-        else:
+        pend_ids, grads = self._take_calls()
+        if pend_ids is None:
             pend_ids = torch.empty(0, dtype=torch.int32, device=self.device)
             grads = [torch.empty((0, t.Dp), dtype=torch.float32, device=self.device)
                      for t in self.tables]
@@ -759,7 +732,7 @@ class NVSparseGroup(object):
                 pend_ids.record_stream(cs)
                 for g in grads:
                     g.record_stream(cs)
-        descs = (ops.PxPushTable * nt)()
+        descs = (ops.PushTable * nt)()
         for d, t, g in zip(descs, self.tables, grads):
             d.grads, d.staging = g.data_ptr(), t.staging.data_ptr()
             d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
@@ -775,7 +748,7 @@ class NVSparseGroup(object):
                 d.scale = t.scale
         self._keep = (pend_ids, grads, descs)
         _count()
-        ops.check(L.px_sparse_push(
+        ops.check(ops.lib().px_sparse_push(
             _vp(pend_ids.data_ptr()), n, descs, nt, _DT[gdt],
             _DT[self.wire_dtype] if sync else 0, 0 if sync else 1,
             _vp(self.ids_dev.data_ptr()) if sync else _vp(0),
@@ -783,13 +756,25 @@ class NVSparseGroup(object):
             ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
             1 if self.local_aggregation else 0, self.max_blocks, _sp(cs)), "sparse_push")
 
+    def _owner_tables(self, rings, sender_scaled):
+        """OwnerTable per member table, merging the rows at device address rings[i]; the
+        owner applies the ScaleGradients factor unless the sender did (`sender_scaled`)."""
+        descs = (ops.OwnerTable * len(self.tables))()
+        for d, t, ring in zip(descs, self.tables, rings):
+            d.ring, d.table = ring, t.table.data_ptr()
+            d.slot0 = t.slots[0].data_ptr() if t.nslots > 0 else 0
+            d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
+            d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
+            d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
+            d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
+            avg = (1.0 / self.world) if t.average else 1.0
+            d.avg = avg if sender_scaled else avg * t.scale
+        return descs
+
     def stage_apply(self, step, stream=None):
         """Owner side, one kernel: merge rows from all sources, apply the optimizer."""
-        from .. import ops
-        L = _lib()
         cs = stream if stream is not None else self.fabric.comm_stream
         n = max(self._last_n, 1)
-        nt = len(self.tables)
         # 16 half-warps per CTA, one entry per half-warp: as many CTAs as fit on the device at once
         # (4 per SM at 64 registers; the merge variant is a cooperative launch)
         blocks = max(1, min(max(self.max_blocks, consts.NUM_SMS * 4)
@@ -797,22 +782,12 @@ class NVSparseGroup(object):
                             else self.max_blocks,
                             (n * (self.world if self.replicated else 1) + 15) // 16))
         use_merge = self.world > 1 or not self.local_aggregation
-        descs = (ops.PxOwnerTable * nt)()
-        for d, t in zip(descs, self.tables):
-            d.ring, d.table = t.ring_buf.local_ptr, t.table.data_ptr()
-            d.slot0 = t.slots[0].data_ptr() if t.nslots > 0 else 0
-            d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
-            d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
-            d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
-            d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
-            avg = (1.0 / self.world) if t.average else 1.0
-            if not self.boundary:
-                avg *= t.scale
-            d.avg = avg
+        descs = self._owner_tables([t.ring_buf.local_ptr for t in self.tables],
+                                   sender_scaled=self.boundary)
         self._keep_o = descs
         _count()
-        ops.check(L.px_sparse_owner(
-            descs, nt, _DT[self.wire_dtype], _vp(self.ids_buf.local_ptr),
+        ops.check(ops.lib().px_sparse_owner(
+            descs, len(self.tables), _DT[self.wire_dtype], _vp(self.ids_buf.local_ptr),
             _vp(self.hdr_buf.local_ptr), _vp(self.hdrs_dev.data_ptr()),
             _vp(self.slotmap.data_ptr()), _vp(self.next.data_ptr()), self.cap,
             ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
@@ -823,15 +798,15 @@ class NVSparseGroup(object):
         """%globaltimer stamps (ns) written by the last push / owner kernels:
         push start, pushed flag published, owner start, all sources arrived, applied
         published.  Valid under CUDA-graph replay (the kernels write them every run)."""
-        raw = self.ctl.view(torch.uint8)[self._t_off:self._t_off + 104].clone() \
-            .view(torch.int64).tolist()
+        off = ops.sparse_abi()["ctl_time_offset"]
+        raw = self.ctl.view(torch.uint8)[off:off + 104].clone().view(torch.int64).tolist()
         d = dict(zip(("push_start", "pushed", "owner_start", "arrived", "applied"), raw))
         d["push_phases"] = raw[5:13]        # CTA 0 of the push kernel: end of each phase
         return d
 
     def overflow_count(self):
-        return int(self.ctl.view(torch.uint8)[self._ovf_off:self._ovf_off + 4]
-                   .clone().view(torch.int32).item())
+        off = ops.sparse_abi()["ctl_overflow_offset"]
+        return int(self.ctl.view(torch.uint8)[off:off + 4].clone().view(torch.int32).item())
 
     def release_shared(self):
         for b in (self.hdr_buf, self.ids_buf):
