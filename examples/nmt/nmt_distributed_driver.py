@@ -46,6 +46,9 @@ ap.add_argument("--hparams", default="", help="name=value,... overrides")
 ap.add_argument("--num_train_steps", type=int, default=None)
 ap.add_argument("--steps_per_eval", type=int, default=None)
 ap.add_argument("--random_seed", type=int, default=None)
+ap.add_argument("--clip_embeddings_jointly", action="store_true",
+                help="clip embeddings and dense variables by one global norm, as the "
+                     "reference does (default: each embedding's gradient on its own)")
 ap.add_argument("--eval_only", action="store_true",
                 help="restore the latest checkpoint of out_dir / --ckpt_dir and run the internal "
                      "(perplexity) and external (BLEU, …) evaluations — the reference's nmt_eval.py")
@@ -94,6 +97,8 @@ def build_hparams():
         hp.steps_per_eval = FLAGS.steps_per_eval
     if FLAGS.random_seed is not None:
         hp.random_seed = FLAGS.random_seed
+    if FLAGS.clip_embeddings_jointly:
+        hp.clip_embeddings_jointly = True
     hp.parse(FLAGS.hparams)
     if not hp.vocab_prefix:
         raise ValueError("--vocab_prefix (or --synthetic) is required")

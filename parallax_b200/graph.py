@@ -8,7 +8,7 @@ optimizer spec, and declarative gradient post-processing that in the reference
 lives in the user graph between `tf.gradients` and `apply_gradients`
 (e.g. LM1B: `examples/lm1b/language_model_graph.py:44-62`):
 
-* `ClipByGlobalNorm(max_norm, params)`  — `tf.clip_by_global_norm`
+* `ClipByGlobalNorm(max_norm, params, include_sparse)` — `tf.clip_by_global_norm`
 * `ScaleGradients(factor, params)`      — e.g. embedding grads × batch_size
 * `ClipByValue(clip, params)`            — `tf.clip_by_value`
 * `ExponentialMovingAverage(decay, params)` — `ema.apply(lstm_vars)`
@@ -48,12 +48,31 @@ class GradRule(object):
 
 
 class ClipByGlobalNorm(GradRule):
-    """Scale the (aggregated) dense gradients of `params` so that their joint
-    L2 norm is at most `max_norm` (`tf.clip_by_global_norm`)."""
+    """Scale the aggregated gradients of `params` so that their joint L2 norm is
+    at most `max_norm` (`tf.clip_by_global_norm`).
 
-    def __init__(self, max_norm, params=None):
+    With ``include_sparse=False`` (the default) only dense variables are matched:
+    their gradient is the mean over workers after `ScaleGradients`.
+
+    With ``include_sparse=True`` every sparse variable (embedding table) matched by
+    `params` joins the norm too.  Its gradient is the one the optimizer applies
+    this step: after `ScaleGradients`, duplicate ids merged, summed over workers
+    (÷ num_workers with ``average_sparse``); rows not touched contribute 0.  Then::
+
+        norm  = sqrt(Σ_dense ‖g_v‖² + Σ_sparse Σ_rows ‖g_v[row]‖²)
+        scale = max_norm / max(norm, max_norm)
+
+    and every matched gradient, dense and sparse, is multiplied by `scale`
+    before its update; sparse optimizers still touch only the rows that received
+    gradient.  This equals ``torch.nn.utils.clip_grad_norm_`` over the matched
+    parameters of a single-device model whose embeddings have dense gradients.
+    A variable belongs to the first clip rule that matches it.  Needs
+    ``sync=True``."""
+
+    def __init__(self, max_norm, params=None, include_sparse=False):
         super().__init__(params)
         self.max_norm = float(max_norm)
+        self.include_sparse = bool(include_sparse)
 
 
 class ScaleGradients(GradRule):
@@ -133,6 +152,15 @@ class Graph(object):
     # -- helpers used by the engine -------------------------------------------
     def clip_rules(self):
         return [r for r in self.grad_rules if isinstance(r, ClipByGlobalNorm)]
+
+    def joint_clip_index(self, name):
+        """Index in `clip_rules()` of the rule that clips sparse variable `name`
+        jointly with its dense variables (the first rule matching `name`, when it
+        has ``include_sparse``), else -1."""
+        for i, r in enumerate(self.clip_rules()):
+            if r.applies_to(name):
+                return i if r.include_sparse else -1
+        return -1
 
     def scale_for(self, name):
         f = 1.0

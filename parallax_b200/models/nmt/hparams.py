@@ -139,6 +139,9 @@ def create_standard_hparams():
         # train
         optimizer="sgd", batch_size=128, init_op="uniform", init_weight=0.1,
         max_gradient_norm=5.0, learning_rate=1.0, warmup_steps=0,
+        # True: one global norm over dense variables and embeddings, as the reference
+        # clips (`nmt_graph`); False: each embedding's gradient is clipped on its own
+        clip_embeddings_jointly=False,
         warmup_scheme="t2t", decay_scheme="luong234",
         colocate_gradients_with_ops=True, num_train_steps=12000,
         # data constraints

@@ -451,11 +451,14 @@ class Seq2Seq(nn.Module):
     def _embed(self, table, ids):
         """lookup + (training) clip of the gradient flowing back into the looked-up
         rows.  The reference clips embeddings and dense variables by ONE joint
-        global norm (`model.py:196-205`); the engine's clip reduces over the dense
-        buckets only, so the sparse gradient of each table is clipped here by its
-        own norm, per worker, before it is pushed to the row owners."""
+        global norm (`model.py:196-205`); that is what ``clip_embeddings_jointly``
+        selects (`nmt_graph`), and nothing is clipped here.  By default the
+        engine's clip covers the dense variables only, and the sparse gradient of
+        each lookup is clipped here by its own norm, per worker, before it is
+        pushed to the row owners."""
         emb = table(ids).to(self.compute_dtype)
-        if self.training and torch.is_grad_enabled() and self.hp.max_gradient_norm:
+        if self.training and torch.is_grad_enabled() and self.hp.max_gradient_norm and \
+                not self.hp.get("clip_embeddings_jointly", False):
             emb = _ClipGradNorm.apply(emb, float(self.hp.max_gradient_norm))
         return emb
 
@@ -532,9 +535,10 @@ def learning_rate_fn(hp):
 def nmt_graph(model, hp=None):
     """SGD (with the decay schedule) or Adam + global-norm clipping
     (`model.py:160-205`).  The reference clips embeddings and dense variables
-    jointly; here the engine's clip covers the dense variables and each
-    embedding's sparse gradient is clipped by its own norm inside the model
-    (`Seq2Seq._embed`)."""
+    jointly; ``hp.clip_embeddings_jointly`` does the same with one
+    ``ClipByGlobalNorm(include_sparse=True)`` over every variable.  By default the
+    engine's clip covers the dense variables and each embedding's sparse
+    gradient is clipped by its own norm inside the model (`Seq2Seq._embed`)."""
     hp = hp or model.hp
     lr = learning_rate_fn(hp)
     if hp.optimizer == "sgd":
@@ -546,8 +550,12 @@ def nmt_graph(model, hp=None):
     else:
         raise ValueError("Unknown optimizer type %s" % hp.optimizer)
     dense = lambda n: not n.startswith("embedding_")
-    rules = [ClipByGlobalNorm(hp.max_gradient_norm, params=dense)] \
-        if hp.max_gradient_norm else []
+    if not hp.max_gradient_norm:
+        rules = []
+    elif hp.get("clip_embeddings_jointly", False):
+        rules = [ClipByGlobalNorm(hp.max_gradient_norm, include_sparse=True)]
+    else:
+        rules = [ClipByGlobalNorm(hp.max_gradient_norm, params=dense)]
     return Graph(model, optimizer=opt, grad_rules=rules, name="nmt")
 
 

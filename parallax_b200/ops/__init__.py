@@ -96,6 +96,11 @@ _SIGS = {
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                 ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int, c_int,
                                 c_int, c_void_p]),
+    "px_sparse_owner_norm": (c_int, [ctypes.POINTER(OwnerTable), c_int, c_int, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_int,
+                                     ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int,
+                                     c_void_p, c_void_p]),
+    "px_clip_hp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "px_stamp": (c_int, [c_void_p, c_void_p]),
 }
 

@@ -995,3 +995,150 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------- joint global-norm clip
+// ClipByGlobalNorm(include_sparse=True): the norm covers this group's aggregated rows, so
+// it is taken on the owner, from the rings, before the (unchanged) owner kernel applies
+// them.  The clip factor then reaches the owner kernel through the slot it already
+// multiplies by, hp[HP_GSCALE], in a private copy of the group's hyper-parameters.
+
+// Σ over the touched rows of ‖avg · hp[HP_GSCALE] · Σ_entries row‖², i.e. exactly the rows
+// px_sparse_owner_kernel would hand to the optimizer, added to *sumsq.  Links entries per
+// row like the owner kernel's merge path (one grid barrier, cooperative launch), resets the
+// slotmap entries it linked and returns ctl->bar / ctl->apply_done to 0; publishes no flag
+// and leaves ctl->step alone, so the owner kernel runs next exactly as it would have.
+template <typename WireT>
+__global__ void __launch_bounds__(256)
+px_sparse_owner_norm_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl, float* sumsq) {
+  __shared__ int s_pre[PX_MAX_RANKS + 1];
+  __shared__ double s_part[8];
+  const uint32_t* cnt = a.hdr + 2 * PX_MAX_RANKS;
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int s = 0; s < g.W; ++s) {
+      s_pre[s] = acc;
+      acc += (int)ld_volatile_u32(cnt + s);
+    }
+    s_pre[g.W] = acc;
+  }
+  __syncthreads();
+  const int total = s_pre[g.W];
+  if (a.use_merge) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+      int s = 0;
+      while (i >= s_pre[s + 1]) ++s;
+      const int e = s * a.cap + (i - s_pre[s]);
+      const int r = a.ring_ids[e];
+      if (r >= 0) a.next[e] = atomicExch(&a.slotmap[r], e);
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      atomicAdd(&ctl->bar, 1u);
+      while (ld_volatile_u32(&ctl->bar) < gridDim.x) { }
+      __threadfence();
+    }
+    __syncthreads();
+  }
+  // 16 lanes per entry, as in the owner kernel; fp64 partial sums
+  const int lane = threadIdx.x & 15, warps = blockDim.x >> 4;
+  const unsigned hmask = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
+  double acc = 0.0;
+  for (int i = blockIdx.x * warps + (threadIdx.x >> 4); i < total; i += gridDim.x * warps) {
+    int s = 0;
+    while (i >= s_pre[s + 1]) ++s;
+    const int e = s * a.cap + (i - s_pre[s]);
+    const int r = a.ring_ids[e];
+    if (r < 0) continue;
+    if (a.use_merge && __ldcg(a.slotmap + r) != e) continue;       // not the list head
+#pragma unroll 1
+    for (int t = 0; t < a.nt; ++t) {
+      const OwnerTable& T = a.t[t];
+      const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
+      const float gmul = T.avg * T.hp[HP_GSCALE];
+      for (int cidx = lane; cidx < T.D4; cidx += 16) {
+        float4 gv = ld_wire4<WireT>(T.ring + (size_t)e * row_bytes, cidx);
+        if (a.use_merge) {
+          for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
+            const float4 o = ld_wire4<WireT>(T.ring + (size_t)x * row_bytes, cidx);
+            gv.x += o.x; gv.y += o.y; gv.z += o.z; gv.w += o.w;
+          }
+        }
+        gv.x *= gmul; gv.y *= gmul; gv.z *= gmul; gv.w *= gmul;
+        acc += (double)gv.x * gv.x + (double)gv.y * gv.y + (double)gv.z * gv.z +
+               (double)gv.w * gv.w;
+      }
+    }
+    __syncwarp(hmask);
+    if (a.use_merge && lane == 0) a.slotmap[r] = -1;
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) b += s_part[w];
+    if (b != 0.0) atomicAdd(sumsq, (float)b);
+    // every CTA has left the grid barrier once it takes a ticket: the last one resets it
+    if (atomicAdd(&ctl->apply_done, 1u) == gridDim.x - 1) { ctl->bar = 0; ctl->apply_done = 0; }
+  }
+}
+
+// out = hp with out[HP_GSCALE] = hp[HP_GSCALE] · *scale: the hyper-parameters one group
+// applies with this step (the shared vector stays untouched for every other reader).
+__global__ void px_clip_hp_kernel(const float* hp, const float* scale, float* out) {
+  if (threadIdx.x <= HP_FLAGS)
+    out[threadIdx.x] = threadIdx.x == HP_GSCALE ? hp[threadIdx.x] * *scale : hp[threadIdx.x];
+}
+
+extern "C" {
+
+// `sumsq` += the squared norm of what px_sparse_owner would apply this step (see the kernel).
+// Launched after the group's push and before its px_sparse_owner, with the same ring / slotmap
+// arguments; waits for every source's `pushed` flag first.
+int px_sparse_owner_norm(const OwnerTable* tabs, int nt, int wire_dtype, const int32_t* ring_ids,
+                         void* hdr, int32_t* slotmap, int32_t* next, int cap, const GroupGeom* g,
+                         void* ctl, int use_merge, int blocks, float* sumsq,
+                         cudaStream_t stream) {
+  if (nt < 1 || nt > PX_GRP_MAX) return -4;
+  GroupGeom G = *g;
+  OwnerArgs a{};
+  a.fixed_cnt = -1;
+  a.nt = nt; a.ring_ids = ring_ids; a.hdr = (uint32_t*)hdr; a.hdrs = nullptr;
+  a.slotmap = slotmap; a.next = next; a.cap = cap; a.rank = 0; a.use_merge = use_merge;
+  for (int t = 0; t < nt; ++t) a.t[t] = tabs[t];
+  if (blocks < 1) blocks = 1;
+  if (G.W > 1)
+    px_sparse_wait_kernel<<<1, 32, 0, stream>>>((const uint32_t*)hdr, (const SparseCtl*)ctl, G.W);
+  const void* fn = wire_dtype == 0 ? (const void*)px_sparse_owner_norm_kernel<float>
+                                   : (const void*)px_sparse_owner_norm_kernel<__nv_bfloat16>;
+  static int max_coop[2] = {0, 0};
+  int& mc = max_coop[wire_dtype == 0 ? 0 : 1];
+  if (mc == 0) {
+    int per_sm = 0, dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0);
+    mc = per_sm * sms;
+    if (mc < 1) mc = 1;
+  }
+  SparseCtl* C = (SparseCtl*)ctl;
+  void* args[] = {&a, &G, &C, &sumsq};
+  cudaError_t e;
+  if (use_merge) {
+    if (blocks > mc) blocks = mc;
+    if (blocks > PX_NUM_SMS * 4) blocks = PX_NUM_SMS * 4;
+    e = cudaLaunchCooperativeKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
+  } else {
+    e = cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
+  }
+  if (e != cudaSuccess) return (int)e;
+  return (int)cudaGetLastError();
+}
+
+int px_clip_hp(const float* hp, const float* scale, float* out, cudaStream_t stream) {
+  px_clip_hp_kernel<<<1, 32, 0, stream>>>(hp, scale, out);
+  return (int)cudaGetLastError();
+}
+
+}  // extern "C"

@@ -233,6 +233,7 @@ class TrainEngine(object):
         self.tables = {}
         self.dense = None
         self.step_times = []
+        self._check_joint_clip(sync)
         self._build()
         self._consistency_check()
         self._start_aux()
@@ -290,11 +291,54 @@ class TrainEngine(object):
             if g.trainable():
                 self.dense = HostDenseGroup(dense_named, g.optimizer, comm,
                                             self.route, g)
+                self._link_joint_tables()
         elif self.backend == "nvlink":
             from .nvlink_backend import build_nvlink
             build_nvlink(self)
         else:
             raise ValueError("unknown fabric %r" % self.backend)
+
+    def _link_joint_tables(self):
+        """Host / library fabric: hand the tables of `include_sparse` clip rules to the
+        dense group, which applies them once the rule's norm is known."""
+        self.dense.joint_tables = [t.t for t in self._table_order() if t.clip_rule >= 0]
+
+    def _check_joint_clip(self, sync):
+        """Refuse at build what a `ClipByGlobalNorm(include_sparse=True)` cannot mean."""
+        g = self.graph
+        if not any(r.include_sparse for r in g.clip_rules()):
+            return
+        if not sync:
+            raise ValueError(
+                "ClipByGlobalNorm(include_sparse=True) needs sync=True: an asynchronous "
+                "PS has no aggregated sparse gradient to take the norm of")
+        if self.backend == "nvlink" and \
+                self.config.communication_config.ps_config.protocol == "nccl":
+            raise NotImplementedError(
+                "ClipByGlobalNorm(include_sparse=True) is not implemented for "
+                "PSConfig(protocol='nccl') on the NVLink fabric; use "
+                "sess_config={'fabric': 'library'} (or 'host') for a joint clip over "
+                "library collectives")
+        opts = self.config.sess_config if isinstance(self.config.sess_config, dict) else {}
+        declared = list(opts.get("sparse_groups") or
+                        getattr(self.model, "co_lookup_groups", None) or [])
+        known = set(self.analysis.sparse_modules)
+        for paths in declared:
+            paths = [p for p in paths if p in known]
+            rules = {g.joint_clip_index(p + ".weight" if p else "weight") for p in paths}
+            if len(rules) > 1:
+                raise ValueError(
+                    "co-lookup group %s: its tables must all be clipped by the same "
+                    "ClipByGlobalNorm(include_sparse=True) rule or all by none" % paths)
+
+    def grad_norm(self, i):
+        """Pre-clip global norm of clip rule `i` (index in the graph's
+        `ClipByGlobalNorm` rules) from the last completed step, as a float."""
+        rule = self.graph.clip_rules()[i]
+        if self.backend in ("host", "library"):
+            return float(self.dense.last_grad_norm.get(id(rule), 0.0))
+        st = self.dense.clip_state.get(i) if self.dense is not None else None
+        return float(st.norm.item()) if st is not None else 0.0
 
     def _start_aux(self):
         """Timeline, stall watchdog and autotuner (SURVEY §5.1, §5.3)."""
@@ -633,6 +677,8 @@ class TrainEngine(object):
                 self.tables[name] = new
                 if holder is not None:
                     holder.table = new
+            if self.dense is not None:
+                self._link_joint_tables()
         # captured graphs hold the old tables; the new ones allocate their rings
         # lazily, so run a few eager steps before capturing again
         self._graph_state = None
@@ -678,6 +724,8 @@ class TrainEngine(object):
                 ng.capacity_hint = ng.capacity_hint or cap
             new_groups.append(ng)
         self.sparse_groups = new_groups
+        if self.dense is not None:
+            self.dense.link_groups(new_groups)
 
     # ------------------------------------------------------------ reporting
     def export_report(self, path):

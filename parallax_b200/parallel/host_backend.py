@@ -50,6 +50,9 @@ class HostDenseGroup(object):
                 if self.ema_rule.applies_to(n):
                     self.ema[i] = self.master[i].clone()
         self.last_grad_norm = {}
+        # sparse tables clipped jointly with dense variables (`HostSparseTable.clip_rule`):
+        # aggregated before this group's step, applied by `_clip` with the rule's scale
+        self.joint_tables = []
         # make every replica start from rank 0's values
         # (reference `mpi/runner.py:134-139` broadcast of global variables)
         for m, p in zip(self.master, self.params):
@@ -86,7 +89,7 @@ class HostDenseGroup(object):
                     n = g.numel()
                     grads[i] = flat[off:off + n].view_as(g)
                     off += n
-            self._clip(grads)
+            self._clip(grads, step)
             for i, g in enumerate(grads):
                 _optim.apply_dense_(kind, self.master[i], g, self.slots[i], hp)
         else:
@@ -108,18 +111,37 @@ class HostDenseGroup(object):
                 p.copy_(m.to(p.dtype))
         self.zero_grad()
 
-    def _clip(self, grads):
-        for rule in self.graph.clip_rules():
+    def _clip(self, grads, step=None):
+        for ri, rule in enumerate(self.graph.clip_rules()):
             idx = [i for i, n in enumerate(self.names) if rule.applies_to(n)]
-            if not idx:
+            tabs = [t for t in self.joint_tables if t.clip_rule == ri]
+            if not idx and not tabs:
                 continue
             sq = sum(float((grads[i] ** 2).sum()) for i in idx)
+            if tabs:
+                sq += self._sparse_sumsq(tabs)
             norm = sq ** 0.5
             self.last_grad_norm[id(rule)] = norm
             scale = rule.max_norm / max(norm, rule.max_norm)
             if scale < 1.0:
                 for i in idx:
                     grads[i] = grads[i] * scale
+            for t in tabs:
+                t.apply(step, scale)
+
+    def _sparse_sumsq(self, tabs):
+        """Σg² of the merged rows of `tabs` over the whole job.  The dense Σ is taken
+        from the all-reduced gradients, identical on every rank, so only the sparse
+        part is summed: the owners' shares of partitioned tables with one
+        all-reduce; a replicated table was merged in full on every rank and counts
+        once."""
+        part = sum(t.sumsq() for t in tabs if not t.replicated)
+        rep = sum(t.sumsq() for t in tabs if t.replicated)
+        if self.comm.world > 1 and any(not t.replicated for t in tabs):
+            buf = torch.tensor([part], dtype=torch.float64, device=tabs[0].device)
+            self.comm.all_reduce_sum_(buf)
+            part = float(buf[0])
+        return part + rep
 
     # -- checkpoint -----------------------------------------------------------
     def state_dict(self):
@@ -165,6 +187,8 @@ class HostSparseTable(object):
         self.local_aggregation = bool(
             config.communication_config.ps_config.local_aggregation)
         self.scale = graph.scale_for(name)
+        self.clip_rule = graph.joint_clip_index(name)
+        self.merged = []
         L = self.layout
         shard = torch.zeros(L.rows_local, self.D, dtype=torch.float32)
         g, l = L.global_ids_of_owner(comm.rank)
@@ -206,6 +230,17 @@ class HostSparseTable(object):
 
     # -- backward / update ------------------------------------------------------
     def finish_step(self, step):
+        """Aggregate and apply; a table clipped jointly with other variables
+        (`clip_rule` >= 0) only aggregates here and is applied by the dense group
+        once the rule's norm is known."""
+        self.aggregate(step)
+        if self.clip_rule < 0:
+            self.apply(step)
+
+    def aggregate(self, step):
+        """All-to-all (or all-gather) of this step's rows and the duplicate merge on
+        the owner.  Keeps the owner's (local rows, merged gradient) segments for
+        `apply`."""
         L, W, me = self.layout, self.comm.world, self.comm.rank
         if self.pending:
             ids = torch.cat([p[0] for p in self.pending])
@@ -223,8 +258,6 @@ class HostSparseTable(object):
             agg.index_add_(0, inv, rows)
             rows = agg
         self.stats["unique_rows"] += int(ids.numel())
-        hp = self.optimizer.hyper(step)
-        kind = self.optimizer.kind
         if self.replicated:
             # AR run option (Horovod semantics): all-gather of indices and values,
             # every replica applies the full update
@@ -246,14 +279,28 @@ class HostSparseTable(object):
                 for n in rc:
                     segs.append((ids_c[off:off + n], rows_c[off:off + n]))
                     off += n
+        self.merged = []
         for seg_ids, seg_rows in segs:
             u, inv = torch.unique(seg_ids, return_inverse=True)
             g = torch.zeros(u.numel(), self.D, device=self.device)
             g.index_add_(0, inv, seg_rows)
             if self.average and self.route.sync:
                 g.div_(W)
-            _optim.apply_sparse_rows_(kind, self.shard, L.local_row_of(u), g,
+            self.merged.append((L.local_row_of(u), g))
+
+    def sumsq(self):
+        """Σg² (float64) over the merged rows of the last `aggregate` held here."""
+        return sum(float((g.double() ** 2).sum()) for _, g in self.merged)
+
+    def apply(self, step, scale=1.0):
+        """The optimizer on the segments of the last `aggregate`, gradient × `scale`."""
+        hp = self.optimizer.hyper(step)
+        for rows, g in self.merged:
+            if scale != 1.0:
+                g = g * scale
+            _optim.apply_sparse_rows_(self.optimizer.kind, self.shard, rows, g,
                                       self.slots, hp)
+        self.merged = []
 
     # -- checkpoint / inspection -------------------------------------------------
     def _gather_full(self, local):

@@ -375,6 +375,10 @@ class NVSparseGroup(object):
         self._done_step = -1
         self._last_n = 1
         self._row_cnt = None
+        # ClipByGlobalNorm(include_sparse=True): (dense group, clip state) of the rule this
+        # group contributes to, and the group's private hyper-parameters for the clipped apply
+        self.joint_clip = None
+        self.hp_clip = None
         NVSparseGroup._seq += 1
 
     # ---------------------------------------------------------------- forward
@@ -680,13 +684,21 @@ class NVSparseGroup(object):
             cs = stream if stream is not None else self.fabric.comm_stream
             with timeline.activity(self.name, "SPARSE_PUSH_APPLY", gpu=True, stream=cs,
                                    args="rows=%d" % sum(c[0].numel() for c in self.calls)):
-                self.stage_push(step, stream)
-                if self.route.sync:
-                    self.stage_apply(step, stream)
+                self._push_then_apply(step, stream)
         else:
-            self.stage_push(step, stream)
-            if self.route.sync:
-                self.stage_apply(step, stream)
+            self._push_then_apply(step, stream)
+
+    def _push_then_apply(self, step, stream):
+        self.stage_push(step, stream)
+        if self.joint_clip is not None:
+            # the apply waits for the rule's norm: the dense group issues it after the
+            # rule's last contributor (`NVDenseGroup.contributed`)
+            dense, st = self.joint_clip
+            cs = stream if stream is not None else self.fabric.comm_stream
+            self.stage_norm(st.local if self.norm_counts() else None, cs)
+            dense.contributed(st, cs)
+        elif self.route.sync:
+            self.stage_apply(step, stream)
 
     def _take_calls(self):
         """Pending ids and per-table gradient rows of this step's lookups, concatenated,
@@ -756,9 +768,11 @@ class NVSparseGroup(object):
             ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
             1 if self.local_aggregation else 0, self.max_blocks, _sp(cs)), "sparse_push")
 
-    def _owner_tables(self, rings, sender_scaled):
+    def _owner_tables(self, rings, sender_scaled, hp=None):
         """OwnerTable per member table, merging the rows at device address rings[i]; the
-        owner applies the ScaleGradients factor unless the sender did (`sender_scaled`)."""
+        owner applies the ScaleGradients factor unless the sender did (`sender_scaled`).
+        `hp`: the device hyper-parameter vector to use instead of the shared one."""
+        hp_ptr = (hp if hp is not None else self.hp.dev).data_ptr()
         descs = (ops.OwnerTable * len(self.tables))()
         for d, t, ring in zip(descs, self.tables, rings):
             d.ring, d.table = ring, t.table.data_ptr()
@@ -766,24 +780,31 @@ class NVSparseGroup(object):
             d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
             d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
             d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
-            d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
+            d.hp, d.D4, d.kind = hp_ptr, t.D4, _optim.KIND_ID[t.kind]
             avg = (1.0 / self.world) if t.average else 1.0
             d.avg = avg if sender_scaled else avg * t.scale
         return descs
 
-    def stage_apply(self, step, stream=None):
-        """Owner side, one kernel: merge rows from all sources, apply the optimizer."""
-        cs = stream if stream is not None else self.fabric.comm_stream
+    def _owner_blocks(self):
         n = max(self._last_n, 1)
         # 16 half-warps per CTA, one entry per half-warp: as many CTAs as fit on the device at once
         # (4 per SM at 64 registers; the merge variant is a cooperative launch)
-        blocks = max(1, min(max(self.max_blocks, consts.NUM_SMS * 4)
-                            if self.max_blocks >= consts.NUM_SMS
-                            else self.max_blocks,
-                            (n * (self.world if self.replicated else 1) + 15) // 16))
-        use_merge = self.world > 1 or not self.local_aggregation
+        return max(1, min(max(self.max_blocks, consts.NUM_SMS * 4)
+                          if self.max_blocks >= consts.NUM_SMS
+                          else self.max_blocks,
+                          (n * (self.world if self.replicated else 1) + 15) // 16))
+
+    def _use_merge(self):
+        return self.world > 1 or not self.local_aggregation
+
+    def stage_apply(self, step, stream=None, hp=None):
+        """Owner side, one kernel: merge rows from all sources, apply the optimizer
+        (with the hyper-parameter vector `hp` instead of the shared one when given)."""
+        cs = stream if stream is not None else self.fabric.comm_stream
+        blocks = self._owner_blocks()
+        use_merge = self._use_merge()
         descs = self._owner_tables([t.ring_buf.local_ptr for t in self.tables],
-                                   sender_scaled=self.boundary)
+                                   sender_scaled=self.boundary, hp=hp)
         self._keep_o = descs
         _count()
         ops.check(ops.lib().px_sparse_owner(
@@ -792,6 +813,38 @@ class NVSparseGroup(object):
             _vp(self.slotmap.data_ptr()), _vp(self.next.data_ptr()), self.cap,
             ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
             1 if use_merge else 0, blocks, -1, _sp(cs)), "sparse_owner")
+
+    def norm_counts(self):
+        """Whether this rank's `stage_norm` adds to the global norm: every owner of a
+        partitioned group, only rank 0 of a replicated one (every replica merges every row)."""
+        return not self.replicated or self.rank == 0
+
+    def stage_norm(self, sumsq, stream=None):
+        """Owner side, after `stage_push` and before `stage_apply`: add to the fp32 device
+        scalar `sumsq` the squared norm of the rows `stage_apply` will hand to the optimizer
+        (merged over sources, × average × ScaleGradients × hp[HP_GSCALE]).  Nothing is
+        launched when `sumsq` is None."""
+        if sumsq is None:
+            return
+        cs = stream if stream is not None else self.fabric.comm_stream
+        descs = self._owner_tables([t.ring_buf.local_ptr for t in self.tables],
+                                   sender_scaled=self.boundary)
+        self._keep_nrm = descs
+        _count()
+        ops.check(ops.lib().px_sparse_owner_norm(
+            descs, len(self.tables), _DT[self.wire_dtype], _vp(self.ids_buf.local_ptr),
+            _vp(self.hdr_buf.local_ptr), _vp(self.slotmap.data_ptr()),
+            _vp(self.next.data_ptr()), self.cap, ctypes.byref(self.geom),
+            _vp(self.ctl.data_ptr()), 1 if self._use_merge() else 0, self._owner_blocks(),
+            _vp(sumsq.data_ptr()), _sp(cs)), "sparse_owner_norm")
+
+    def clip_hp(self, scale, stream=None):
+        """The group's private hyper-parameters for a clipped apply: the shared vector with
+        hp[HP_GSCALE] × the device scalar `scale`."""
+        from . import nvops
+        nvops.clip_hp(self.hp.dev, scale, self.hp_clip,
+                      stream if stream is not None else self.fabric.comm_stream)
+        return self.hp_clip
 
     # ---------------------------------------------------------------- inspection
     def device_times(self):

@@ -78,8 +78,9 @@ class _Bucket(object):
 
 class NVDenseGroup(object):
     def __init__(self, named_params, optimizer, fabric, route, graph,
-                 options=None):
+                 options=None, sparse_groups=()):
         self.fabric, self.route, self.graph = fabric, route, graph
+        self.sparse_groups = list(sparse_groups)
         self.optimizer = optimizer
         self.heap = fabric.heap
         self.rank, self.world = fabric.rank, fabric.world
@@ -214,16 +215,34 @@ class NVDenseGroup(object):
             torch.cuda.synchronize(self.device)
         for b in buckets:
             self._alloc_state(b)
-        # clip-rule scalars
+        # clip-rule scalars.  A rule's contributors are its dense buckets and, with
+        # include_sparse, the sparse groups whose tables it matches; the norm is complete,
+        # and the rule's updates are issued, once the last of them has been enqueued
         self.clip_state = {}
-        for ci in sorted({b.clip for b in buckets if b.clip >= 0}):
+        joint = {self.graph.joint_clip_index(grp.tables[0].name) for grp in self.sparse_groups}
+        for ci in sorted({b.clip for b in buckets if b.clip >= 0} | (joint - {-1})):
             st = _Bucket()
+            st.index = ci
             st.local = torch.zeros(4, dtype=torch.float32, device=self.device)
             st.total = torch.zeros(4, dtype=torch.float32, device=self.device)
             st.scale = torch.ones(1, dtype=torch.float32, device=self.device)
             st.norm = torch.zeros(1, dtype=torch.float32, device=self.device)
             st.buckets = [b for b in buckets if b.clip == ci]
             self.clip_state[ci] = st
+        self.link_groups(self.sparse_groups)
+
+    def link_groups(self, groups):
+        """Attach the sparse groups of `include_sparse` clip rules to their rule's state
+        (at build, and again when re-partitioning replaced the groups)."""
+        self.sparse_groups = list(groups)
+        for ci, st in self.clip_state.items():
+            st.groups = sorted((grp for grp in groups
+                                if self.graph.joint_clip_index(grp.tables[0].name) == ci),
+                               key=lambda grp: grp.name)
+            st.left = len(st.buckets) + len(st.groups)
+            for grp in st.groups:
+                grp.joint_clip = (self, st)
+                grp.hp_clip = torch.zeros_like(grp.hp.dev)
 
     def _alloc_state(self, b):
         W, dev = self.world, self.device
@@ -365,18 +384,7 @@ class NVDenseGroup(object):
                                  st.local, b.n, 1.0 / W, ema_decay, self.kind,
                                  MODE_REDUCE, b.dtype, CH_COMM, max_blocks=mb,
                                  stream=cs, use_mc=b.mc, slot2=s2)
-                if b is st.buckets[-1]:
-                    self._finish_clip(st, cs)
-                    for bb in st.buckets:
-                        t0 = bb.slots[0] if self.nslots > 0 else None
-                        t1 = bb.slots[1] if self.nslots > 1 else None
-                        t2 = bb.slots[2] if self.nslots > 2 else None
-                        nvops.dense_step(heap, self._grad_sources(bb),
-                                         self._param_targets(bb), bb.master, t0, t1,
-                                         bb.ema, bb.red, self.hp, st.scale, None,
-                                         bb.n, 1.0 / W, ema_decay, self.kind,
-                                         MODE_UPDATE, bb.dtype, CH_COMM,
-                                         max_blocks=mb, stream=cs, use_mc=bb.mc, slot2=t2)
+                self.contributed(st, cs)
         elif self.update == "replicated":
             # classic AR: all-reduce (mean) then every replica updates itself
             if self.protocol == "nccl" and W > 1:
@@ -396,10 +404,8 @@ class NVDenseGroup(object):
                                         max_blocks=mb, stream=cs)
             if st is None:
                 self._local_update(b, None, cs)
-            elif b is st.buckets[-1]:
-                self._finish_clip(st, cs)
-                for bb in st.buckets:
-                    self._local_update(bb, st.scale, cs)
+            else:
+                self.contributed(st, cs)
         else:  # async PS
             clip = None
             if st is not None:
@@ -430,8 +436,38 @@ class NVDenseGroup(object):
             b._self_targets = arr
         return arr
 
+    def contributed(self, st, cs):
+        """One contributor of clip rule `st` (a dense bucket's Σg² reduction or a sparse
+        group's `stage_norm`) has been enqueued on `cs`.  After the last one: the global
+        norm and scale, each group's clipped hyper-parameters, the rule's dense updates,
+        then the groups' deferred owner kernels in name order — the same order on every
+        rank, since the contributors arrive in autograd order."""
+        st.left -= 1
+        if st.left:
+            return
+        st.left = len(st.buckets) + len(st.groups)
+        self._finish_clip(st, cs)
+        hps = [grp.clip_hp(st.scale, cs) for grp in st.groups]
+        W, mb = self.world, self.fabric.dense_blocks
+        ema_decay = self.ema_rule.decay if self.ema_rule is not None else 0.0
+        for bb in st.buckets:
+            if self.update == "sharded":
+                t0 = bb.slots[0] if self.nslots > 0 else None
+                t1 = bb.slots[1] if self.nslots > 1 else None
+                t2 = bb.slots[2] if self.nslots > 2 else None
+                nvops.dense_step(self.heap, self._grad_sources(bb),
+                                 self._param_targets(bb), bb.master, t0, t1,
+                                 bb.ema, bb.red, self.hp, st.scale, None,
+                                 bb.n, 1.0 / W, ema_decay, self.kind,
+                                 MODE_UPDATE, bb.dtype, CH_COMM,
+                                 max_blocks=mb, stream=cs, use_mc=bb.mc, slot2=t2)
+            else:
+                self._local_update(bb, st.scale, cs)
+        for grp, hp in zip(st.groups, hps):
+            grp.stage_apply(grp._cur_step, cs, hp=hp)
+
     def _finish_clip(self, st, cs):
-        rule = self.clip_rules[st.buckets[0].clip]
+        rule = self.clip_rules[st.index]
         if self.world > 1:
             nvops.allreduce_oneshot(self.heap, st.local, st.total,
                                     self.fabric.small_stage, 4, torch.float32,
@@ -644,9 +680,10 @@ def build_nvlink(engine):
                 b.data = b.data.to(cdt)
     dense_named = [(n, p) for n, p in engine.model.named_parameters()
                    if p.requires_grad and not getattr(p, "_parallax_skip", False)]
-    if g.trainable() and dense_named:
+    joint = any(r.include_sparse for r in g.clip_rules())
+    if g.trainable() and (dense_named or joint):
         engine.dense = NVDenseGroup(dense_named, g.optimizer, fabric, engine.route,
-                                    g, options=opts)
+                                    g, options=opts, sparse_groups=engine.sparse_groups)
     torch.cuda.synchronize(dev)
     parallax_log.info(
         "nvlink fabric: rank %d/%d, %d dense buckets, %d sparse tables, "

@@ -103,6 +103,13 @@ def clip_scale(sumsq_total, max_norm, scale_out, norm_out, zero_after, stream=No
               "clip_scale")
 
 
+def clip_hp(hp, scale, out, stream=None):
+    """out = hp with out[HP_GSCALE] multiplied by the device scalar `scale`."""
+    L = ops.lib()
+    _count()
+    ops.check(L.px_clip_hp(_p(hp), _p(scale), _p(out), _s(stream)), "clip_hp")
+
+
 def dense_async(my_grads, my_params, master_c, slot0_c, slot1_c, hp, clip, n,
                 kind, dtype, rank, world, max_blocks=64, stream=None, slot2_c=None):
     L = ops.lib()
