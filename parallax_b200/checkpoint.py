@@ -74,7 +74,8 @@ def save_sharded(engine, path, is_chief):
         writers = [0] if t.replicated else list(range(comm.world))
         files = ["sparse-%s-rank%d.pt" % (_safe(name), r) for r in writers]
         manifest["sparse"][name] = {
-            "V": t.V, "D": t.D, "nslots": t.nslots, "files": files,
+            "V": t.V, "D": t.D, "nslots": t.nslots, "slot_dim": _table_slot_dim(t),
+            "files": files,
             "placement": [t.layout.P, t.layout.strategy, t.layout.world, t.layout.owners,
                           bool(t.replicated)]}
         if comm.rank in writers:
@@ -116,6 +117,10 @@ def load_sharded(engine, path):
         if ent["V"] != t.V or ent["D"] != t.D:
             raise RuntimeError("checkpoint variable %r has shape (%d, %d), the model (%d, %d)"
                                % (name, ent["V"], ent["D"], t.V, t.D))
+        if t.nslots and int(ent["nslots"]) and _slot_dim(ent) != _table_slot_dim(t):
+            raise ValueError("checkpoint variable %r has slots of width %d, but its optimizer "
+                             "keeps slots of width %d" % (name, _slot_dim(ent),
+                                                          _table_slot_dim(t)))
         same = ent["placement"] == [t.layout.P, t.layout.strategy, t.layout.world,
                                     t.layout.owners, bool(t.replicated)]
         files = ent["files"]
@@ -171,10 +176,23 @@ def read_manifest(path):
         return json.load(f)
 
 
+def _table_slot_dim(t):
+    """Columns of each slot of table `t`: its `slot_dim` (1 for a row-wise optimizer), or D
+    for a table that does not declare one."""
+    return int(getattr(t, "slot_dim", t.D))
+
+
+def _slot_dim(ent):
+    """Columns of each slot of a manifest entry: D, or 1 for a row-wise optimizer (manifests
+    written before row-wise optimizers existed have no "slot_dim": their slots are D wide)."""
+    return int(ent.get("slot_dim", ent["D"]))
+
+
 def assemble_table(path, name, manifest=None):
     """One sparse variable of a sharded checkpoint as full logical tensors
-    ``{"weight": [V, D], "slots": [[V, D], ...]}`` — no engine, no GPU: what an offline tool
-    (`tools/inspect_checkpoint`, an evaluation script on another machine) needs."""
+    ``{"weight": [V, D], "slots": [[V, D] or [V, 1] (row-wise), ...]}`` — no engine, no GPU:
+    what an offline tool (`tools/inspect_checkpoint`, an evaluation script on another
+    machine) needs."""
     man = manifest or read_manifest(path)
     ent = man["sparse"][name]
     V, D, ns = int(ent["V"]), int(ent["D"]), int(ent["nslots"])
@@ -183,7 +201,7 @@ def assemble_table(path, name, manifest=None):
         sh = torch.load(os.path.join(path, fn), map_location="cpu", weights_only=False)
         if w is None:
             w = torch.zeros(V, D, dtype=sh["weight"].dtype)
-            slots = [torch.zeros(V, D, dtype=s_.dtype) for s_ in sh["slots"][:ns]]
+            slots = [torch.zeros(V, _slot_dim(ent), dtype=s_.dtype) for s_ in sh["slots"][:ns]]
         w[sh["ids"]] = sh["weight"]
         for dst, src in zip(slots, sh["slots"]):
             dst[sh["ids"]] = src
@@ -203,7 +221,7 @@ def assemble_sharded(path, max_table_bytes=None):
     sd = {"global_step": int(d["global_step"]), "dense": d.get("dense"),
           "buffers": d.get("buffers", {}), "sparse": {}, "skipped": []}
     for name, ent in sorted(man["sparse"].items()):
-        nbytes = int(ent["V"]) * int(ent["D"]) * 4 * (1 + int(ent["nslots"]))
+        nbytes = int(ent["V"]) * 4 * (int(ent["D"]) + int(ent["nslots"]) * _slot_dim(ent))
         if max_table_bytes is not None and nbytes > max_table_bytes:
             sd["skipped"].append(name)
             continue

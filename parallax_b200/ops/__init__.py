@@ -41,7 +41,8 @@ class PushTable(ctypes.Structure):
 class OwnerTable(ctypes.Structure):
     _fields_ = [("ring", c_void_p), ("table", c_void_p), ("slot0", c_void_p),
                 ("slot1", c_void_p), ("slot2", c_void_p), ("shadow", c_void_p),
-                ("hp", c_void_p), ("D4", c_int), ("kind", c_int), ("avg", c_float)]
+                ("hp", c_void_p), ("D4", c_int), ("kind", c_int), ("avg", c_float),
+                ("D", c_int)]
 
 
 _SIGS = {

@@ -8,16 +8,20 @@
 //   family 0: sgd, momentum(+nesterov), adagrad, adam, rmsprop          (<= 2 slots)
 //   family 1: adadelta, ftrl, proximal sgd, proximal adagrad, adagrad-DA, centered rmsprop
 //             (<= 3 slots; needs l1/l2/lr_power and the global step)
-// Numerics oracle: `parallax_b200/optim.py::apply_dense_`.
+//   family 2: row-wise adagrad — one accumulator per table row, fed by the row's mean g²;
+//             sparse owner kernel only (`px_sparse_owner_kernel<.., 2>` in sparse.cu), since
+//             the rule needs the whole row before it can update any element of it
+// Numerics oracle: `parallax_b200/optim.py::apply_dense_` / `apply_sparse_rows_`.
 #pragma once
 #include <cuda_runtime.h>
 
 enum {
   PX_SGD = 0, PX_MOMENTUM = 1, PX_ADAGRAD = 2, PX_ADAM = 3, PX_RMSPROP = 4,
   PX_ADADELTA = 5, PX_FTRL = 6, PX_PROX_SGD = 7, PX_PROX_ADAGRAD = 8, PX_ADAGRAD_DA = 9,
-  PX_CENTERED_RMSPROP = 10
+  PX_CENTERED_RMSPROP = 10, PX_ROWWISE_ADAGRAD = 11
 };
-#define PX_KIND_FAMILY(kind) ((kind) <= PX_RMSPROP ? 0 : 1)
+#define PX_KIND_FAMILY(kind) \
+  ((kind) <= PX_RMSPROP ? 0 : (kind) <= PX_CENTERED_RMSPROP ? 1 : 2)
 
 // device hyper-parameter vector (8 floats), see optim.py
 enum { HP_LR = 0, HP_A, HP_B, HP_EPS, HP_WD, HP_STEP, HP_GSCALE, HP_FLAGS };

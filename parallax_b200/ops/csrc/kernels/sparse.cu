@@ -635,6 +635,8 @@ struct OwnerTable {
   const float* hp;
   int D4, kind;
   float avg;                    // 1/num_workers (average_sparse) × owner-side gradient scale
+  int D;                        // true row width, read by family 2 only (the row-wise rule
+                                // averages Σg² over it); fills the 8-byte alignment tail
 };
 struct OwnerArgs {
   OwnerTable t[PX_GRP_MAX];
@@ -648,6 +650,109 @@ struct OwnerArgs {
   int fixed_cnt;                // >= 0: library-collective arm — every source delivered exactly this
                                 // many entries (negative row id = not mine), no flags involved
 };
+
+// Σ over the entries linked from list head e of one 4-element group of a wire row, in fp32
+template <typename WireT>
+__device__ __forceinline__ float4 ld_merged4(const OwnerArgs& a, const char* ring,
+                                             size_t row_bytes, int e, int c) {
+  float4 g = ld_wire4<WireT>(ring + (size_t)e * row_bytes, c);
+  if (a.use_merge) {
+    for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
+      const float4 o = ld_wire4<WireT>(ring + (size_t)x * row_bytes, c);
+      g.x += o.x; g.y += o.y; g.z += o.z; g.w += o.w;
+    }
+  }
+  return g;
+}
+
+// Family 2 (row-wise Adagrad) on local row r of table T, by the 16 lanes of one half-warp:
+//   s[r] += (1/D) Σ_j g_j²        (T.slot0 is a dense [rows_local] fp32 array)
+//   w[r, j] -= lr · g_j / (sqrt(s[r]) + eps)
+// Pass 1 merges and scales the row and reduces Σg² over the 16 lanes; pass 2 updates the
+// row.  Rows of up to PX_RW_REG_F4 · 64 columns keep their gradient and master values in
+// registers from pass 1 (every load of the row, and lane 0's load of s[r], is then in flight
+// at once); wider rows merge the gradient again from the ring in pass 2 (pass 1 just brought
+// it into L2).  Padding columns carry zero gradient and stay unchanged.
+#define PX_RW_REG_F4 2
+
+__device__ __forceinline__ void px_store_row4(const OwnerTable& T, size_t row, int c,
+                                              const float4& w) {
+  reinterpret_cast<float4*>(T.table)[row * T.D4 + c] = w;
+  if (T.shadow) {
+    __nv_bfloat162 lo = __floats2bfloat162_rn(w.x, w.y), hi = __floats2bfloat162_rn(w.z, w.w);
+    *reinterpret_cast<uint2*>(reinterpret_cast<char*>(T.shadow) +
+                              (row * ((T.D4 + 1) / 2 * 2) + c) * 8) =
+        make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+  }
+}
+
+__device__ __forceinline__ void px_sgd4(float step, const float4& g, float4& w) {
+  w.x = fmaf(-step, g.x, w.x); w.y = fmaf(-step, g.y, w.y);
+  w.z = fmaf(-step, g.z, w.z); w.w = fmaf(-step, g.w, w.w);
+}
+
+template <typename WireT>
+__device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const OwnerTable& T, int e,
+                                                 int r, int lane, unsigned hmask) {
+  const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
+  const float gmul = T.avg * T.hp[HP_GSCALE];
+  const float s_old = lane == 0 ? T.slot0[r] : 0.f;
+  const bool in_regs = T.D4 <= 16 * PX_RW_REG_F4;
+  const float4* wrow = reinterpret_cast<const float4*>(T.table) + (size_t)r * T.D4;
+  float4 gk[PX_RW_REG_F4], wk[PX_RW_REG_F4];
+  float ss = 0.f;
+  if (in_regs) {
+#pragma unroll
+    for (int k = 0; k < PX_RW_REG_F4; ++k) {
+      const int c = lane + 16 * k;
+      if (c < T.D4) {
+        wk[k] = wrow[c];
+        gk[k] = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < PX_RW_REG_F4; ++k) {
+      if (lane + 16 * k < T.D4) {
+        float4& g = gk[k];
+        g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
+        ss = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, fmaf(g.w, g.w, ss))));
+      }
+    }
+  } else {
+    for (int c = lane; c < T.D4; c += 16) {
+      float4 g = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+      g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
+      ss = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, fmaf(g.w, g.w, ss))));
+    }
+  }
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) ss += __shfl_xor_sync(hmask, ss, o);
+  float s = 0.f;
+  if (lane == 0) {
+    s = s_old + ss / (float)T.D;
+    T.slot0[r] = s;
+  }
+  s = __shfl_sync(hmask, s, threadIdx.x & 16);
+  const float step = T.hp[HP_LR] / (sqrtf(s) + T.hp[HP_EPS]);
+  if (in_regs) {
+#pragma unroll
+    for (int k = 0; k < PX_RW_REG_F4; ++k) {
+      const int c = lane + 16 * k;
+      if (c < T.D4) {
+        px_sgd4(step, gk[k], wk[k]);
+        px_store_row4(T, (size_t)r, c, wk[k]);
+      }
+    }
+  } else {
+    for (int c = lane; c < T.D4; c += 16) {
+      float4 g = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+      g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
+      float4 w = wrow[c];
+      px_sgd4(step, g, w);
+      px_store_row4(T, (size_t)r, c, w);
+    }
+  }
+}
 
 // One warp that waits for every source's `pushed` flag.  Launched right before the owner kernel
 // on the comm stream: the owner's (cooperative, whole-GPU) grid then starts with its inputs
@@ -665,7 +770,7 @@ __global__ void px_sparse_wait_kernel(const uint32_t* hdr, const SparseCtl* ctl,
 // optimizer once per touched row, publish `applied`.  Launched cooperatively when use_merge (one
 // grid barrier between linking and applying).
 template <typename WireT, int FAM>
-__global__ void __launch_bounds__(256, FAM == 0 ? 4 : 2)
+__global__ void __launch_bounds__(256, FAM == 1 ? 2 : 4)
 px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
   __shared__ bool s_last;
   const bool stamp = blockIdx.x == 0 && threadIdx.x == 0;
@@ -740,6 +845,12 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
               const int lines = (T.D4 * 16 + 127) / 128;
               for (int l = lane; l < lines; l += 16) {
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) + off + l * 128));
+                if (FAM == 2) {
+                  // one fp32 accumulator per row: its pitch is 4 bytes, not the row's
+                  if (l == 0)
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(T.slot0 + rn));
+                  continue;
+                }
                 if (T.slot0)
                   asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.slot0) + off + l * 128));
                 if (T.slot1)
@@ -756,6 +867,10 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
 #pragma unroll 1
       for (int t = 0; t < a.nt; ++t) {
         const OwnerTable& T = a.t[t];
+        if (FAM == 2) {
+          px_rowwise_apply<WireT>(a, T, e, r, lane, hmask);
+          continue;
+        }
         const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
         const float gmul = T.avg * T.hp[HP_GSCALE];
         const PxHP hp = px_load_hp(T.hp);
@@ -863,6 +978,7 @@ const char* px_sparse_abi() {
     SIZE(OwnerTable); FIELD(OwnerTable, ring); FIELD(OwnerTable, table); FIELD(OwnerTable, slot0);
     FIELD(OwnerTable, slot1); FIELD(OwnerTable, slot2); FIELD(OwnerTable, shadow);
     FIELD(OwnerTable, hp); FIELD(OwnerTable, D4); FIELD(OwnerTable, kind); FIELD(OwnerTable, avg);
+    FIELD(OwnerTable, D);
 #undef SIZE
 #undef FIELD
     return s;
@@ -932,6 +1048,7 @@ int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt
   const size_t smem = ((size_t)4 * sizeof(int32_t) << hbits) + 2 * PX_ID_CHUNK * sizeof(int32_t);
   SparseCtl* C = (SparseCtl*)ctl;
 #define PUSH(GT, WT, AS, FAM) launch_push<GT, WT, AS, FAM>(blocks, smem, stream, pend_ids, n, a, G, C, hbits, dedup)
+  if (async && fam == 2) return -7;             // row-wise rules need the merged row
   if (async) {
     if (grad_dtype == 0) { if (fam == 0) PUSH(float, float, true, 0); else PUSH(float, float, true, 1); }
     else { if (fam == 0) PUSH(__nv_bfloat16, float, true, 0); else PUSH(__nv_bfloat16, float, true, 1); }
@@ -977,9 +1094,11 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
   SparseCtl* C = (SparseCtl*)ctl;
   const void* fn;
   if (wire_dtype == 0) fn = fam == 0 ? (const void*)px_sparse_owner_kernel<float, 0>
-                                     : (const void*)px_sparse_owner_kernel<float, 1>;
+                          : fam == 1 ? (const void*)px_sparse_owner_kernel<float, 1>
+                                     : (const void*)px_sparse_owner_kernel<float, 2>;
   else fn = fam == 0 ? (const void*)px_sparse_owner_kernel<__nv_bfloat16, 0>
-                     : (const void*)px_sparse_owner_kernel<__nv_bfloat16, 1>;
+          : fam == 1 ? (const void*)px_sparse_owner_kernel<__nv_bfloat16, 1>
+                     : (const void*)px_sparse_owner_kernel<__nv_bfloat16, 2>;
   void* args[] = {&a, &G, &C};
   cudaError_t e;
   if (use_merge) {

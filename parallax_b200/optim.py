@@ -21,6 +21,8 @@ Update rules (g = aggregated gradient):
 * adam     : m = β₁m+(1-β₁)g ; v = β₂v+(1-β₂)g² ;
              w -= lr·sqrt(1-β₂ᵗ)/(1-β₁ᵗ) · m/(sqrt(v)+ε)
 * rmsprop  : ms = ρ·ms+(1-ρ)g² ; mom = μ·mom + lr·g/sqrt(ms+ε) ; w -= mom
+* rowwise_adagrad (sparse variables only): one accumulator per row,
+             s += mean_j(g_j²) ; w -= lr·g / (sqrt(s) + ε)
 
 Sparse variants touch only the rows present in the aggregated gradient
 ("lazy" Adam/momentum, exactly like TF's sparse apply ops).
@@ -38,19 +40,50 @@ KINDS = ("sgd", "momentum", "adagrad", "adam", "rmsprop")
 EXT_KINDS = ("adadelta", "ftrl", "proximal_sgd", "proximal_adagrad", "adagrad_da",
              "centered_rmsprop")
 HOST_KINDS = EXT_KINDS            # historical name
-KIND_ID = {k: i for i, k in enumerate(KINDS + EXT_KINDS)}
+# family 2: rules that keep one fp32 slot value per table ROW (sparse variables only; the
+# sparse owner kernel merges a whole row before it applies it)
+ROWWISE_KINDS = ("rowwise_adagrad",)
+KIND_ID = {k: i for i, k in enumerate(KINDS + EXT_KINDS + ROWWISE_KINDS)}
 # number of fp32 state slots per kind
 NUM_SLOTS = {"sgd": 0, "momentum": 1, "adagrad": 1, "adam": 2, "rmsprop": 2,
              "adadelta": 2, "ftrl": 2, "proximal_sgd": 0, "proximal_adagrad": 1,
-             "adagrad_da": 2, "centered_rmsprop": 3}
+             "adagrad_da": 2, "centered_rmsprop": 3, "rowwise_adagrad": 1}
 SLOT_NAMES = {
     "sgd": (), "momentum": ("momentum",), "adagrad": ("accumulator",),
     "adam": ("m", "v"), "rmsprop": ("ms", "mom"),
     "adadelta": ("accum", "accum_update"), "ftrl": ("accum", "linear"), "proximal_sgd": (),
     "proximal_adagrad": ("accumulator",),
     "adagrad_da": ("gradient_accumulator", "gradient_squared_accumulator"),
-    "centered_rmsprop": ("ms", "mg", "mom"),
+    "centered_rmsprop": ("ms", "mg", "mom"), "rowwise_adagrad": ("accumulator",),
 }
+
+
+def kind_family(kind):
+    """Kernel template family of `kind` (`optim_rules.cuh`): 0, 1 or 2 (row-wise)."""
+    return 0 if kind in KINDS else 1 if kind in EXT_KINDS else 2
+
+
+def slot_width(kind, D):
+    """Columns of each state slot of a [V, D] variable: 1 for row-wise rules, else D."""
+    return 1 if kind in ROWWISE_KINDS else D
+
+
+def table_row_bytes(kind, D):
+    """Bytes one row of a sparse variable of width D takes on its owner: the fp32 master row
+    and the fp32 slots, every D-wide row padded to a multiple of 4 columns."""
+    Dp = (D + 3) // 4 * 4
+    return 4 * Dp + 4 * NUM_SLOTS[kind] * slot_width(kind, Dp)
+
+
+def check_table_slots(name, kind, V, D, slots):
+    """Raise ValueError unless every tensor of `slots` has the logical shape of a slot of
+    sparse variable `name` ([V, D], trained with `kind`): [V, D], or [V, 1] for a row-wise
+    rule — so that a checkpoint of another optimizer cannot be broadcast into the slots."""
+    want = (V, slot_width(kind, D))
+    for i, s in enumerate(slots):
+        if tuple(s.shape) != want:
+            raise ValueError("sparse variable %r: slot %d has shape %s, but its %s optimizer "
+                             "keeps slots of shape %s" % (name, i, tuple(s.shape), kind, want))
 
 
 def require_fused(kind, where):
@@ -236,6 +269,32 @@ class CenteredRMSProp(RMSProp):
     kind = "centered_rmsprop"
 
 
+class RowWiseAdagrad(Optimizer):
+    """Row-wise Adagrad for embedding tables (FBGEMM's ``EXACT_ROWWISE_ADAGRAD``): one fp32
+    accumulator per row instead of one per element.  For a row with aggregated gradient g
+    of the table's D columns::
+
+        s   += (1/D) · Σ_j g_j²
+        w_j -= lr · g_j / (sqrt(s) + epsilon)
+
+    Lazy like every sparse rule: rows without a gradient this step, and their accumulators,
+    are untouched.  With D = 1 it is Adagrad.  A *sparse-variable* optimizer: pass it as
+    ``Graph(..., sparse_optimizer=RowWiseAdagrad(...))``; the engine refuses it for dense
+    variables and with ``sync=False``."""
+    kind = "rowwise_adagrad"
+
+    def __init__(self, learning_rate, initial_accumulator_value=0.1, epsilon=0.0, **kw):
+        super().__init__(learning_rate, **kw)
+        self.initial_accumulator_value = float(initial_accumulator_value)
+        self.epsilon = float(epsilon)
+
+    def slot_init(self):
+        return (self.initial_accumulator_value,)
+
+    def _fill(self, hp, step):
+        hp[HP_EPS] = self.epsilon
+
+
 # TF-style aliases
 AdadeltaOptimizer = Adadelta
 FtrlOptimizer = Ftrl
@@ -320,6 +379,10 @@ def apply_dense_(kind, w, g, slots, hp):
         gg_acc.addcmul_(g, g)
         tmp = torch.sign(g_acc) * (g_acc.abs() - a * t).clamp(min=0.0) if a > 0 else g_acc
         w.copy_(-lr * tmp / (b * t * lr + gg_acc.sqrt()))
+    elif kind == "rowwise_adagrad":       # rows of w (dim 0); acc is [rows, 1]
+        (acc,) = slots
+        acc.add_((g * g).mean(dim=-1, keepdim=True))
+        w.addcdiv_(g, acc.sqrt().add_(eps), value=-lr)
     else:  # pragma: no cover
         raise ValueError(kind)
     return w

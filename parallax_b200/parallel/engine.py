@@ -25,7 +25,7 @@ import time
 import torch
 import torch.nn as tnn
 
-from .. import consts
+from .. import consts, optim as _optim
 from ..analyzer import analyze
 from ..log import parallax_log
 from . import modes
@@ -234,6 +234,7 @@ class TrainEngine(object):
         self.dense = None
         self.step_times = []
         self._check_joint_clip(sync)
+        self._check_rowwise(sync)
         self._build()
         self._consistency_check()
         self._start_aux()
@@ -260,14 +261,13 @@ class TrainEngine(object):
             # byte-greedy placement of every sparse variable's partitions on the owners — the
             # same rule as the NVLink fabric (`ps/between_graph_parallel.py:49-70`)
             from .layout import assign_owners
-            from .. import optim as _optim
-            nsl = _optim.NUM_SLOTS[g.sparse_optimizer.kind] if g.sparse_optimizer else 0
+            kind = g.sparse_optimizer.kind if g.sparse_optimizer else "sgd"
             items = []
             for path, mod in sorted(self.analysis.sparse_modules.items()):
                 info = self.analysis.variables[path + ".weight" if path else "weight"]
                 rows = (int(mod.weight.shape[0]) + info.partitions - 1) // info.partitions
                 items.append((path, info.partitions,
-                              rows * ((int(mod.weight.shape[1]) + 3) // 4 * 16) * (1 + nsl)))
+                              rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]))))
             placed = assign_owners(items, comm.world) \
                 if bool(cfg.communication_config.ps_config.boundary_among_servers) else {}
             for path, mod in self.analysis.sparse_modules.items():
@@ -330,6 +330,23 @@ class TrainEngine(object):
                 raise ValueError(
                     "co-lookup group %s: its tables must all be clipped by the same "
                     "ClipByGlobalNorm(include_sparse=True) rule or all by none" % paths)
+
+    def _check_rowwise(self, sync):
+        """Refuse at build, before anything is allocated, what a row-wise optimizer
+        (`optim.ROWWISE_KINDS`: one accumulator per embedding row) cannot do."""
+        g = self.graph
+        opt, sparse_opt = g.optimizer, g.sparse_optimizer
+        if opt is not None and opt.kind in _optim.ROWWISE_KINDS and self.analysis.dense:
+            raise ValueError(
+                "%s keeps one accumulator per embedding row and trains sparse variables "
+                "only, but the model has trainable dense variables: pass it as "
+                "Graph(..., sparse_optimizer=%s(...)) and give optimizer= a dense rule"
+                % (type(opt).__name__, type(opt).__name__))
+        if sparse_opt is not None and sparse_opt.kind in _optim.ROWWISE_KINDS and not sync:
+            raise ValueError(
+                "%s needs sync=True: the asynchronous push applies every worker's rows "
+                "element by element on the owner, without the merged row a row-wise rule "
+                "needs" % type(sparse_opt).__name__)
 
     def grad_norm(self, i):
         """Pre-clip global norm of clip rule `i` (index in the graph's
@@ -699,9 +716,8 @@ class TrainEngine(object):
                 new_groups.append(grp)
                 continue
             state = [(t.full_weight(), t.full_slots()) for t in olds]
-            nsl = olds[0].nslots
-            nbytes = sum(((t.V + num_partitions - 1) // num_partitions) * t.Dp * 4 * (1 + nsl)
-                         for t in olds)
+            nbytes = sum(((t.V + num_partitions - 1) // num_partitions) *
+                         _optim.table_row_bytes(t.kind, t.D) for t in olds)
             owners = assign_owners([("g", num_partitions, nbytes)], self.comm.world)["g"] \
                 if bool(ps_cfg.boundary_among_servers) else None
             cap = grp.cap

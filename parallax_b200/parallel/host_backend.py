@@ -24,6 +24,8 @@ from .layout import TableLayout
 
 
 def _slots_like(t, optimizer):
+    if optimizer.kind in _optim.ROWWISE_KINDS:      # one value per row of a sparse table
+        t = t[:, :1]
     return tuple(torch.full_like(t, v, dtype=torch.float32)
                  for v in optimizer.slot_init())
 
@@ -201,6 +203,8 @@ class HostSparseTable(object):
             shard[l] = weight.detach().to(torch.float32).cpu()[g]
         self.shard = shard.to(self.device)
         self.slots = _slots_like(self.shard, optimizer)
+        self.nslots = len(self.slots)
+        self.slot_dim = _optim.slot_width(optimizer.kind, self.D)
         self.pending = []
         self.out_dtype = weight.dtype if weight.device.type != "meta" \
             else torch.float32
@@ -324,6 +328,8 @@ class HostSparseTable(object):
         return [self._gather_full(s) for s in self.slots]
 
     def load_full(self, weight, slots=None):
+        if slots is not None:
+            _optim.check_table_slots(self.name, self.optimizer.kind, self.V, self.D, slots)
         g, l = self.layout.global_ids_of_owner(
             0 if self.replicated else self.comm.rank)
         l = l.to(self.device)

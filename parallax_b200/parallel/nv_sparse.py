@@ -134,10 +134,14 @@ class NVSparseTable(object):
         heap = self.heap
         self.tab_buf = heap.alloc(rows * self.Dp * 4, "table:" + name)
         self.table = self.tab_buf.tensor(torch.float32, rows * self.Dp).view(rows, self.Dp)
+        # a row-wise rule keeps one fp32 per row: a dense [rows_local] array (the kernels
+        # address it with a 4-byte pitch); every other rule keeps padded rows like the table
+        self.slot_dim = _optim.slot_width(self.kind, self.D)
+        slot_cols = _optim.slot_width(self.kind, self.Dp)
         self.slot_bufs, self.slots = [], []
         for v in optimizer.slot_init():
-            sb = heap.alloc(rows * self.Dp * 4, "slot:" + name)
-            t = sb.tensor(torch.float32, rows * self.Dp).view(rows, self.Dp)
+            sb = heap.alloc(rows * slot_cols * 4, "slot:" + name)
+            t = sb.tensor(torch.float32, rows * slot_cols).view(rows, slot_cols)
             t.fill_(v)
             self.slot_bufs.append(sb)
             self.slots.append(t)
@@ -241,22 +245,27 @@ class NVSparseTable(object):
         return self.group.cap
 
     # -------------------------------------------------------------- checkpoint
+    def _width(self, what):
+        """Logical columns of "weight" (D) or of slot `what` (D, or 1 for a row-wise rule)."""
+        return self.D if what == "weight" else self.slot_dim
+
     def local_rows(self, what="weight"):
-        """(global ids, rows [n, D]) of the real rows this rank owns — the unit of a
-        sharded checkpoint (no cross-rank traffic)."""
+        """(global ids, rows [n, D] — [n, 1] for a row-wise slot) of the real rows this rank
+        owns — the unit of a sharded checkpoint (no cross-rank traffic)."""
         src = self.table if what == "weight" else self.slots[int(what)]
+        d = self._width(what)
         gs, rows = [], []
         for g, l in self.layout.owner_chunks(0 if self.replicated else self.rank):
             gs.append(g)
-            rows.append(src[l.to(self.device), :self.D].cpu())
+            rows.append(src[l.to(self.device), :d].cpu())
         if not gs:
-            return torch.zeros(0, dtype=torch.int64), torch.zeros(0, self.D)
+            return torch.zeros(0, dtype=torch.int64), torch.zeros(0, d)
         return torch.cat(gs), torch.cat(rows)
 
-    def _gather_full(self, local):
+    def _gather_full(self, local, d):
         L, W = self.layout, self.world
-        local = local[:, :self.D].contiguous()
-        out = torch.zeros(self.V, self.D)
+        local = local[:, :d].contiguous()
+        out = torch.zeros(self.V, d)
         if self.replicated or W == 1:
             g, l = L.global_ids_of_owner(0 if self.replicated else self.rank)
             out[g] = local.cpu()[l]
@@ -269,25 +278,31 @@ class NVSparseTable(object):
 
     def full_weight(self):
         torch.cuda.synchronize(self.device)
-        return self._gather_full(self.table)
+        return self._gather_full(self.table, self.D)
 
     def full_slots(self):
         torch.cuda.synchronize(self.device)
-        return [self._gather_full(s) for s in self.slots]
+        return [self._gather_full(s, self.slot_dim) for s in self.slots]
 
     def load_full(self, weight, slots=None):
+        if slots is not None:
+            _optim.check_table_slots(self.name, self.kind, self.V, self.D, slots)
         for g, l in self.layout.owner_chunks(0 if self.replicated else self.rank):
             l = l.to(self.device)
             self.table[l, :self.D] = weight.float()[g].to(self.device)
             if slots is not None:
                 for s, full in zip(self.slots, slots):
-                    s[l, :self.D] = full.float()[g].to(self.device)
+                    s[l, :self.slot_dim] = full.float()[g].to(self.device)
         self.refresh_shadow()
         torch.cuda.synchronize(self.device)
 
     def load_rows(self, ids, rows, what="weight"):
         """Scatter (global id, row) pairs into this rank's shard; ids owned by other
         ranks are ignored (sharded-checkpoint restore, any source layout)."""
+        d = self._width(what)
+        if rows.dim() != 2 or int(rows.shape[1]) != d:
+            raise ValueError("sparse variable %r: %s rows of shape %s, want [n, %d]"
+                             % (self.name, what, tuple(rows.shape), d))
         L = self.layout
         ids = ids.to(torch.int64)
         own = torch.ones_like(ids, dtype=torch.bool) if self.replicated else \
@@ -295,7 +310,7 @@ class NVSparseTable(object):
         if own.any():
             l = L.local_row_of(ids[own]).to(self.device)
             dst = self.table if what == "weight" else self.slots[int(what)]
-            dst[l, :self.D] = rows[own].float().to(self.device)
+            dst[l, :d] = rows[own].float().to(self.device)
 
     def release(self):
         """Free this table's symmetric segments (collective)."""
@@ -326,7 +341,7 @@ class NVSparseGroup(object):
                 raise ValueError(
                     "co-lookup group: %r and %r differ in rows / partitions / strategy / "
                     "owner placement" % (t0.name, t.name))
-            if (t.kind in _optim.KINDS) != (t0.kind in _optim.KINDS):
+            if _optim.kind_family(t.kind) != _optim.kind_family(t0.kind):
                 raise ValueError("co-lookup group mixes optimizer families")
         self.tables = list(tables)
         self.name = name or "+".join(t.name for t in tables)
@@ -780,7 +795,7 @@ class NVSparseGroup(object):
             d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
             d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
             d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
-            d.hp, d.D4, d.kind = hp_ptr, t.D4, _optim.KIND_ID[t.kind]
+            d.hp, d.D4, d.D, d.kind = hp_ptr, t.D4, t.D, _optim.KIND_ID[t.kind]
             avg = (1.0 / self.world) if t.average else 1.0
             d.avg = avg if sender_scaled else avg * t.scale
         return descs

@@ -629,11 +629,11 @@ def build_nvlink(engine):
     # byte-greedy placement of every partition of every sparse variable on its owner
     # (`ps/between_graph_parallel.py:49-70`); PSConfig.boundary_among_servers=False keeps
     # the naive round-robin placement
-    nslots = _optim.NUM_SLOTS[g.sparse_optimizer.kind]
+    kind = g.sparse_optimizer.kind
     def item_bytes(path, mod):
         info = engine.analysis.variables[pname_of(path)]
         rows = (int(mod.weight.shape[0]) + info.partitions - 1) // info.partitions
-        return info.partitions, rows * ((int(mod.weight.shape[1]) + 3) // 4 * 16) * (1 + nslots)
+        return info.partitions, rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]))
     mods = dict(sparse_items)
     place_items, seen = [], set()
     for path, mod in sparse_items:

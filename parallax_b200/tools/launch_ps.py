@@ -11,9 +11,11 @@ one, and this tool answers it offline with exactly the code the engine runs
     # owner map of the sparse variables of an exported analysis, on 8 owners
     python -m parallax_b200.tools.launch_ps --analysis out/analysis_worker_0.json --owners 8
     # or variables given by hand: name:rows:dim[:partitions[:slots]]; '+' joins a
-    # co-lookup group
+    # co-lookup group; `slots` is a count of D-wide fp32 slots or an optimizer kind
+    # (`rowwise_adagrad` keeps one fp32 per row)
     python -m parallax_b200.tools.launch_ps --owners 8 \
         emb:793470:512:32:1 softmax_w:793470:512:32:1+softmax_b:793470:1:32:1
+    python -m parallax_b200.tools.launch_ps --owners 8 emb:793470:512:32:rowwise_adagrad
 
 It prints, per owner, the partitions and bytes it would hold, the imbalance of the
 byte-greedy placement and of naive round-robin (`PSConfig.boundary_among_servers=False`),
@@ -25,6 +27,7 @@ import argparse
 import json
 import sys
 
+from .. import optim
 from ..parallel.layout import assign_owners
 
 
@@ -32,9 +35,23 @@ def _parse_var(spec):
     f = spec.split(":")
     if len(f) < 3:
         raise ValueError("variable spec %r: want name:rows:dim[:partitions[:slots]]" % spec)
+    slots = f[4] if len(f) > 4 else 0
+    if isinstance(slots, str) and not slots.isdigit():
+        if slots not in optim.NUM_SLOTS:
+            raise ValueError("variable spec %r: slots %r is neither a count nor an optimizer "
+                             "kind (%s)" % (spec, slots, ", ".join(optim.NUM_SLOTS)))
+    else:
+        slots = int(slots)
     return {"name": f[0], "rows": int(f[1]), "dim": int(f[2]),
-            "partitions": int(f[3]) if len(f) > 3 else None,
-            "slots": int(f[4]) if len(f) > 4 else 0}
+            "partitions": int(f[3]) if len(f) > 3 else None, "slots": slots}
+
+
+def row_bytes(v):
+    """Owner bytes of one row of variable `v`: the padded fp32 row and its slots, `slots`
+    D-wide slots or those of the optimizer kind it names."""
+    if isinstance(v["slots"], str):
+        return optim.table_row_bytes(v["slots"], v["dim"])
+    return ((v["dim"] + 3) // 4 * 16) * (1 + v["slots"])
 
 
 def plan(groups, owners, greedy=True):
@@ -47,8 +64,7 @@ def plan(groups, owners, greedy=True):
             raise ValueError("group %s: members differ in partition count %s"
                              % ([v["name"] for v in grp], sorted(parts)))
         P = parts.pop()
-        nbytes = sum(((v["rows"] + P - 1) // P) * ((v["dim"] + 3) // 4 * 16) * (1 + v["slots"])
-                     for v in grp)
+        nbytes = sum(((v["rows"] + P - 1) // P) * row_bytes(v) for v in grp)
         items.append((gi, P, nbytes))
     placed = assign_owners(items, owners) if greedy else \
         {gi: [p % owners for p in range(P)] for gi, P, _ in items}
