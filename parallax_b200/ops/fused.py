@@ -49,14 +49,20 @@ def _count(n=1):
 # ===========================================================================
 # LSTM layer
 # ===========================================================================
+def _acc(t):
+    """The references' accumulation type: fp32 for bf16/fp32 inputs, fp64 kept as fp64 (the
+    tests' oracle)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 def lstm_layer_reference(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
     """x: [T, B, E] → (H [T, B, P], c_T, h_T); plain autograd-able torch."""
     T, Bsz, E = x.shape
     S = W_P.shape[0]
     xw = torch.addmm(bias, x.reshape(T * Bsz, E), Wx).view(T, Bsz, 4 * S)
-    c, h, outs = c0.float(), h0, []
+    c, h, outs = _acc(c0), h0, []
     for t in range(T):
-        gates = torch.addmm(xw[t], h, Wh).float()
+        gates = _acc(torch.addmm(xw[t], h, Wh))
         i, j, f, o = gates.split(S, dim=1)
         c = torch.sigmoid(f + forget_bias) * c + torch.sigmoid(i) * torch.tanh(j)
         m = (torch.sigmoid(o) * torch.tanh(c)).to(x.dtype)
@@ -274,6 +280,9 @@ class _LSTMLayerFn(torch.autograd.Function):
         bounds = [round(i * T / nchunks) for i in range(nchunks + 1)]   # over t, ascending
         state = {"first": True}
         ws2 = sinks.side_stream(dev, 1) if (nchunks == 1 and _dbias_stream()) else None
+        # over several chunks the bias gradient is summed in fp32 and rounded once at the end:
+        # adding chunk sums into the bf16 output rounds it once per chunk
+        dbias_acc = torch.zeros(4 * S, dtype=torch.float32, device=dev) if nchunks > 1 else None
 
         def wgrad(lo, hi):
             """accumulate the contribution of steps [lo, hi) (their dgates / dh_tot are final)"""
@@ -287,15 +296,18 @@ class _LSTMLayerFn(torch.autograd.Function):
                 if state["first"]:
                     torch.mm(hT, dg, out=dWh_o)
                     torch.mm(xT, dg, out=dWx_o)
-                    if ws2 is None:
+                    if ws2 is None and dbias_acc is None:
                         torch.sum(dg, 0, out=dbias_o)
                     torch.mm(mT, dh2, out=dWP_o)
                     state["first"] = False
                 else:
                     dWh_o.addmm_(hT, dg)
                     dWx_o.addmm_(xT, dg)
-                    dbias_o.add_(dg.sum(0))
                     dWP_o.addmm_(mT, dh2)
+                if dbias_acc is not None:
+                    dbias_acc.add_(dg.sum(0, dtype=torch.float32))
+                    if lo == 0:                 # the last chunk
+                        dbias_o.copy_(dbias_acc)
         pending_hi = T
         Wc = ctx.Wc
         mode = _bwd_fused_w()
@@ -385,6 +397,8 @@ class _LSTMLayerFn(torch.autograd.Function):
             ev_b = ev
         for t_ in (dgates, dh_tot, x, h_all, m_all, dWh_o, dWx_o, dbias_o, dWP_o):
             t_.record_stream(ws)
+        if dbias_acc is not None:
+            dbias_acc.record_stream(ws)
         outs, plain = [], False
         for ref, o, sunk, e_ in ((W_ref, dW if stacked else dWx_o, w_sunk, ev),
                                  (bias_ref, dbias_o, b_sunk, ev_b), (WP_ref, dWP_o, p_sunk, ev)):
@@ -435,8 +449,8 @@ def lstm_layer_stacked(x, W, bias, W_P, c0, h0, forget_bias=1.0):
 def sampled_softmax_reference(inputs, true_w, samp_w, true_b, samp_b, logq_true,
                               logq_samp, targets, sampled):
     """Per-example loss [N] (tf.nn.sampled_softmax_loss semantics)."""
-    true_logits = (inputs * true_w).sum(-1).float() + true_b.float() - logq_true
-    samp_logits = (inputs @ samp_w.t()).float() + (samp_b.float() - logq_samp)
+    true_logits = _acc((inputs * true_w).sum(-1)) + _acc(true_b) - logq_true
+    samp_logits = _acc(inputs @ samp_w.t()) + (_acc(samp_b) - logq_samp)
     hits = targets.unsqueeze(1) == sampled.unsqueeze(0)
     samp_logits = samp_logits.masked_fill(hits, float("-inf"))
     lse = torch.logsumexp(torch.cat([true_logits.unsqueeze(1), samp_logits], 1), 1)
@@ -477,7 +491,7 @@ class _SampledSoftmaxFn(torch.autograd.Function):
         d_samp_w = probs.t() @ gi
         d_true_w = (gt * inputs.float()).to(dt)
         d_samp_b = (probs.float().t() @ g) if probs.dtype == torch.float32 else \
-            (probs.t() @ g.to(dt).unsqueeze(1)).squeeze(1).float()
+            torch.mm(probs.t(), g.to(dt).unsqueeze(1), out_dtype=torch.float32).squeeze(1)
         d_true_b = gt.squeeze(1)
         return d_inputs, d_true_w, d_samp_w, d_true_b, d_samp_b, None, None, None, None
 
@@ -587,6 +601,10 @@ class _SampledSoftmaxHeadFn(torch.autograd.Function):
         torch.mm(probs.t(), gi, out=d_w_all[N:])                   # d w_sampled
         if db.dtype == dt:                                         # d b_sampled
             torch.mm(probs.t(), grow.view(N, 1), out=db[N:].view(S, 1))
+        elif dt == torch.bfloat16 and db.dtype == torch.float32:
+            # fp32 straight out of the product: a bf16 result would round the gradient of an
+            # fp32 bias to 8 bits
+            db[N:].copy_(torch.mm(probs.t(), grow.view(N, 1), out_dtype=torch.float32).view(S))
         else:
             db[N:].copy_((probs.t() @ grow.view(N, 1)).view(S))
         db = db.view(b_shape)

@@ -39,6 +39,47 @@ def test_sampled_softmax_head_node_matches_autograd_of_the_reference(weighted):
     assert torch.allclose(o2, ref, atol=1e-6)
 
 
+def test_lstm_layer_reference_gradcheck_fp64():
+    """The LSTM oracle every device test trusts: its autograd agrees with finite differences,
+    which needs it to stay in fp64 end to end when given fp64."""
+    from parallax_b200.ops.fused import lstm_layer_reference
+    torch.manual_seed(0)
+    T, B, E, S, P = 3, 2, 3, 4, 2
+    mk = lambda *s: (torch.randn(*s, dtype=torch.float64) * 0.5).requires_grad_(True)
+    args = (mk(T, B, E), mk(E, 4 * S), mk(P, 4 * S), mk(4 * S), mk(S, P), mk(B, S), mk(B, P))
+
+    def f(*a):
+        H, c, h = lstm_layer_reference(*a, forget_bias=0.7)
+        assert H.dtype == c.dtype == h.dtype == torch.float64
+        return H, c, h
+    assert torch.autograd.gradcheck(f, args)
+
+
+def test_sampled_softmax_reference_gradcheck_fp64_with_masked_hit():
+    from parallax_b200.ops.fused import sampled_softmax_reference
+    torch.manual_seed(1)
+    N, S, P = 4, 6, 3
+    mk = lambda *s: torch.randn(*s, dtype=torch.float64).requires_grad_(True)
+    targets = torch.tensor([3, 7, 1, 9])
+    sampled = torch.tensor([2, 7, 5, 3, 8, 0])          # rows 0 and 1 each have a hit
+    lqt, lqs = torch.randn(N, dtype=torch.float64), torch.randn(S, dtype=torch.float64)
+    args = (mk(N, P), mk(N, P), mk(S, P), mk(N), mk(S))
+
+    def f(*a):
+        out = sampled_softmax_reference(*a, lqt, lqs, targets, sampled)
+        assert out.dtype == torch.float64
+        return out
+    assert torch.autograd.gradcheck(f, args)
+    # the masked logit takes no part: moving the hit column's bias changes nothing in its row
+    a = [t.detach() for t in args]
+    base = f(*a)
+    b2 = a[4].clone()
+    b2[1] += 5.0
+    moved = sampled_softmax_reference(a[0], a[1], a[2], a[3], b2, lqt, lqs, targets, sampled)
+    assert moved[1] == base[1]
+    assert moved[0] != base[0]
+
+
 def test_lm1b_time_major_rows_give_the_batch_major_loss(monkeypatch):
     """The model orders its rows (t, b); the loss is the mean over all rows, so it must equal
     the batch-major formulation of `examples/lm1b/language_model.py:88-107`."""

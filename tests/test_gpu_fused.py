@@ -34,7 +34,7 @@ def test_lstm_layer_matches_reference(dtype, tol):
 
 
 @pytest.mark.parametrize("tc_fwd", ["0", "1"])
-def test_lstm_layer_bf16_tcgen05_backward_path(tc_fwd, monkeypatch):
+def test_lstm_layer_bf16_wgmma_backward_path(tc_fwd, monkeypatch):
     """B=128, 4S multiple of 1024: the recurrent backward product runs on the
     wgmma split-K kernel with the fused addend; with PARALLAX_LSTM_TC_FWD=1 the
     forward step runs on the wgmma kernel with the LSTM cell fused in its

@@ -1,0 +1,543 @@
+"""The LM1B hot-path kernels against fp64 at the shapes the benchmark runs.
+
+Every reference is plain PyTorch in fp64 on the same bf16/fp32-rounded inputs the kernel
+receives.  Where a kernel's rounding cannot be bounded elementwise (whole layers, the loss
+head), its error is held to that of the same PyTorch composition run in the kernel's own
+dtype: ``err(kernel) <= 2·err(torch) + floor·max|ref|``, for the max-abs error and for the
+relative Frobenius error (`_within`).  The measured ratios are printed (``pytest -s``)."""
+import ctypes
+import math
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+_vp = ctypes.c_void_p
+FACTOR = 2.0
+
+
+def _p(t):
+    return _vp(t.data_ptr())
+
+
+def _stream():
+    return _vp(torch.cuda.current_stream().cuda_stream)
+
+
+def _lib():
+    from parallax_b200 import ops
+    from parallax_b200.ops import fused, gemm  # noqa: F401  (register the signatures)
+    return ops.lib()
+
+
+def _gen(seed):
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def _leaf(t, dt):
+    """A fresh leaf copy: runs never share a tensor, so no gradient accumulates across them."""
+    return t.detach().to(dt, copy=True).requires_grad_(True)
+
+
+def _ulp_bf16(x):
+    """bf16 spacing at |x| (8 significant bits), x in fp64."""
+    a = x.abs().clamp_min(2.0 ** -126)
+    return torch.exp2(torch.floor(torch.log2(a)) - 7)
+
+
+def _assert_elementwise(name, got, ref, scale, dtype):
+    """fp32: |Δ| <= 1e-6·scale + 4e-6·|ref|.  bf16: one bf16 ulp of the fp64 value plus the same
+    1e-6·scale floor, which covers the fp32 cancellation of 1 − tanh², 1 − σ and tanh near 0
+    (`scale`: magnitude of the operands, elementwise)."""
+    got = got.double()
+    assert not torch.isnan(got).any(), name + ": NaN"
+    if dtype == torch.float32:
+        bound = 1e-6 * scale + 4e-6 * ref.abs()
+    else:
+        bound = _ulp_bf16(ref) + 1e-6 * scale
+    err = (got - ref).abs()
+    ok = err <= bound
+    if not bool(ok.all()):
+        i = int(torch.argmax((err - bound).reshape(-1)))
+        raise AssertionError("%s: %d elements out of bound; worst at %d: got %r ref %r bound %r"
+                             % (name, int((~ok).sum()), i, float(got.reshape(-1)[i]),
+                                float(ref.reshape(-1)[i]), float(bound.reshape(-1)[i])))
+
+
+def _errs(got, ref):
+    d = got.double() - ref
+    nr = float(ref.norm())
+    return float(d.abs().max()), float(d.norm()) / (nr if nr > 0 else 1.0)
+
+
+def _floor(dtype, numel):
+    """Relative floor of the calibrated bound for a computation in `dtype`.  bf16: 1e-3, or one
+    bf16 rounding (2^-8) over sqrt(numel) if larger: with a handful of elements the PyTorch
+    error is one draw of that rounding and may come out near zero.  fp32: 1e-5, which leaves
+    room for the kernels' fast exp/log (tens of fp32 ulps) and none for a step done in bf16
+    (2^-9)."""
+    if dtype == torch.bfloat16:
+        return max(1e-3, 2.0 ** -8 / math.sqrt(numel))
+    return 1e-5
+
+
+def _within(got, ref, low, dtype, factor=FACTOR):
+    """The self-calibrating bound (module docstring) for a kernel computing in `dtype` ->
+    (ok, ratio of max-abs errors, ratio of Frobenius errors)."""
+    e_k, f_k = _errs(got, ref)
+    e_t, f_t = _errs(low, ref)
+    floor = _floor(dtype, ref.numel())
+    scale = float(ref.abs().max())
+    ok = e_k <= factor * e_t + floor * scale and f_k <= factor * f_t + floor
+    return ok, e_k / max(e_t, 1e-300), f_k / max(f_t, 1e-300)
+
+
+def _assert_calibrated(name, got, ref, low, dtype, factor=FACTOR):
+    assert got.shape == ref.shape, (name, got.shape, ref.shape)
+    assert torch.isfinite(got).all(), name + ": inf/NaN"
+    ok, r_max, r_fro = _within(got, ref, low, dtype, factor)
+    e_k, f_k = _errs(got, ref)
+    print("ratio %-36s max %.3f fro %.3f  rel-err max %.2e fro %.2e"
+          % (name, r_max, r_fro, e_k / max(float(ref.abs().max()), 1e-300), f_k))
+    assert ok, (name, _errs(got, ref), _errs(low, ref), float(ref.abs().max()))
+
+
+# ===========================================================================
+# LSTM cell kernels, called directly
+# ===========================================================================
+_CELL_SHAPES = [(3, 100), (16, 64), (128, 2048), (256, 2048)]   # 256·2048 > 132·8·256
+
+
+def _pre_activations(B, S, dt, seed):
+    """Gate pre-activations with ±20 and ±90 sprinkled in: __expf overflows at ±90."""
+    x = torch.randn(B, 4 * S, device="cuda", generator=_gen(seed)) * 3.0
+    v = x.view(-1)
+    v[::7], v[3::11], v[5::13], v[1::17] = 20.0, -20.0, 90.0, -90.0
+    return x.to(dt)
+
+
+def _cell_fwd64(g, cp, fb):
+    S = cp.shape[1]
+    g = g.double()
+    i, j, f, o = g.split(S, dim=1)
+    si, tj, sf, so = torch.sigmoid(i), torch.tanh(j), torch.sigmoid(f + fb), torch.sigmoid(o)
+    c = sf * cp.double() + si * tj
+    return torch.cat([si, tj, sf, so], 1), c, so * torch.tanh(c)
+
+
+@pytest.mark.parametrize("dt", [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize("B,S", _CELL_SHAPES)
+@pytest.mark.parametrize("fb", [0.0, 1.0, 2.5])
+def test_lstm_cell_fwd_kernel_vs_fp64(dt, B, S, fb):
+    L = _lib()
+    g = _pre_activations(B, S, dt, seed=B * S)
+    cp = torch.randn(B, S, device="cuda", generator=_gen(1)) * 2.0
+    act = torch.empty(B, 4 * S, dtype=dt, device="cuda")
+    c_new = torch.empty(B, S, device="cuda")
+    m = torch.empty(B, S, dtype=dt, device="cuda")
+    assert L.px_lstm_cell_fwd(_p(g), _p(cp), _p(act), _p(c_new), _p(m), B, S, fb,
+                              0 if dt == torch.float32 else 1, _stream()) == 0
+    torch.cuda.synchronize()
+    act64, c64, m64 = _cell_fwd64(g, cp, fb)
+    sc = 1.0 + cp.double().abs()
+    _assert_elementwise("act", act, act64, 1.0, dt)
+    _assert_elementwise("c_new", c_new, c64, sc, torch.float32)
+    _assert_elementwise("m", m, m64, sc, dt)
+    # saturated gates: exactly 0 or 1, never NaN (σ(-90): __expf(90) = inf)
+    gv = g.double()
+    for gate in (0, 2, 3):
+        pre = gv[:, gate * S:(gate + 1) * S] + (fb if gate == 2 else 0.0)
+        a = act[:, gate * S:(gate + 1) * S].double()
+        assert bool((a[pre >= 90] == 1).all()) and bool((a[pre <= -90] == 0).all()), gate
+    tj = act[:, S:2 * S].double()
+    assert bool((tj[gv[:, S:2 * S].abs() >= 20].abs() == 1).all())
+
+
+@pytest.mark.parametrize("dt", [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize("B,S", _CELL_SHAPES)
+@pytest.mark.parametrize("interleaved", [0, 1])
+def test_lstm_cell_bwd_kernel_vs_fp64(dt, B, S, interleaved):
+    if interleaved and S % 32:
+        pytest.skip("the gate-interleaved layout tiles 32 units")
+    from parallax_b200.ops.fused import gate_interleave_perm
+    L = _lib()
+    gen = _gen(B + S + interleaved)
+    act = torch.cat([torch.sigmoid(_pre_activations(B, S, torch.float32, seed=S)[:, :S]),
+                     torch.tanh(torch.randn(B, S, device="cuda", generator=gen) * 2),
+                     torch.sigmoid(torch.randn(B, S, device="cuda", generator=gen) * 3 + 1),
+                     torch.sigmoid(torch.randn(B, S, device="cuda", generator=gen) * 3)], 1).to(dt)
+    cp = torch.randn(B, S, device="cuda", generator=gen) * 2.0
+    cn = torch.randn(B, S, device="cuda", generator=gen) * 2.0
+    cn.view(-1)[::9] = 30.0                                # tanh(c) = 1: 1 − tanh² cancels
+    dm = (torch.randn(B, S, device="cuda", generator=gen) * 0.5).to(dt)
+    dc_in = torch.randn(B, S, device="cuda", generator=gen) * 0.5
+    if interleaved:
+        perm, inv = gate_interleave_perm(S, "cuda")
+        act_k = act.index_select(1, perm).contiguous()
+    else:
+        act_k = act
+    dc = dc_in.clone()
+    dg = torch.empty(B, 4 * S, dtype=dt, device="cuda")
+    assert L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act_k), _p(cp), _p(cn), _p(dg), B, S,
+                              0 if dt == torch.float32 else 1, interleaved, _stream()) == 0
+    torch.cuda.synchronize()
+    if interleaved:
+        dg = dg.index_select(1, inv)
+    si, tj, sf, so = act.double().split(S, dim=1)
+    tc = torch.tanh(cn.double())
+    dmv = dm.double()
+    dcv = dc_in.double() + dmv * so * (1 - tc * tc)
+    ref = torch.cat([dcv * tj * si * (1 - si), dcv * si * (1 - tj * tj),
+                     dcv * cp.double() * sf * (1 - sf), dmv * tc * so * (1 - so)], 1)
+    sc = (dc_in.double().abs() + dmv.abs()) * (1.0 + cp.double().abs())
+    _assert_elementwise("dgates", dg, ref, sc.repeat(1, 4), dt)
+    _assert_elementwise("dc", dc, dcv * sf, sc, torch.float32)
+
+
+# ===========================================================================
+# fused wgmma gates kernel (PARALLAX_LSTM_TC_FWD=1), called directly
+# ===========================================================================
+def _run_gates_tc(h, Wh, xw, cp, fb):
+    """Plain-layout operands in; the kernel sees the gate-interleaved layout.  Returns its
+    (act in plain column order, c_new, m)."""
+    from parallax_b200.ops.fused import gate_interleave_perm
+    L = _lib()
+    M, K = h.shape
+    S = cp.shape[1]
+    perm, inv = gate_interleave_perm(S, "cuda")
+    WhP = Wh.index_select(1, perm).t().contiguous()        # [4S, K], K-contiguous
+    xw_l = xw.index_select(1, perm).contiguous()
+    c_new = torch.empty(M, S, device="cuda")
+    m = torch.empty(M, S, dtype=torch.bfloat16, device="cuda")
+    act = torch.empty(M, 4 * S, dtype=torch.bfloat16, device="cuda")
+    assert L.px_lstm_gates_tc(_p(h), _p(WhP), _p(xw_l), _p(cp), _p(c_new), _p(m), _p(act),
+                              M, S, K, fb, _stream()) == 0
+    torch.cuda.synchronize()
+    return act.index_select(1, inv), c_new, m
+
+
+@pytest.mark.parametrize("M", [128, 256])
+@pytest.mark.parametrize("S", [256, 2048])
+@pytest.mark.parametrize("K", [64, 512, 1024])
+@pytest.mark.parametrize("fb", [0.0, 1.0])
+def test_lstm_gates_tc_exact_product_vs_fp64(M, S, K, fb):
+    """h and Wh are small multiples of 2^-4: the product is exact in fp32, so every output
+    meets the cell kernel's elementwise bounds."""
+    gen = _gen(M + S + K)
+    h = (torch.randint(-2, 3, (M, K), device="cuda", generator=gen) / 16.0).bfloat16()
+    Wh = (torch.randint(-2, 3, (K, 4 * S), device="cuda", generator=gen) / 16.0).bfloat16()
+    xw = torch.randn(M, 4 * S, device="cuda", generator=gen).bfloat16()
+    cp = torch.randn(M, S, device="cuda", generator=gen) * 2.0
+    act, c_new, m = _run_gates_tc(h, Wh, xw, cp, fb)
+    act64, c64, m64 = _cell_fwd64(h.double() @ Wh.double() + xw.double(), cp, fb)
+    sc = 1.0 + cp.double().abs()
+    _assert_elementwise("act", act, act64, 1.0, torch.bfloat16)
+    _assert_elementwise("c_new", c_new, c64, sc, torch.float32)
+    _assert_elementwise("m", m, m64, sc, torch.bfloat16)
+
+
+def test_lstm_gates_tc_random_vs_fp64():
+    """Random operands: the bounds widen by the fp32 accumulation error of the product,
+    2^-16·(|h|·|Wh|), propagated through the cell (|σ'|, |tanh'| <= 1)."""
+    M, S, K, fb = 128, 2048, 512, 1.0
+    gen = _gen(5)
+    h = (torch.randn(M, K, device="cuda", generator=gen) * 0.5).bfloat16()
+    Wh = (torch.randn(K, 4 * S, device="cuda", generator=gen) * 0.05).bfloat16()
+    xw = torch.randn(M, 4 * S, device="cuda", generator=gen).bfloat16()
+    cp = torch.randn(M, S, device="cuda", generator=gen) * 2.0
+    act, c_new, m = _run_gates_tc(h, Wh, xw, cp, fb)
+    act64, c64, m64 = _cell_fwd64(h.double() @ Wh.double() + xw.double(), cp, fb)
+    perr = 2.0 ** -16 * (h.double().abs() @ Wh.double().abs())
+    pu = sum(perr.split(S, dim=1))
+    sc_c = (1.0 + cp.double().abs()) * (1.0 + 1e6 * pu)
+    _assert_elementwise("act", act, act64, 1.0 + 1e6 * perr, torch.bfloat16)
+    _assert_elementwise("c_new", c_new, c64, sc_c, torch.float32)
+    _assert_elementwise("m", m, m64, sc_c, torch.bfloat16)
+
+
+# ===========================================================================
+# whole layer at the bench shape, every scheduling / kernel variant
+# ===========================================================================
+B_, E_, S_, P_ = 128, 512, 2048, 512
+_NAMES = ["H", "cT", "hT", "dx", "dW", "dbias", "dW_P", "dc0", "dh0"]
+# dc flows back through σ(f) of every step.  The kernels read σ(f) from the bf16 activations
+# saved by the forward pass; the PyTorch composition keeps it in fp32 in its graph.  Each step
+# multiplies dc by a factor rounded to 2^-9: on one H100 the kernel's max-abs error is 2.45x
+# PyTorch's at T = 4 and 1.79x at T = 6 (Frobenius 1.46x and 1.42x).
+_FACTOR_OF = {"dc0": 3.0}
+_ref_cache = {}
+
+
+def _layer_inputs(T):
+    gen = _gen(T)
+    mk = lambda sc, *s: (torch.randn(*s, device="cuda", generator=gen) * sc).bfloat16()
+    return dict(x=mk(1.0, T, B_, E_), W=mk(0.04, E_ + P_, 4 * S_), b=mk(0.1, 4 * S_),
+                WP=mk(0.03, S_, P_), c0=torch.randn(B_, S_, device="cuda", generator=gen) * 0.5,
+                h0=mk(0.3, B_, P_), gH=mk(0.1, T, B_, P_),
+                gc=torch.randn(B_, S_, device="cuda", generator=gen) * 0.1, gh=mk(0.1, B_, P_))
+
+
+def _run_layer(kind, inp, dt, before_backward=None):
+    """kind: "plain" (lstm_layer, Wx and Wh separate) | "stacked" | "reference" (PyTorch).
+    Returns [H, cT, hT, dx, dW (stacked [E+P, 4S]), dbias, dW_P, dc0, dh0]."""
+    from parallax_b200.ops import fused
+    x, W, b, WP, h0 = (_leaf(inp[k], dt) for k in ("x", "W", "b", "WP", "h0"))
+    c0 = _leaf(inp["c0"], torch.float64 if dt == torch.float64 else torch.float32)
+    if kind == "stacked":
+        H, cT, hT = fused.lstm_layer_stacked(x, W, b, WP, c0, h0, 1.0)
+    elif kind == "plain":
+        Wx, Wh = _leaf(W[:E_], dt), _leaf(W[E_:], dt)
+        H, cT, hT = fused.lstm_layer(x, Wx, Wh, b, WP, c0, h0, 1.0)
+    else:
+        H, cT, hT = fused.lstm_layer_reference(x, W[:E_], W[E_:], b, WP, c0, h0, 1.0)
+    if before_backward is not None:
+        before_backward()
+    torch.autograd.backward([H, cT, hT], [inp["gH"].to(H.dtype), inp["gc"].to(cT.dtype),
+                                          inp["gh"].to(hT.dtype)])
+    torch.cuda.synchronize()
+    dW = torch.cat([Wx.grad, Wh.grad]) if kind == "plain" else W.grad
+    grads = [x.grad, dW, b.grad, WP.grad, c0.grad, h0.grad]
+    return [t.detach() for t in (H, cT, hT)] + [None if g is None else g.detach() for g in grads]
+
+
+def _layer_refs(T):
+    if T not in _ref_cache:
+        inp = _layer_inputs(T)
+        _ref_cache[T] = (inp, _run_layer("reference", inp, torch.float64),
+                         _run_layer("reference", inp, torch.bfloat16))
+    return _ref_cache[T]
+
+
+_VARIANTS = {
+    "default": {},
+    "l2_splitk": {"PARALLAX_GEMM_CLUSTER": "0"},
+    "tc_fwd": {"PARALLAX_LSTM_TC_FWD": "1"},
+    "fusedw_tc": {"PARALLAX_LSTM_BWD_FUSEDW": "tc"},
+    "fusedw_cublas": {"PARALLAX_LSTM_BWD_FUSEDW": "cublas"},
+    "wgrad_chunks2": {"PARALLAX_LSTM_WGRAD_CHUNKS": "2"},
+    "wgrad_chunks3": {"PARALLAX_LSTM_WGRAD_CHUNKS": "3"},
+    "dbias_same_stream": {"PARALLAX_LSTM_DBIAS_STREAM": "0"},
+    "wpt_in_backward": {"PARALLAX_LSTM_WPT_SIDE": "0"},
+}
+
+
+@pytest.mark.parametrize("kind", ["plain", "stacked"])
+@pytest.mark.parametrize("variant", list(_VARIANTS))
+def test_lstm_layer_variants_vs_fp64(kind, variant, monkeypatch):
+    """B 128, E 512, S 2048, P 512 (the bench layer), T 4 (T 6 for three weight-gradient
+    chunks): outputs and every input gradient against fp64."""
+    for k, v in _VARIANTS[variant].items():
+        monkeypatch.setenv(k, v)
+    T = 6 if variant == "wgrad_chunks3" else 4
+    inp, ref, low = _layer_refs(T)
+    got = _run_layer(kind, inp, torch.bfloat16)
+    for name, g, r, lo in zip(_NAMES, got, ref, low):
+        _assert_calibrated("%s/%s/%s" % (kind, variant, name), g, r, lo, torch.bfloat16,
+                           _FACTOR_OF.get(name, FACTOR))
+
+
+def test_lstm_layer_schedule_variants_bit_identical(monkeypatch):
+    """Moving the W_P transpose or the bias sum to another stream changes no arithmetic, and the
+    cluster split-K reduction has a fixed order: these runs agree bit for bit.  A missing stream
+    wait shows up here as a difference."""
+    inp, _, _ = _layer_refs(4)
+    base = _run_layer("stacked", inp, torch.bfloat16)
+    for env in ({}, {"PARALLAX_LSTM_WPT_SIDE": "0"}, {"PARALLAX_LSTM_DBIAS_STREAM": "0"}):
+        with monkeypatch.context() as mp:
+            for k, v in env.items():
+                mp.setenv(k, v)
+            got = _run_layer("stacked", inp, torch.bfloat16)
+        for name, a, b in zip(_NAMES, base, got):
+            assert torch.equal(a.reshape(-1).view(torch.uint8), b.reshape(-1).view(torch.uint8)), \
+                (env, name)
+
+
+@pytest.mark.parametrize("variant", ["default", "wgrad_chunks2", "dbias_same_stream"])
+def test_lstm_layer_stacked_writes_bucket_sinks(variant, monkeypatch):
+    """The model's path: the weight gradients go straight into views of one gradient bucket on
+    the side streams, autograd gets None for those parameters, and the bucket bytes around
+    the views keep their bits."""
+    from parallax_b200.ops import fused, sinks
+    for k, v in _VARIANTS[variant].items():
+        monkeypatch.setenv(k, v)
+    inp, ref, low = _layer_refs(4)
+    x, W, b, WP, h0 = (_leaf(inp[k], torch.bfloat16) for k in ("x", "W", "b", "WP", "h0"))
+    c0 = _leaf(inp["c0"], torch.float32)
+    gap = 64
+    sizes = [W.numel(), b.numel(), WP.numel()]
+    bucket = torch.full((sum(sizes) + gap * 4,), float("nan"), dtype=torch.bfloat16,
+                        device="cuda")
+    sentinel = bucket.view(torch.int16)[0].item()
+    offs, o = [], gap
+    for n in sizes:
+        offs.append(o)
+        o += n + gap
+    views = [bucket[o_:o_ + n].view(p.shape) for o_, n, p in zip(offs, sizes, (W, b, WP))]
+    delivered = {}
+    params = (W, b, WP)
+    try:
+        for i, (p, v) in enumerate(zip(params, views)):
+            sinks.register(p, v, lambda ev, i=i: delivered.__setitem__(i, ev))
+        H, cT, hT = fused.lstm_layer_stacked(x, W, b, WP, c0, h0, 1.0)
+        torch.autograd.backward([H, cT, hT], [inp["gH"], inp["gc"], inp["gh"]])
+        assert sorted(delivered) == [0, 1, 2]
+        for ev in delivered.values():
+            if ev is not None:
+                torch.cuda.current_stream().wait_event(ev)
+        torch.cuda.synchronize()
+    finally:
+        sinks.unregister_all(params)
+    assert W.grad is None and b.grad is None and WP.grad is None
+    got = {"dx": x.grad, "dW": views[0], "dbias": views[1], "dW_P": views[2], "dc0": c0.grad,
+           "dh0": h0.grad, "H": H.detach(), "cT": cT.detach(), "hT": hT.detach()}
+    for i, name in enumerate(_NAMES):
+        _assert_calibrated("sinks/%s/%s" % (variant, name), got[name], ref[i], low[i],
+                           torch.bfloat16, _FACTOR_OF.get(name, FACTOR))
+    bits = bucket.view(torch.int16)
+    keep = torch.ones_like(bits, dtype=torch.bool)
+    for o_, n in zip(offs, sizes):
+        keep[o_:o_ + n] = False
+    assert bool((bits[keep] == sentinel).all()), "bytes between the sink views were written"
+
+
+# ===========================================================================
+# sampled softmax: the fused head and the PARALLAX_SSM_HEAD=0 path
+# ===========================================================================
+_V = 100000
+_SSM_SHAPES = ([(2560, 8192, 512)] + [(256, 1024, p) for p in (8, 64, 520)] +
+               [(256, s, 64) for s in (1, 256, 1024, 1025, 2048, 2049, 4096, 4097, 8192, 8193,
+                                       16384, 16385)])
+
+
+def _ssm_inputs(N, S, P, seed):
+    """The first H rows each have an accidental hit whose logit leads its row by far (the
+    sampled row is the input row scaled to a logit of 20), so a missing mask moves the loss."""
+    gen = _gen(seed)
+    a = math.sqrt(2.0 / math.sqrt(P))                    # logits ~ N(0, 4)
+    inputs = torch.randn(N, P, device="cuda", generator=gen) * a
+    w_all = torch.randn(N + S, P, device="cuda", generator=gen) * a
+    b_all = torch.randn(N + S, 1, device="cuda", generator=gen) * 0.5
+    logq = torch.randn(N + S, device="cuda", generator=gen) * 0.5 - 8.0
+    targets = torch.randint(0, _V, (N,), device="cuda", generator=gen)
+    sampled = torch.randperm(_V, device="cuda", generator=gen)[:S]
+    H = min(8, S, N)
+    sampled[:H] = targets[:H]
+    x = inputs[:H]
+    w_all[N:N + H] = x * (20.0 / (x * x).sum(1, keepdim=True))
+    return inputs, w_all, b_all, logq, targets, sampled
+
+
+def _ssm_rounded(data, dt, bdt):
+    """The inputs as the kernel receives them: every run, fp64 included, starts from these."""
+    inputs, w_all, b_all, logq, targets, sampled = data
+    return inputs.to(dt), w_all.to(dt), b_all.to(bdt), logq, targets, sampled
+
+
+def _ssm_objective(entry, inputs, w_all, b_all, logq, targets, sampled, rw):
+    """-> (mean loss, per-row loss or None, dtrue or None)."""
+    from parallax_b200.ops import fused
+    N = inputs.shape[0]
+    if entry == "reference":
+        b = b_all.reshape(-1)
+        rows = fused.sampled_softmax_reference(inputs, w_all[:N], w_all[N:], b[:N], b[N:],
+                                               logq[:N], logq[N:], targets, sampled)
+        obj = (rows * rw if rw is not None else rows).mean()
+        return obj, rows, None
+    obj = fused.sampled_softmax_head(inputs, w_all, b_all, logq, targets, sampled, row_w=rw)
+    if entry == "head":
+        assert obj.grad_fn.name().startswith("_SampledSoftmaxHeadFn") or \
+            w_all.shape[0] - N > 256 * 64
+    with torch.no_grad():
+        if entry == "loss":
+            b = b_all.reshape(-1)
+            rows = fused.sampled_softmax_loss(inputs, w_all[:N], w_all[N:], b[:N], b[N:],
+                                              logq[:N], logq[N:], targets, sampled)
+            return obj, rows, None
+        if w_all.shape[0] - N > 256 * 64:
+            return obj, None, None
+        adj = b_all.reshape(-1).float() - logq
+        _, rows, dtrue = fused._head_forward(inputs, w_all, adj, targets.long().contiguous(),
+                                             sampled.long().contiguous())
+        return obj, rows, dtrue
+
+
+def _ssm_run(entry, data, dt, bdt, rw):
+    inputs, w_all, b_all, logq, targets, sampled = data
+    i, w, b = _leaf(inputs, dt), _leaf(w_all, dt), _leaf(b_all, bdt)
+    lq = logq.double() if dt == torch.float64 else logq
+    r = None if rw is None else (rw.double() if dt == torch.float64 else rw)
+    obj, rows, dtrue = _ssm_objective(entry, i, w, b, lq, targets, sampled, r)
+    (obj * 7.0).backward()
+    torch.cuda.synchronize()
+    N = inputs.shape[0]
+    out = {"loss": obj.detach().reshape(1), "d_inputs": i.grad, "d_w_true": w.grad[:N],
+           "d_w_samp": w.grad[N:], "d_b_true": b.grad[:N], "d_b_samp": b.grad[N:]}
+    if rows is not None:
+        out["rows"] = rows.detach()
+    if entry == "reference":
+        out["dtrue"] = torch.exp(-out["rows"]) - 1.0      # p(true) − 1, loss = −log p(true)
+    elif dtrue is not None:
+        out["dtrue"] = dtrue
+    return out
+
+
+@pytest.mark.parametrize("N,S,P", _SSM_SHAPES)
+@pytest.mark.parametrize("entry", ["head", "loss"])
+@pytest.mark.parametrize("dt,bdt", [(torch.float32, torch.float32),
+                                    (torch.bfloat16, torch.float32),
+                                    (torch.bfloat16, torch.bfloat16)])
+@pytest.mark.parametrize("weighted", [False, True])
+def test_sampled_softmax_vs_fp64(N, S, P, entry, dt, bdt, weighted, monkeypatch):
+    if entry == "loss":
+        monkeypatch.setenv("PARALLAX_SSM_HEAD", "0")
+    data = _ssm_rounded(_ssm_inputs(N, S, P, seed=N + S + P), dt, bdt)
+    rw = torch.rand(N, device="cuda", generator=_gen(9)) if weighted else None
+    ref = _ssm_run("reference", data, torch.float64, torch.float64, rw)
+    low = _ssm_run("reference", data, dt, bdt, rw)
+    got = _ssm_run(entry, data, dt, bdt, rw)
+    tag = "%s/%s/%d,%d,%d" % (entry, str(dt)[6:], N, S, P)
+    for k in got:
+        # the compute dtype, not the output's, sets the floor
+        _assert_calibrated("%s/%s" % (tag, k), got[k], ref[k], low[k], dt)
+    if (N, S, P) == (2560, 8192, 512) and not weighted:
+        # the hits matter: the fp64 reference without the mask breaks the bound
+        inputs, w_all, b_all, logq, targets, sampled = data
+        nomask = sampled.clone()
+        nomask[:8] = -1
+        un = _ssm_run("reference", (inputs, w_all, b_all, logq, targets, nomask),
+                      torch.float64, torch.float64, rw)
+        for k in ("rows", "d_b_samp"):
+            assert not _within(un[k], ref[k], low[k], dt)[0], k
+
+
+@pytest.mark.parametrize("dt", [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize("S", [1, 1024, 8192])
+def test_sampled_softmax_all_sampled_hit_row_and_extreme_offsets(dt, S):
+    """Row 0: every sampled id is its target -> loss 0 and d true-logit 0 exactly.  Bias
+    offsets of ±80 on the other rows and columns: no inf, no NaN, still on the fp64 value."""
+    from parallax_b200.ops import fused
+    N, P = 256, 64
+    inputs, w_all, b_all, logq, targets, sampled = _ssm_inputs(N, S, P, seed=S)
+    sampled = torch.full_like(sampled, int(targets[0]))
+    b_all = b_all.clone()
+    b_all.view(-1)[1::2] += 80.0
+    b_all.view(-1)[2::2] -= 80.0
+    data = _ssm_rounded((inputs, w_all, b_all, logq, targets, sampled), dt, dt)
+    inputs, w_all, b_all = data[:3]
+    adj = b_all.reshape(-1).float() - logq
+    _, rows, dtrue = fused._head_forward(inputs.contiguous(), w_all.contiguous(), adj, targets,
+                                         sampled)
+    torch.cuda.synchronize()
+    assert float(rows[0]) == 0.0 and float(dtrue[0]) == 0.0
+    assert torch.isfinite(rows).all() and torch.isfinite(dtrue).all()
+    ref = _ssm_run("reference", data, torch.float64, torch.float64, None)
+    low = _ssm_run("reference", data, dt, dt, None)
+    for entry in ("head", "loss"):
+        with pytest.MonkeyPatch.context() as mp:
+            if entry == "loss":
+                mp.setenv("PARALLAX_SSM_HEAD", "0")
+            got = _ssm_run(entry, data, dt, dt, None)
+        assert float(got["rows"][0]) == 0.0
+        for k in got:
+            _assert_calibrated("extreme/%s/%s" % (entry, k), got[k], ref[k], low[k], dt)
