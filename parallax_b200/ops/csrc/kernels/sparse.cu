@@ -37,7 +37,11 @@
 #include "optim_rules.cuh"
 #include "sparse_group.cuh"
 
+#include <algorithm>
+#include <climits>
+#include <mutex>
 #include <string>
+#include <unordered_map>
 
 __device__ __forceinline__ unsigned long long px_globaltimer() {
   unsigned long long t;
@@ -72,6 +76,16 @@ __device__ __forceinline__ uint32_t hash_slot(int id) {
   uint32_t x = (uint32_t)id * 0x85EBCA6Bu;
   x ^= x >> 13; x *= 0xC2B2AE35u;
   return x ^ (x >> 16);
+}
+
+// 4 fp32 <-> 4 bf16 (round to nearest even) in 8 bytes
+__device__ __forceinline__ uint2 pack_bf16x4(const float4& v) {
+  __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+  return make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+}
+__device__ __forceinline__ float4 unpack_bf16x4(const uint2& v) {
+  return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u),
+                     __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xffff0000u));
 }
 
 // ------------------------------------------------------------------ lookup
@@ -128,11 +142,10 @@ px_sparse_lookup_kernel(const IdT* __restrict__ ids, int n, LookupArgs a,
           if (!T.out_bf16) {
             st_v4(reinterpret_cast<float4*>(T.out) + (size_t)i * T.D4 + c, v);
           } else {
-            __nv_bfloat162 lo = __floats2bfloat162_rn(__uint_as_float(v.x), __uint_as_float(v.y));
-            __nv_bfloat162 hi = __floats2bfloat162_rn(__uint_as_float(v.z), __uint_as_float(v.w));
             *reinterpret_cast<uint2*>(reinterpret_cast<char*>(T.out) +
                                       ((size_t)i * T.D4 + c) * 8) =
-                make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+                pack_bf16x4(make_float4(__uint_as_float(v.x), __uint_as_float(v.y),
+                                        __uint_as_float(v.z), __uint_as_float(v.w)));
           }
         }
       }
@@ -148,10 +161,8 @@ __device__ __forceinline__ float4 ld_grad4(const GradT* base, size_t f4_index) {
     return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z),
                        __uint_as_float(v.w));
   } else {
-    const uint2 v = *reinterpret_cast<const uint2*>(reinterpret_cast<const char*>(base) +
-                                                    f4_index * 8);
-    return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u),
-                       __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xffff0000u));
+    return unpack_bf16x4(*reinterpret_cast<const uint2*>(reinterpret_cast<const char*>(base) +
+                                                         f4_index * 8));
   }
 }
 
@@ -162,8 +173,7 @@ __device__ __forceinline__ void st_wire4(char* row_base, int c, const float4& v)
                  make_uint4(__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z),
                             __float_as_uint(v.w)));
   } else {
-    __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-    const uint2 o = make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
+    const uint2 o = pack_bf16x4(v);
     asm volatile("st.global.L1::no_allocate.v2.u32 [%0], {%1,%2};"
                  ::"l"(row_base + (size_t)c * 8), "r"(o.x), "r"(o.y) : "memory");
   }
@@ -178,11 +188,16 @@ __device__ __forceinline__ float4 ld_wire4(const char* row_base, int c) {
     uint2 v;
     asm volatile("ld.global.L1::no_allocate.v2.u32 {%0,%1}, [%2];"
                  : "=r"(v.x), "=r"(v.y) : "l"(row_base + (size_t)c * 8) : "memory");
-    return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u),
-                       __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xffff0000u));
+    return unpack_bf16x4(v);
   }
 }
 
+// bf16 shadow of 4 elements of one table row (shadow rows are padded to a multiple of 8)
+__device__ __forceinline__ void store_shadow4(__nv_bfloat16* shadow, size_t row, int D4, int c,
+                                              const float4& w) {
+  *reinterpret_cast<uint2*>(reinterpret_cast<char*>(shadow) + (row * ((D4 + 1) / 2 * 2) + c) * 8) =
+      pack_bf16x4(w);
+}
 
 // optimizer on 4 elements of one table row (+ bf16 shadow refresh); used by the owner kernel on
 // local rows and by the async push on remote rows
@@ -206,12 +221,7 @@ __device__ __forceinline__ void px_row_apply4(int kind, const PxHP& h, const flo
   if (p0) *p0 = s0;
   if (p1) *p1 = s1;
   if (p2) *p2 = s2;
-  if (shadow) {
-    __nv_bfloat162 lo = __floats2bfloat162_rn(w.x, w.y), hi = __floats2bfloat162_rn(w.z, w.w);
-    *reinterpret_cast<uint2*>(reinterpret_cast<char*>(shadow) +
-                              (row * ((D4 + 1) / 2 * 2) + c) * 8) =
-        make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
-  }
+  if (shadow) store_shadow4(shadow, row, D4, c, w);
 }
 
 // same for 8 consecutive elements (two float4 groups 2*c2, 2*c2+1): every load is issued
@@ -653,16 +663,102 @@ struct OwnerArgs {
 
 // Σ over the entries linked from list head e of one 4-element group of a wire row, in fp32
 template <typename WireT>
-__device__ __forceinline__ float4 ld_merged4(const OwnerArgs& a, const char* ring,
+__device__ __forceinline__ float4 ld_merged4(const OwnerArgs& a, const OwnerTable& T,
                                              size_t row_bytes, int e, int c) {
-  float4 g = ld_wire4<WireT>(ring + (size_t)e * row_bytes, c);
+  float4 g = ld_wire4<WireT>(T.ring + (size_t)e * row_bytes, c);
   if (a.use_merge) {
     for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
-      const float4 o = ld_wire4<WireT>(ring + (size_t)x * row_bytes, c);
+      const float4 o = ld_wire4<WireT>(T.ring + (size_t)x * row_bytes, c);
       g.x += o.x; g.y += o.y; g.z += o.z; g.w += o.w;
     }
   }
   return g;
+}
+
+// the same for 8 elements (4-element groups 2*c2, 2*c2+1) of a bf16 wire row into f[8]: one
+// 16-byte load per entry
+__device__ __forceinline__ void ld_merged8(const OwnerArgs& a, const OwnerTable& T,
+                                           size_t row_bytes, int e, int c2, float* f) {
+  Vec16<__nv_bfloat16>::unpack(
+      ld_v4_stream(reinterpret_cast<const uint4*>(T.ring + (size_t)e * row_bytes) + c2), f);
+  if (a.use_merge) {
+    for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
+      float o[8];
+      Vec16<__nv_bfloat16>::unpack(
+          ld_v4_stream(reinterpret_cast<const uint4*>(T.ring + (size_t)x * row_bytes) + c2), o);
+#pragma unroll
+      for (int q = 0; q < 8; ++q) f[q] += o[q];
+    }
+  }
+}
+
+// ---- the entry walk of the owner and owner-norm kernels
+// Entries of all sources form ONE index space [0, total): a (source, j) double loop would hand
+// every half-warp one entry per source — W entries in sequence for the first few half-warps and
+// nothing for the rest.  s_pre[s] is the index of source s's first entry; returns total.
+// Every source delivered a.fixed_cnt entries when it is >= 0, else the count in its header word.
+__device__ __forceinline__ int owner_prefix(const OwnerArgs& a, const GroupGeom& g, int* s_pre) {
+  const uint32_t* cnt = a.hdr + 2 * PX_MAX_RANKS;
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int s = 0; s < g.W; ++s) {
+      s_pre[s] = acc;
+      acc += a.fixed_cnt >= 0 ? a.fixed_cnt : (int)ld_volatile_u32(cnt + s);
+    }
+    s_pre[g.W] = acc;
+  }
+  __syncthreads();
+  return s_pre[g.W];
+}
+
+// index i -> ring entry e = s * cap + j; the search for source s starts at the s passed in
+__device__ __forceinline__ int owner_entry(const OwnerArgs& a, const int* s_pre, int i, int& s) {
+  while (i >= s_pre[s + 1]) ++s;
+  return s * a.cap + (i - s_pre[s]);
+}
+
+// Merge path: every entry pushes itself on the list of its row (at most one entry per source when
+// the senders aggregate locally, so lists are <= W long), then a grid barrier on ctl->bar (all
+// CTAs are co-resident: cooperative launch).  The `stamp` thread times the barrier in t_dbg[6..7].
+__device__ __forceinline__ void owner_link(const OwnerArgs& a, const int* s_pre, int total,
+                                           SparseCtl* ctl, bool stamp) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    int s = 0;
+    const int e = owner_entry(a, s_pre, i, s);
+    const int r = a.ring_ids[e];
+    if (r >= 0) a.next[e] = atomicExch(&a.slotmap[r], e);
+  }
+  if (stamp) ctl->t_dbg[6] = px_globaltimer();
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    atomicAdd(&ctl->bar, 1u);
+    while (ld_volatile_u32(&ctl->bar) < gridDim.x) { }
+    __threadfence();
+  }
+  __syncthreads();
+  if (stamp) ctl->t_dbg[7] = px_globaltimer();
+}
+
+// 16 lanes per entry (two entries per warp in flight).  visit(i, s) runs for every entry i (of
+// source s); head(e, r) for every entry e that heads the list of its row r (without merge: every
+// entry of a row of mine), after which the half-warp resets slotmap[r] for the next step.
+template <typename Visit, typename Head>
+__device__ __forceinline__ void owner_walk(const OwnerArgs& a, const int* s_pre, int total,
+                                           Visit visit, Head head) {
+  const int warps = blockDim.x >> 4;
+  const unsigned hmask = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
+  for (int i = blockIdx.x * warps + (threadIdx.x >> 4); i < total; i += gridDim.x * warps) {
+    int s = 0;
+    const int e = owner_entry(a, s_pre, i, s);
+    const int r = a.ring_ids[e];
+    visit(i, s);
+    if (r < 0) continue;
+    if (a.use_merge && __ldcg(a.slotmap + r) != e) continue;          // not the list head
+    head(e, r);
+    __syncwarp(hmask);
+    if (a.use_merge && (threadIdx.x & 15) == 0) a.slotmap[r] = -1;
+  }
 }
 
 // Family 2 (row-wise Adagrad) on local row r of table T, by the 16 lanes of one half-warp:
@@ -678,12 +774,7 @@ __device__ __forceinline__ float4 ld_merged4(const OwnerArgs& a, const char* rin
 __device__ __forceinline__ void px_store_row4(const OwnerTable& T, size_t row, int c,
                                               const float4& w) {
   reinterpret_cast<float4*>(T.table)[row * T.D4 + c] = w;
-  if (T.shadow) {
-    __nv_bfloat162 lo = __floats2bfloat162_rn(w.x, w.y), hi = __floats2bfloat162_rn(w.z, w.w);
-    *reinterpret_cast<uint2*>(reinterpret_cast<char*>(T.shadow) +
-                              (row * ((T.D4 + 1) / 2 * 2) + c) * 8) =
-        make_uint2(*reinterpret_cast<uint32_t*>(&lo), *reinterpret_cast<uint32_t*>(&hi));
-  }
+  if (T.shadow) store_shadow4(T.shadow, row, T.D4, c, w);
 }
 
 __device__ __forceinline__ void px_sgd4(float step, const float4& g, float4& w) {
@@ -707,7 +798,7 @@ __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const Owner
       const int c = lane + 16 * k;
       if (c < T.D4) {
         wk[k] = wrow[c];
-        gk[k] = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+        gk[k] = ld_merged4<WireT>(a, T, row_bytes, e, c);
       }
     }
 #pragma unroll
@@ -720,7 +811,7 @@ __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const Owner
     }
   } else {
     for (int c = lane; c < T.D4; c += 16) {
-      float4 g = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+      float4 g = ld_merged4<WireT>(a, T, row_bytes, e, c);
       g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
       ss = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, fmaf(g.w, g.w, ss))));
     }
@@ -745,7 +836,7 @@ __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const Owner
     }
   } else {
     for (int c = lane; c < T.D4; c += 16) {
-      float4 g = ld_merged4<WireT>(a, T.ring, row_bytes, e, c);
+      float4 g = ld_merged4<WireT>(a, T, row_bytes, e, c);
       g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
       float4 w = wrow[c];
       px_sgd4(step, g, w);
@@ -783,136 +874,69 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
     __syncthreads();
   }
   if (stamp) ctl->t_own[1] = px_globaltimer();
-  // apply phase: 16 lanes per entry (two entries per warp in flight)
   const int lane = threadIdx.x & 15, warps = blockDim.x >> 4;
   const unsigned hmask = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
-  const uint32_t* cnt = a.hdr + 2 * PX_MAX_RANKS;
-  // entries of all sources form ONE index space [0, total): a (source, j) double loop would
-  // hand every half-warp one entry per source — W entries in sequence for the first few
-  // half-warps and nothing for the rest
   __shared__ int s_pre[PX_MAX_RANKS + 1];
-  if (threadIdx.x == 0) {
-    int acc = 0;
-    for (int s = 0; s < g.W; ++s) {
-      s_pre[s] = acc;
-      acc += a.fixed_cnt >= 0 ? a.fixed_cnt : (int)ld_volatile_u32(cnt + s);
-    }
-    s_pre[g.W] = acc;
-  }
-  __syncthreads();
-  const int total = s_pre[g.W];
-  if (a.use_merge) {
-    // link: every entry pushes itself on the list of its row (at most one entry per source when
-    // the senders aggregate locally, so lists are <= W long)
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-      int s = 0;
-      while (i >= s_pre[s + 1]) ++s;
-      const int e = s * a.cap + (i - s_pre[s]);
-      const int r = a.ring_ids[e];
-      if (r >= 0) a.next[e] = atomicExch(&a.slotmap[r], e);
-    }
-    // grid barrier (all CTAs are co-resident: cooperative launch)
-    if (stamp) ctl->t_dbg[6] = px_globaltimer();
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      atomicAdd(&ctl->bar, 1u);
-      while (ld_volatile_u32(&ctl->bar) < gridDim.x) { }
-      __threadfence();
-    }
-    __syncthreads();
-    if (stamp) ctl->t_dbg[7] = px_globaltimer();
-  }
-  {
-    for (int i = blockIdx.x * warps + (threadIdx.x >> 4); i < total; i += gridDim.x * warps) {
-      int s = 0;
-      while (i >= s_pre[s + 1]) ++s;
-      const int e = s * a.cap + (i - s_pre[s]);
-      const int r = a.ring_ids[e];
-      {
-        // the rows of a batch are scattered over a multi-GB table: every touch is a DRAM
-        // (and usually a TLB) miss.  Prefetch this half-warp's NEXT entry's table / slot rows
-        // into L2 now, so that miss overlaps the work on the current entry.
-        const int in = i + gridDim.x * warps;
-        if (in < total) {
-          int sn = s;
-          while (in >= s_pre[sn + 1]) ++sn;
-          const int rn = a.ring_ids[sn * a.cap + (in - s_pre[sn])];
-          if (rn >= 0) {
-            for (int t = 0; t < a.nt; ++t) {
-              const OwnerTable& T = a.t[t];
-              const size_t off = (size_t)rn * T.D4 * 16;             // row offset in bytes
-              const int lines = (T.D4 * 16 + 127) / 128;
-              for (int l = lane; l < lines; l += 16) {
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) + off + l * 128));
-                if (FAM == 2) {
-                  // one fp32 accumulator per row: its pitch is 4 bytes, not the row's
-                  if (l == 0)
-                    asm volatile("prefetch.global.L2 [%0];" ::"l"(T.slot0 + rn));
-                  continue;
-                }
-                if (T.slot0)
-                  asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.slot0) + off + l * 128));
-                if (T.slot1)
-                  asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.slot1) + off + l * 128));
-              }
-            }
-          }
-        }
-      }
-      if (r < 0) continue;
-      if (a.use_merge) {
-        if (__ldcg(a.slotmap + r) != e) continue;          // not the list head
-      }
-#pragma unroll 1
-      for (int t = 0; t < a.nt; ++t) {
-        const OwnerTable& T = a.t[t];
+  const int total = owner_prefix(a, g, s_pre);
+  if (a.use_merge) owner_link(a, s_pre, total, ctl, stamp);
+  // the rows of a batch are scattered over a multi-GB table: every touch is a DRAM (and usually
+  // a TLB) miss.  Prefetch this half-warp's NEXT entry's table / slot rows into L2 now, so that
+  // miss overlaps the work on the current entry.
+  auto prefetch_next = [&](int i, int s) {
+    const int in = i + gridDim.x * warps;
+    if (in >= total) return;
+    const int rn = a.ring_ids[owner_entry(a, s_pre, in, s)];
+    if (rn < 0) return;
+    for (int t = 0; t < a.nt; ++t) {
+      const OwnerTable& T = a.t[t];
+      const size_t off = (size_t)rn * T.D4 * 16;             // row offset in bytes
+      const int lines = (T.D4 * 16 + 127) / 128;
+      for (int l = lane; l < lines; l += 16) {
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) + off + l * 128));
         if (FAM == 2) {
-          px_rowwise_apply<WireT>(a, T, e, r, lane, hmask);
+          // one fp32 accumulator per row: its pitch is 4 bytes, not the row's
+          if (l == 0)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(T.slot0 + rn));
           continue;
         }
-        const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
-        const float gmul = T.avg * T.hp[HP_GSCALE];
-        const PxHP hp = px_load_hp(T.hp);
-        if (sizeof(WireT) == 2 && (T.D4 & 1) == 0) {
-          // bf16 wire rows: one 16-byte load carries 8 elements = two float4 groups
-          for (int c2 = lane; c2 < T.D4 / 2; c2 += 16) {
-            float f[8];
-            Vec16<__nv_bfloat16>::unpack(
-                ld_v4_stream(reinterpret_cast<const uint4*>(T.ring + (size_t)e * row_bytes) + c2), f);
-            if (a.use_merge) {
-              for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
-                float o[8];
-                Vec16<__nv_bfloat16>::unpack(
-                    ld_v4_stream(reinterpret_cast<const uint4*>(T.ring + (size_t)x * row_bytes) + c2), o);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) f[q] += o[q];
-              }
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q) f[q] *= gmul;
-            px_row_apply8<FAM>(T.kind, hp, f, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
-                               (size_t)r, T.D4, c2);
-          }
-          continue;
-        }
-        for (int cidx = lane; cidx < T.D4; cidx += 16) {
-          float4 gv = ld_wire4<WireT>(T.ring + (size_t)e * row_bytes, cidx);
-          if (a.use_merge) {
-            for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
-              const float4 o = ld_wire4<WireT>(T.ring + (size_t)x * row_bytes, cidx);
-              gv.x += o.x; gv.y += o.y; gv.z += o.z; gv.w += o.w;
-            }
-          }
-          gv.x *= gmul; gv.y *= gmul; gv.z *= gmul; gv.w *= gmul;
-          px_row_apply4<FAM>(T.kind, hp, gv, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
-                             (size_t)r, T.D4, cidx);
-        }
+        if (T.slot0)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.slot0) + off + l * 128));
+        if (T.slot1)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.slot1) + off + l * 128));
       }
-      __syncwarp(hmask);
-      if (a.use_merge && lane == 0) a.slotmap[r] = -1;
     }
-  }
+  };
+  auto apply = [&](int e, int r) {
+#pragma unroll 1
+    for (int t = 0; t < a.nt; ++t) {
+      const OwnerTable& T = a.t[t];
+      if (FAM == 2) {
+        px_rowwise_apply<WireT>(a, T, e, r, lane, hmask);
+        continue;
+      }
+      const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
+      const float gmul = T.avg * T.hp[HP_GSCALE];
+      const PxHP hp = px_load_hp(T.hp);
+      if (sizeof(WireT) == 2 && (T.D4 & 1) == 0) {
+        for (int c2 = lane; c2 < T.D4 / 2; c2 += 16) {
+          float f[8];
+          ld_merged8(a, T, row_bytes, e, c2, f);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) f[q] *= gmul;
+          px_row_apply8<FAM>(T.kind, hp, f, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
+                             (size_t)r, T.D4, c2);
+        }
+        continue;
+      }
+      for (int cidx = lane; cidx < T.D4; cidx += 16) {
+        float4 gv = ld_merged4<WireT>(a, T, row_bytes, e, cidx);
+        gv.x *= gmul; gv.y *= gmul; gv.z *= gmul; gv.w *= gmul;
+        px_row_apply4<FAM>(T.kind, hp, gv, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
+                           (size_t)r, T.D4, cidx);
+      }
+    }
+  };
+  owner_walk(a, s_pre, total, prefetch_next, apply);
   // ---- completion: publish applied[me] = step to every rank (one fence per CTA, see push)
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -946,6 +970,42 @@ static void launch_push(int blocks, size_t smem, cudaStream_t stream, const int3
   }
   px_sparse_push_kernel<GT, WT, AS, FAM><<<blocks, 256, smem, stream>>>(pend_ids, n, a, G, ctl,
                                                                          hbits, dedup);
+}
+
+// The most CTAs of 256 threads of `fn` the device keeps resident at once: the largest grid a
+// cooperative launch of `fn` may have.  Cached per kernel.
+static int coop_max_blocks(const void* fn) {
+  static std::mutex mu;
+  static std::unordered_map<const void*, int> cache;
+  std::lock_guard<std::mutex> lock(mu);
+  int& n = cache[fn];
+  if (n == 0) {
+    int per_sm = 0, dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0);
+    n = std::max(per_sm * sms, 1);
+  }
+  return n;
+}
+
+// Launches the owner-side kernel `fn` with parameters `args`, after a one-warp kernel that waits
+// for every source's `pushed` flag when the entry counts come from those flags.  With merge, `fn`
+// has a grid barrier inside: a cooperative launch of at most PX_NUM_SMS * 4 CTAs, of at most as
+// many as `fn` keeps resident, and of at most `coop_cap`.
+static int launch_owner_side(const void* fn, void** args, const OwnerArgs& a, const GroupGeom& G,
+                             SparseCtl* ctl, int blocks, int coop_cap, cudaStream_t stream) {
+  if (a.fixed_cnt < 0 && G.W > 1) px_sparse_wait_kernel<<<1, 32, 0, stream>>>(a.hdr, ctl, G.W);
+  blocks = std::max(blocks, 1);
+  cudaError_t e;
+  if (a.use_merge) {
+    blocks = std::min({blocks, PX_NUM_SMS * 4, coop_max_blocks(fn), coop_cap});
+    e = cudaLaunchCooperativeKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
+  } else {
+    e = cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
+  }
+  if (e != cudaSuccess) return (int)e;
+  return (int)cudaGetLastError();
 }
 
 extern "C" {
@@ -1078,19 +1138,6 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
     if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
     a.t[t] = tabs[t];
   }
-  if (blocks < 1) blocks = 1;
-  if (fixed_cnt < 0 && G.W > 1)
-    px_sparse_wait_kernel<<<1, 32, 0, stream>>>((const uint32_t*)hdr, (const SparseCtl*)ctl, G.W);
-  static int max_coop = 0;
-  if (max_coop == 0) {
-    int per_sm = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, px_sparse_owner_kernel<float, 1>, 256,
-                                                  0);
-    max_coop = per_sm * sms;
-    if (max_coop < 1) max_coop = 1;
-  }
   SparseCtl* C = (SparseCtl*)ctl;
   const void* fn;
   if (wire_dtype == 0) fn = fam == 0 ? (const void*)px_sparse_owner_kernel<float, 0>
@@ -1100,17 +1147,10 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
           : fam == 1 ? (const void*)px_sparse_owner_kernel<__nv_bfloat16, 1>
                      : (const void*)px_sparse_owner_kernel<__nv_bfloat16, 2>;
   void* args[] = {&a, &G, &C};
-  cudaError_t e;
-  if (use_merge) {
-    // one grid barrier inside: every CTA must be resident
-    if (blocks > max_coop) blocks = max_coop;
-    if (blocks > PX_NUM_SMS * 4) blocks = PX_NUM_SMS * 4;
-    e = cudaLaunchCooperativeKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
-  } else {
-    e = cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
-  }
-  if (e != cudaSuccess) return (int)e;
-  return (int)cudaGetLastError();
+  // Merge grids are also held to the residency of px_sparse_owner_kernel<float, 1> (3 CTAs per
+  // SM on the H100): a tuning cap, under which the benchmark numbers were taken.
+  return launch_owner_side(fn, args, a, G, C, blocks,
+                           coop_max_blocks((const void*)px_sparse_owner_kernel<float, 1>), stream);
 }
 
 }  // extern "C"
@@ -1122,8 +1162,8 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
 // multiplies by, hp[HP_GSCALE], in a private copy of the group's hyper-parameters.
 
 // Σ over the touched rows of ‖avg · hp[HP_GSCALE] · Σ_entries row‖², i.e. exactly the rows
-// px_sparse_owner_kernel would hand to the optimizer, added to *sumsq.  Links entries per
-// row like the owner kernel's merge path (one grid barrier, cooperative launch), resets the
+// px_sparse_owner_kernel would hand to the optimizer, added to *sumsq.  Links and walks the
+// entries with the owner kernel's helpers (one grid barrier, cooperative launch), resets the
 // slotmap entries it linked and returns ctl->bar / ctl->apply_done to 0; publishes no flag
 // and leaves ctl->step alone, so the owner kernel runs next exactly as it would have.
 template <typename WireT>
@@ -1131,66 +1171,25 @@ __global__ void __launch_bounds__(256)
 px_sparse_owner_norm_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl, float* sumsq) {
   __shared__ int s_pre[PX_MAX_RANKS + 1];
   __shared__ double s_part[8];
-  const uint32_t* cnt = a.hdr + 2 * PX_MAX_RANKS;
-  if (threadIdx.x == 0) {
-    int acc = 0;
-    for (int s = 0; s < g.W; ++s) {
-      s_pre[s] = acc;
-      acc += (int)ld_volatile_u32(cnt + s);
-    }
-    s_pre[g.W] = acc;
-  }
-  __syncthreads();
-  const int total = s_pre[g.W];
-  if (a.use_merge) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-      int s = 0;
-      while (i >= s_pre[s + 1]) ++s;
-      const int e = s * a.cap + (i - s_pre[s]);
-      const int r = a.ring_ids[e];
-      if (r >= 0) a.next[e] = atomicExch(&a.slotmap[r], e);
-    }
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      atomicAdd(&ctl->bar, 1u);
-      while (ld_volatile_u32(&ctl->bar) < gridDim.x) { }
-      __threadfence();
-    }
-    __syncthreads();
-  }
-  // 16 lanes per entry, as in the owner kernel; fp64 partial sums
-  const int lane = threadIdx.x & 15, warps = blockDim.x >> 4;
-  const unsigned hmask = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
+  const int total = owner_prefix(a, g, s_pre);
+  if (a.use_merge) owner_link(a, s_pre, total, ctl, false);
+  // fp64 partial sums of 4-element groups
+  const int lane = threadIdx.x & 15;
   double acc = 0.0;
-  for (int i = blockIdx.x * warps + (threadIdx.x >> 4); i < total; i += gridDim.x * warps) {
-    int s = 0;
-    while (i >= s_pre[s + 1]) ++s;
-    const int e = s * a.cap + (i - s_pre[s]);
-    const int r = a.ring_ids[e];
-    if (r < 0) continue;
-    if (a.use_merge && __ldcg(a.slotmap + r) != e) continue;       // not the list head
+  owner_walk(a, s_pre, total, [](int, int) {}, [&](int e, int r) {
 #pragma unroll 1
     for (int t = 0; t < a.nt; ++t) {
       const OwnerTable& T = a.t[t];
       const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
       const float gmul = T.avg * T.hp[HP_GSCALE];
       for (int cidx = lane; cidx < T.D4; cidx += 16) {
-        float4 gv = ld_wire4<WireT>(T.ring + (size_t)e * row_bytes, cidx);
-        if (a.use_merge) {
-          for (int x = __ldcg(a.next + e); x != -1; x = __ldcg(a.next + x)) {
-            const float4 o = ld_wire4<WireT>(T.ring + (size_t)x * row_bytes, cidx);
-            gv.x += o.x; gv.y += o.y; gv.z += o.z; gv.w += o.w;
-          }
-        }
+        float4 gv = ld_merged4<WireT>(a, T, row_bytes, e, cidx);
         gv.x *= gmul; gv.y *= gmul; gv.z *= gmul; gv.w *= gmul;
         acc += (double)gv.x * gv.x + (double)gv.y * gv.y + (double)gv.z * gv.z +
                (double)gv.w * gv.w;
       }
     }
-    __syncwarp(hmask);
-    if (a.use_merge && lane == 0) a.slotmap[r] = -1;
-  }
+  });
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
   __syncthreads();
@@ -1226,33 +1225,11 @@ int px_sparse_owner_norm(const OwnerTable* tabs, int nt, int wire_dtype, const i
   a.nt = nt; a.ring_ids = ring_ids; a.hdr = (uint32_t*)hdr; a.hdrs = nullptr;
   a.slotmap = slotmap; a.next = next; a.cap = cap; a.rank = 0; a.use_merge = use_merge;
   for (int t = 0; t < nt; ++t) a.t[t] = tabs[t];
-  if (blocks < 1) blocks = 1;
-  if (G.W > 1)
-    px_sparse_wait_kernel<<<1, 32, 0, stream>>>((const uint32_t*)hdr, (const SparseCtl*)ctl, G.W);
   const void* fn = wire_dtype == 0 ? (const void*)px_sparse_owner_norm_kernel<float>
                                    : (const void*)px_sparse_owner_norm_kernel<__nv_bfloat16>;
-  static int max_coop[2] = {0, 0};
-  int& mc = max_coop[wire_dtype == 0 ? 0 : 1];
-  if (mc == 0) {
-    int per_sm = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0);
-    mc = per_sm * sms;
-    if (mc < 1) mc = 1;
-  }
   SparseCtl* C = (SparseCtl*)ctl;
   void* args[] = {&a, &G, &C, &sumsq};
-  cudaError_t e;
-  if (use_merge) {
-    if (blocks > mc) blocks = mc;
-    if (blocks > PX_NUM_SMS * 4) blocks = PX_NUM_SMS * 4;
-    e = cudaLaunchCooperativeKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
-  } else {
-    e = cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, 0, stream);
-  }
-  if (e != cudaSuccess) return (int)e;
-  return (int)cudaGetLastError();
+  return launch_owner_side(fn, args, a, G, C, blocks, INT_MAX, stream);
 }
 
 int px_clip_hp(const float* hp, const float* scale, float* out, cudaStream_t stream) {

@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 def _tables(world, V, D, P, opt, run_option="HYBRID", sync=True, average=False,
             local_agg=True, out_dtype=torch.float32, strategy="mod", cap=None, owners=None,
-            boundary=True):
+            boundary=True, blocks=4):
     from tests.gpu_utils import make_world
     from parallax_b200.parallel import modes
     from parallax_b200.parallel.nvlink_backend import NVSparseTable
@@ -25,10 +25,11 @@ def _tables(world, V, D, P, opt, run_option="HYBRID", sync=True, average=False,
     g = torch.Generator().manual_seed(7)
     W0 = torch.randn(V, D, generator=g)
     graph = Graph(torch.nn.Linear(1, 1), optimizer=opt)
+    options = {"sparse_capacity": {"emb.weight": cap or 4096}, "sparse_early_push": False}
+    if blocks is not None:                  # None: the default, sized from the row count
+        options["sparse_blocks"] = blocks
     tabs = [NVSparseTable("emb.weight", W0, P, strategy, opt, f, route, graph, cfg,
-                          out_dtype=out_dtype, owners=owners,
-                          options={"sparse_capacity": {"emb.weight": cap or 4096},
-                                   "sparse_blocks": 4, "sparse_early_push": False})
+                          out_dtype=out_dtype, owners=owners, options=options)
             for f in fabs]
     return fabs, tabs, W0
 
@@ -135,6 +136,55 @@ def test_push_claim_apply(world, run_option, kind, local_agg):
                 torch.testing.assert_close(t.table[:, :D].cpu(), ref_w, rtol=2e-4, atol=2e-5)
         else:
             torch.testing.assert_close(_full(tabs, V, D), ref_w, rtol=2e-4, atol=2e-5)
+    for f in fabs:
+        f.close()
+
+
+@pytest.mark.parametrize("kind", ["ftrl", "centered_rmsprop"])
+def test_bf16_wire_family1_merge_at_default_grid(kind):
+    """bf16 wire, a family-1 rule and the merge path, with `sparse_blocks` at its default:
+    6 000 rows per rank make the owner ask for more CTAs than its bf16 family-1 kernel keeps
+    resident (2 per SM), so the cooperative launch must be capped by that kernel's residency."""
+    from parallax_b200 import consts
+    V, D, P, world, n = 20011, 32, 4, 2, 6000
+    # epsilon keeps the centered RMSProp step a smooth function of g: near eps = 0 it is
+    # lr·sign(g), which a bf16 rounding of a merged row that nearly cancels could flip
+    opt = {"ftrl": optim.Ftrl(0.3, l1_regularization_strength=0.01),
+           "centered_rmsprop": optim.CenteredRMSProp(0.05, momentum=0.5, epsilon=1e-2)}[kind]
+    fabs, tabs, W0 = _tables(world, V, D, P, opt, out_dtype=torch.bfloat16, cap=2 * n,
+                             blocks=None)
+    for t in tabs:
+        t._ensure_capacity(n)
+    for t in tabs:
+        t.warm(n)
+    gen = torch.Generator().manual_seed(13)
+    all_ids, all_g, toks = [], [], []
+    for r, t in enumerate(tabs):
+        ids = torch.randint(0, V, (n,), generator=gen)
+        gr = torch.randn(n, D, generator=gen).bfloat16()
+        rows, pend = t.lookup(ids.cuda())
+        toks.append(pend)
+        all_ids.append(ids)
+        all_g.append(gr)
+    torch.cuda.synchronize()
+    for r, t in enumerate(tabs):
+        t.add_pending(toks[r], all_g[r].cuda())
+        t.begin_step(1)
+    torch.cuda.synchronize()
+    _finish_all(tabs, 1)
+    for t in tabs:
+        assert t.group.wire_dtype == torch.bfloat16 and t.group._use_merge()
+        assert t.group._owner_blocks() > 2 * consts.NUM_SMS
+    ids_c, g_c = torch.cat(all_ids), torch.cat(all_g).float()
+    u, inv = torch.unique(ids_c, return_inverse=True)
+    gsum = torch.zeros(u.numel(), D).index_add_(0, inv, g_c)
+    ref_w = W0.clone()
+    ref_slots = tuple(torch.full_like(W0, v) for v in opt.slot_init())
+    optim.apply_sparse_rows_(kind, ref_w, u, gsum, ref_slots, opt.hyper(1))
+    # duplicated ids are summed in fp32 and rounded to bf16 once when they cross the wire
+    torch.testing.assert_close(_full(tabs, V, D), ref_w, rtol=2e-2, atol=2e-2)
+    for t in tabs:
+        torch.testing.assert_close(t.shadow[:, :D].float(), t.table[:, :D].bfloat16().float())
     for f in fabs:
         f.close()
 
