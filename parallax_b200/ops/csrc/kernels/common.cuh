@@ -52,6 +52,13 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* addr) {
   return v;
 }
 
+// %globaltimer (ns): the device clock of every profiling stamp
+__device__ __forceinline__ unsigned long long px_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
 // 16-byte vector load/store.  Peer loads must not go through the
 // non-coherent path (data changes between steps; L1 is only invalidated at
 // kernel boundaries, which is exactly the granularity we synchronise at).

@@ -85,11 +85,6 @@ __device__ __forceinline__ void st_f32(float* p, const float* f) {
 //  * end: the last CTA to finish (ticket) fences, announces "all my parameter stores are out"
 //    in slot 0 of `ch_end` and waits for the same from every peer; the kernel — and with it the
 //    stream — completes only then.  Slot 1 of `ch_end` holds the ticket counter.
-__device__ __forceinline__ unsigned long long px_timer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 __device__ __forceinline__ void px_rank_signal(uint32_t* const* pads, int slot, int rank, int world,
                                                uint32_t e) {
   if (threadIdx.x < world)
@@ -116,14 +111,14 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
   unsigned long long* dbg = reinterpret_cast<unsigned long long*>(
       epoch_ctr + (PX_NUM_CHANNELS - 1) * PX_MAX_BLOCKS);
   const bool stamp0 = blockIdx.x == 0 && threadIdx.x == 0;
-  if (stamp0) dbg[0] = px_timer();
+  if (stamp0) dbg[0] = px_globaltimer();
   uint32_t e_start = 0;
   if (W > 1 && mode != 2) {
     e_start = ld_volatile_u32(epoch_ctr + slot_s) + 1;
     if (blockIdx.x == 0) px_rank_signal(pads, slot_s, a.rank, W, e_start);
     px_rank_wait(pads, slot_s, a.rank, W, e_start);
   }
-  if (stamp0) dbg[1] = px_timer();
+  if (stamp0) dbg[1] = px_globaltimer();
   const size_t slice = a.n / W;
   const size_t nvec = slice / VN;
   const size_t base = (size_t)a.rank * slice;
@@ -208,7 +203,7 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
     }
   }
   if (mode == 1 && a.sumsq != nullptr) block_atomic_sum(ss, a.sumsq);
-  if (stamp0) dbg[2] = px_timer();
+  if (stamp0) dbg[2] = px_globaltimer();
   if (W > 1) {
     __shared__ bool s_last;
     __syncthreads();
@@ -218,14 +213,14 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
     }
     __syncthreads();
     if (s_last) {
-      if (threadIdx.x == 0) dbg[3] = px_timer();
+      if (threadIdx.x == 0) dbg[3] = px_globaltimer();
       if (mode != 1) {
         const uint32_t e_end = ld_volatile_u32(epoch_ctr + slot_e) + 1;
         px_rank_signal(pads, slot_e, a.rank, W, e_end);
         px_rank_wait(pads, slot_e, a.rank, W, e_end);
         if (threadIdx.x == 0) epoch_ctr[slot_e] = e_end;
       }
-      if (threadIdx.x == 0) dbg[4] = px_timer();
+      if (threadIdx.x == 0) dbg[4] = px_globaltimer();
       if (threadIdx.x == 0) {
         if (mode != 2) epoch_ctr[slot_s] = e_start;
         epoch_ctr[slot_e + 1] = 0;
@@ -235,11 +230,7 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
 }
 
 // device timestamp (ns) — a graph-capturable probe for "exposed communication" measurements
-__global__ void px_stamp_kernel(unsigned long long* slot) {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  *slot = t;
-}
+__global__ void px_stamp_kernel(unsigned long long* slot) { *slot = px_globaltimer(); }
 
 // scale = max_norm / max(sqrt(total), max_norm)  (tf.clip_by_global_norm);
 // also exports the norm and zeroes the accumulator for the next step.

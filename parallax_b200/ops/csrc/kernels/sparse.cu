@@ -43,12 +43,6 @@
 #include <string>
 #include <unordered_map>
 
-__device__ __forceinline__ unsigned long long px_globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
 #define PX_SMEM_PARTS 1024
 
 __device__ __forceinline__ void geom_part(const GroupGeom& g, int id, int& p, int& idx) {
@@ -68,9 +62,10 @@ __device__ __forceinline__ void geom_map(const GroupGeom& g, int id, int& owner,
   local = __ldg(g.part_slot + p) * g.rows_per_part + idx;
 }
 
-__device__ __forceinline__ uint32_t hash_cta(int id) {
+// the CTA of a grid of G that owns id: the push kernel hash-partitions ids over its CTAs
+__device__ __forceinline__ int hash_cta(int id, int G) {
   uint32_t x = (uint32_t)id * 2654435761u;
-  return x ^ (x >> 15);
+  return (int)(((unsigned long long)(x ^ (x >> 15)) * (unsigned)G) >> 32);
 }
 __device__ __forceinline__ uint32_t hash_slot(int id) {
   uint32_t x = (uint32_t)id * 0x85EBCA6Bu;
@@ -345,6 +340,69 @@ __device__ __forceinline__ void stage_ids(const int32_t* __restrict__ ids, int b
   }
 }
 
+// read-only probe of the shared-memory id table: the slot holding id, or -1
+__device__ __forceinline__ int find_key(const int32_t* keys, int H, int id) {
+  uint32_t h = hash_slot(id) & (H - 1);
+  int probes = 0;
+  while (keys[h] != id && keys[h] != -1 && ++probes <= H) h = (h + 1) & (H - 1);
+  return keys[h] == id ? (int)h : -1;
+}
+
+// the factor a row leaves with: ScaleGradients on the sender, × hp[HP_GSCALE] when async
+template <bool ASYNC>
+__device__ __forceinline__ float row_scale(const PushTable& T) {
+  return ASYNC ? T.scale * T.hp[HP_GSCALE] : T.scale;
+}
+
+// Row pi of every member table, its id's only position, by the 16 lanes of a half-warp: into ring
+// slot k of `owner`, id after it (sync; `rings`: the ring bases), or onto row `local` (async).
+template <typename GradT, typename WireT, bool ASYNC, int FAM>
+__device__ __forceinline__ void ship_row(const PushArgs& a, const GroupGeom& g,
+                                         char* const (*rings)[PX_MAX_RANKS], int pi, int owner,
+                                         int local, int k, int sub) {
+#pragma unroll 1
+  for (int t = 0; t < a.nt; ++t) {
+    const PushTable& T = a.t[t];
+    const float mul = row_scale<ASYNC>(T);
+    if (!ASYNC && sizeof(GradT) == 2 && sizeof(WireT) == 2 && (T.D4 & 1) == 0 &&
+        !g.replicated) {
+      // bf16 gradient -> bf16 wire: 16-byte copies, four per lane in flight
+      const int nv = T.D4 / 2;
+      const uint4* src = reinterpret_cast<const uint4*>(T.grads) + (size_t)pi * nv;
+      uint4* dst = reinterpret_cast<uint4*>(
+          rings[t][owner] + ((size_t)a.rank * a.cap + k) * ((size_t)T.D4 * 8));
+#pragma unroll 1
+      for (int c = sub; c < nv; c += 64) {
+        uint4 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          v[u] = c + 16 * u < nv ? ld_v4_stream(src + c + 16 * u) : make_uint4(0, 0, 0, 0);
+        if (mul != 1.f) {
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            float f[8];
+            Vec16<__nv_bfloat16>::unpack(v[u], f);
+#pragma unroll
+            for (int q = 0; q < 8; ++q) f[q] *= mul;
+            v[u] = Vec16<__nv_bfloat16>::pack(f);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (c + 16 * u < nv) st_v4_stream(dst + c + 16 * u, v[u]);
+      }
+      continue;
+    }
+#pragma unroll 1
+    for (int c = sub; c < T.D4; c += 16) {
+      float4 v = ld_grad4<GradT>(reinterpret_cast<const GradT*>(T.grads), (size_t)pi * T.D4 + c);
+      v.x *= mul; v.y *= mul; v.z *= mul; v.w *= mul;
+      emit_row<WireT, ASYNC, FAM>(a, g, t, owner, local, k, c, v);
+    }
+  }
+  if (!ASYNC && sub == 0) emit_id(a, g, owner, local, k);
+}
+
 template <typename GradT, typename WireT, bool ASYNC, int FAM>
 __global__ void __launch_bounds__(256)
 px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, GroupGeom g,
@@ -373,19 +431,23 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     const int t = threadIdx.x / PX_MAX_RANKS, r = threadIdx.x % PX_MAX_RANKS;
     s_ring[t][r] = r < g.W ? a.t[t].rings[r] : nullptr;
   }
-#define GEOM_MAP(id, owner, local)                                                     \
-  do {                                                                                 \
-    if (parts_in_smem) {                                                               \
-      int p_, idx_;                                                                    \
-      geom_part(g, (id), p_, idx_);                                                    \
-      owner = s_part_owner[p_];                                                        \
-      local = s_part_slot[p_] * g.rows_per_part + idx_;                                \
-    } else geom_map(g, (id), owner, local);                                            \
-  } while (0)
+  auto place = [&](int id, int& owner, int& local) {
+    if (parts_in_smem) {
+      int p, idx;
+      geom_part(g, id, p, idx);
+      owner = s_part_owner[p];
+      local = s_part_slot[p] * g.rows_per_part + idx;
+    } else {
+      geom_map(g, id, owner, local);
+    }
+  };
+  auto owner_of = [&](int id) { int owner, local; place(id, owner, local); return owner; };
   const int G = gridDim.x, c_me = blockIdx.x;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  const bool raw_all = !dedup;
-#define PX_DBG(i) do { if (c_me == 0 && threadIdx.x == 0) ctl->t_dbg[i] = px_globaltimer(); } while (0)
+  // CTA 0's thread 0 stamps t_push[0] at the start and t_dbg[i] at the end of each phase
+  auto stamp_phase = [&](int i) {
+    if (c_me == 0 && threadIdx.x == 0) ctl->t_dbg[i] = px_globaltimer();
+  };
   if (c_me == 0 && threadIdx.x == 0) ctl->t_push[0] = px_globaltimer();
   for (int h = threadIdx.x; h < H; h += blockDim.x) { keys[h] = -1; cnt[h] = 0; }
   if (threadIdx.x < PX_MAX_RANKS) s_owner_cnt[threadIdx.x] = 0;
@@ -400,15 +462,11 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     for (int j = threadIdx.x; j < m; j += blockDim.x) {
       const int id = ids_s[j];
       if (id < 0) continue;
-      if (raw_all) {
-        if ((base + j) % G == c_me) {
-          int owner, local;
-          GEOM_MAP(id, owner, local);
-          atomicAdd(&s_owner_cnt[owner], 1);
-        }
+      if (!dedup) {
+        if ((base + j) % G == c_me) atomicAdd(&s_owner_cnt[owner_of(id)], 1);
         continue;
       }
-      if ((int)(((unsigned long long)hash_cta(id) * (unsigned)G) >> 32) != c_me) continue;
+      if (hash_cta(id, G) != c_me) continue;
       uint32_t h = hash_slot(id) & (H - 1);
       int probes = 0;
       while (true) {
@@ -420,15 +478,13 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     }
     __syncthreads();
   }
-  PX_DBG(0);
+  stamp_phase(0);
   if (dedup) {
     // ---- pass 2: one ring slot per unique id, one staging row per duplicated id
     for (int h = threadIdx.x; h < H; h += blockDim.x) {
       const int id = keys[h];
       if (id < 0) continue;
-      int owner, local;
-      GEOM_MAP(id, owner, local);
-      kk[h] = atomicAdd(&s_owner_cnt[owner], 1);
+      kk[h] = atomicAdd(&s_owner_cnt[owner_of(id)], 1);
       dup[h] = cnt[h] > 1 ? atomicAdd(&s_ndup, 1) : -1;
     }
     __syncthreads();
@@ -438,15 +494,8 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
       for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int id = pend_ids[i];
         if (id < 0) continue;
-        if ((int)(((unsigned long long)hash_cta(id) * (unsigned)G) >> 32) != c_me) continue;
-        uint32_t h = hash_slot(id) & (H - 1);
-        int probes = 0;
-        while (keys[h] != id && keys[h] != -1 && ++probes <= H) h = (h + 1) & (H - 1);
-        if (keys[h] != id) {
-          int owner, local;
-          GEOM_MAP(id, owner, local);
-          atomicAdd(&s_owner_cnt[owner], 1);
-        }
+        if (hash_cta(id, G) != c_me) continue;
+        if (find_key(keys, H, id) < 0) atomicAdd(&s_owner_cnt[owner_of(id)], 1);
       }
       __syncthreads();
     }
@@ -464,14 +513,11 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
   // raw entries take the slots after the deduplicated ones of this CTA
   if (dedup && s_overflow > 0) {
     for (int h = threadIdx.x; h < H; h += blockDim.x) {
-      if (keys[h] < 0) continue;
-      int owner, local;
-      GEOM_MAP(keys[h], owner, local);
-      atomicMax(&s_owner_cnt[owner], kk[h] + 1);
+      if (keys[h] >= 0) atomicMax(&s_owner_cnt[owner_of(keys[h])], kk[h] + 1);
     }
     __syncthreads();
   }
-  PX_DBG(1);
+  stamp_phase(1);
   // ---- pass 3: ship unique rows, stage duplicated ones.  Per chunk: (a) every thread scans
   // the staged ids and appends its CTA's positions to a work list in shared memory, (b) the
   // list is processed round-robin by half-warps (16 lanes per row, four 16-byte accesses in
@@ -489,27 +535,20 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     for (int j = threadIdx.x; j < m; j += blockDim.x) {
       const int id = ids_s[j];
       if (id < 0) continue;
-      const bool mine = raw_all ? ((base + j) % G == c_me)
-          : ((int)(((unsigned long long)hash_cta(id) * (unsigned)G) >> 32) == c_me);
+      const bool mine = !dedup ? ((base + j) % G == c_me) : hash_cta(id, G) == c_me;
       if (mine) work[atomicAdd(&s_nwork, 1)] = j;
     }
     __syncthreads();
-    if (base == 0) PX_DBG(2);
+    if (base == 0) stamp_phase(2);
     const int nwork = s_nwork;
 #pragma unroll 1
     for (int wi = wid * 2 + half; wi < nwork; wi += nwarps * 2) {
       const int j = work[wi];
       const int pi = base + j;
       const int pid = ids_s[j];
-      int ph = -1;
-      if (!raw_all) {
-        uint32_t h = hash_slot(pid) & (H - 1);
-        int probes = 0;
-        while (keys[h] != pid && keys[h] != -1 && ++probes <= H) h = (h + 1) & (H - 1);
-        if (keys[h] == pid) ph = (int)h;
-      }
+      const int ph = dedup ? find_key(keys, H, pid) : -1;
       int owner, local;
-      GEOM_MAP(pid, owner, local);
+      place(pid, owner, local);
       int k = 0, pcnt = 1;
       if (ph < 0) {                       // raw entry: its own ring slot
         if (sub == 0) k = s_base_k[owner] + atomicAdd(&s_owner_cnt[owner], 1);
@@ -519,48 +558,7 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
         pcnt = cnt[ph];
       }
       if (pcnt == 1) {
-#pragma unroll 1
-        for (int t = 0; t < a.nt; ++t) {
-          const PushTable& T = a.t[t];
-          const float mul = ASYNC ? T.scale * T.hp[HP_GSCALE] : T.scale;
-          if (!ASYNC && sizeof(GradT) == 2 && sizeof(WireT) == 2 && (T.D4 & 1) == 0 &&
-              !g.replicated) {
-            // bf16 gradient -> bf16 wire: 16-byte copies, four per lane in flight
-            const int nv = T.D4 / 2;
-            const uint4* src = reinterpret_cast<const uint4*>(T.grads) + (size_t)pi * nv;
-            uint4* dst = reinterpret_cast<uint4*>(
-                s_ring[t][owner] + ((size_t)a.rank * a.cap + k) * ((size_t)T.D4 * 8));
-#pragma unroll 1
-            for (int c = sub; c < nv; c += 64) {
-              uint4 v[4];
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                v[u] = c + 16 * u < nv ? ld_v4_stream(src + c + 16 * u) : make_uint4(0, 0, 0, 0);
-              if (mul != 1.f) {
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                  float f[8];
-                  Vec16<__nv_bfloat16>::unpack(v[u], f);
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) f[q] *= mul;
-                  v[u] = Vec16<__nv_bfloat16>::pack(f);
-                }
-              }
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                if (c + 16 * u < nv) st_v4_stream(dst + c + 16 * u, v[u]);
-            }
-            continue;
-          }
-#pragma unroll 1
-          for (int c = sub; c < T.D4; c += 16) {
-            float4 v = ld_grad4<GradT>(reinterpret_cast<const GradT*>(T.grads),
-                                       (size_t)pi * T.D4 + c);
-            v.x *= mul; v.y *= mul; v.z *= mul; v.w *= mul;
-            emit_row<WireT, ASYNC, FAM>(a, g, t, owner, local, k, c, v);
-          }
-        }
-        if (!ASYNC && sub == 0) emit_id(a, g, owner, local, k);
+        ship_row<GradT, WireT, ASYNC, FAM>(a, g, s_ring, pi, owner, local, k, sub);
       } else {
         const int d = s_base_dup + dup[ph];
 #pragma unroll 1
@@ -575,7 +573,7 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     }
     __syncthreads();
   }
-  PX_DBG(3);
+  stamp_phase(3);
   // every position of my duplicated ids is staged now (they are all mine)
   // ---- pass 4: flush duplicated ids (warp per id), re-zero the staging rows
   if (dedup && s_ndup > 0) {
@@ -585,13 +583,13 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
         const int h = h0 + __ffs(dm) - 1;
         dm &= dm - 1;
         int owner, local;
-        GEOM_MAP(keys[h], owner, local);
+        place(keys[h], owner, local);
         const int k = s_base_k[owner] + kk[h];
         const int d = s_base_dup + dup[h];
 #pragma unroll 1
         for (int t = 0; t < a.nt; ++t) {
           const PushTable& T = a.t[t];
-          const float mul = ASYNC ? T.scale * T.hp[HP_GSCALE] : T.scale;
+          const float mul = row_scale<ASYNC>(T);
           float4* src = reinterpret_cast<float4*>(T.staging) + (size_t)d * T.D4;
           for (int c = lane; c < T.D4; c += 32) {
             float4 v = __ldcg(src + c);
@@ -604,7 +602,7 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
       }
     }
   }
-  PX_DBG(4);
+  stamp_phase(4);
   // ---- completion: last CTA publishes counts + `pushed` (sync) / bumps the step (async).
   // One fence per CTA: the barrier orders every thread's stores before thread 0's
   // system-scope fence (cumulativity), which orders them before the ticket and the flag.
@@ -614,7 +612,7 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
     s_last = (atomicAdd(&ctl->push_done, 1u) == gridDim.x - 1);
   }
   __syncthreads();
-  PX_DBG(5);
+  stamp_phase(5);
   if (!s_last) return;
   __threadfence_system();
   const uint32_t step = ctl->step + 1;
@@ -957,20 +955,22 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
 }
 
 // ---------------------------------------------------------------------------
-template <typename GT, typename WT, bool AS, int FAM>
-static void launch_push(int blocks, size_t smem, cudaStream_t stream, const int32_t* pend_ids,
-                        int n, const PushArgs& a, const GroupGeom& G, SparseCtl* ctl, int hbits,
-                        int dedup) {
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(px_sparse_push_kernel<GT, WT, AS, FAM>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         4 * 4 * 8192 + 2 * PX_ID_CHUNK * 4);
-    attr = true;
-  }
-  px_sparse_push_kernel<GT, WT, AS, FAM><<<blocks, 256, smem, stream>>>(pend_ids, n, a, G, ctl,
-                                                                         hbits, dedup);
+// Dynamic shared memory of a push launch whose id table has 1 << hbits slots (SMEM layout above)
+static constexpr int kPushHbitsMax = 13;
+static size_t push_smem_bytes(int hbits) {
+  return ((size_t)4 * sizeof(int32_t) << hbits) + 2 * PX_ID_CHUNK * sizeof(int32_t);
 }
+
+// The push instantiations, [async][bf16 gradients][async: optimizer family, sync: bf16 wire];
+// fp32 gradients never travel narrowed, so that entry is null.
+static const void* const kPushKernels[2][2][2] = {
+    {{(const void*)px_sparse_push_kernel<float, float, false, 0>, nullptr},
+     {(const void*)px_sparse_push_kernel<__nv_bfloat16, float, false, 0>,
+      (const void*)px_sparse_push_kernel<__nv_bfloat16, __nv_bfloat16, false, 0>}},
+    {{(const void*)px_sparse_push_kernel<float, float, true, 0>,
+      (const void*)px_sparse_push_kernel<float, float, true, 1>},
+     {(const void*)px_sparse_push_kernel<__nv_bfloat16, float, true, 0>,
+      (const void*)px_sparse_push_kernel<__nv_bfloat16, float, true, 1>}}};
 
 // The most CTAs of 256 threads of `fn` the device keeps resident at once: the largest grid a
 // cooperative launch of `fn` may have.  Cached per kernel.
@@ -1081,7 +1081,7 @@ static inline int push_hbits(int n, int blocks) {
   // >= 4x the expected ids per CTA, 1024..8192 slots (16 B of SMEM per slot)
   long long want = 4LL * ((n + blocks - 1) / blocks);
   int hb = 10;
-  while ((1LL << hb) < want && hb < 13) ++hb;
+  while ((1LL << hb) < want && hb < kPushHbitsMax) ++hb;
   return hb;
 }
 
@@ -1092,7 +1092,7 @@ int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt
                    int cap, const GroupGeom* g, void* ctl, int rank, int dedup, int max_blocks,
                    cudaStream_t stream) {
   if (nt < 1 || nt > PX_GRP_MAX) return -4;
-  const GroupGeom G = *g;
+  GroupGeom G = *g;
   PushArgs a{};
   a.nt = nt; a.ring_ids = (int32_t* const*)ring_ids_dev; a.hdrs = (uint32_t* const*)hdrs_dev;
   a.cap = cap; a.rank = rank;
@@ -1104,22 +1104,21 @@ int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt
   int blocks = (n + 15) / 16;
   if (blocks > max_blocks) blocks = max_blocks;
   if (blocks < 1) blocks = 1;
-  const int hbits = push_hbits(n, blocks);
-  const size_t smem = ((size_t)4 * sizeof(int32_t) << hbits) + 2 * PX_ID_CHUNK * sizeof(int32_t);
-  SparseCtl* C = (SparseCtl*)ctl;
-#define PUSH(GT, WT, AS, FAM) launch_push<GT, WT, AS, FAM>(blocks, smem, stream, pend_ids, n, a, G, C, hbits, dedup)
+  int hbits = push_hbits(n, blocks);
   if (async && fam == 2) return -7;             // row-wise rules need the merged row
-  if (async) {
-    if (grad_dtype == 0) { if (fam == 0) PUSH(float, float, true, 0); else PUSH(float, float, true, 1); }
-    else { if (fam == 0) PUSH(__nv_bfloat16, float, true, 0); else PUSH(__nv_bfloat16, float, true, 1); }
-  } else if (grad_dtype == 0) {
-    if (wire_dtype != 0) return -5;             // never narrow fp32 gradients
-    PUSH(float, float, false, 0);
-  } else {
-    if (wire_dtype == 0) PUSH(__nv_bfloat16, float, false, 0);
-    else PUSH(__nv_bfloat16, __nv_bfloat16, false, 0);
-  }
-#undef PUSH
+  const void* fn = kPushKernels[async != 0][grad_dtype != 0][async ? fam : wire_dtype != 0];
+  if (fn == nullptr) return -5;                 // never narrow fp32 gradients
+  static std::once_flag attr;
+  std::call_once(attr, [] {
+    for (const auto& by_mode : kPushKernels)
+      for (const auto& by_grad : by_mode)
+        for (const void* k : by_grad)
+          if (k) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)push_smem_bytes(kPushHbitsMax));
+  });
+  SparseCtl* C = (SparseCtl*)ctl;
+  void* args[] = {&pend_ids, &n, &a, &G, &C, &hbits, &dedup};
+  cudaLaunchKernel(fn, dim3(blocks), dim3(256), args, push_smem_bytes(hbits), stream);
   return (int)cudaGetLastError();
 }
 

@@ -729,7 +729,6 @@ class NVSparseGroup(object):
         mode).  Separate from `stage_apply` so that a world simulated on one GPU can
         enqueue every rank's push before any rank's (spinning) owner kernel."""
         cs = stream if stream is not None else self.fabric.comm_stream
-        nt = len(self.tables)
         pend_ids, grads = self._take_calls()
         if pend_ids is None:
             pend_ids = torch.empty(0, dtype=torch.int32, device=self.device)
@@ -759,7 +758,22 @@ class NVSparseGroup(object):
                 pend_ids.record_stream(cs)
                 for g in grads:
                     g.record_stream(cs)
-        descs = (ops.PushTable * nt)()
+        descs = self._push_tables(grads, sync)
+        self._keep = (pend_ids, grads, descs)
+        _count()
+        ops.check(ops.lib().px_sparse_push(
+            _vp(pend_ids.data_ptr()), n, descs, len(self.tables), _DT[gdt],
+            _DT[self.wire_dtype] if sync else 0, 0 if sync else 1,
+            _vp(self.ids_dev.data_ptr()) if sync else _vp(0),
+            _vp(self.hdrs_dev.data_ptr()) if sync else _vp(0), self.cap,
+            ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
+            1 if self.local_aggregation else 0, self.max_blocks, _sp(cs)), "sparse_push")
+
+    def _push_tables(self, grads, sync):
+        """PushTable per member table, shipping gradient rows `grads[i]`: into every owner's
+        receive ring (`sync`, ScaleGradients on the sender when the boundary optimisation is
+        on), or through the optimizer onto every owner's table rows (async)."""
+        descs = (ops.PushTable * len(self.tables))()
         for d, t, g in zip(descs, self.tables, grads):
             d.grads, d.staging = g.data_ptr(), t.staging.data_ptr()
             d.hp, d.D4, d.kind = self.hp.dev.data_ptr(), t.D4, _optim.KIND_ID[t.kind]
@@ -773,15 +787,7 @@ class NVSparseGroup(object):
                 d.slot2s = t.dev_ptrs("slot2").data_ptr() if t.nslots > 2 else 0
                 d.shadows = t.dev_ptrs("shadow").data_ptr() if t.use_shadow else 0
                 d.scale = t.scale
-        self._keep = (pend_ids, grads, descs)
-        _count()
-        ops.check(ops.lib().px_sparse_push(
-            _vp(pend_ids.data_ptr()), n, descs, nt, _DT[gdt],
-            _DT[self.wire_dtype] if sync else 0, 0 if sync else 1,
-            _vp(self.ids_dev.data_ptr()) if sync else _vp(0),
-            _vp(self.hdrs_dev.data_ptr()) if sync else _vp(0), self.cap,
-            ctypes.byref(self.geom), _vp(self.ctl.data_ptr()), self.rank,
-            1 if self.local_aggregation else 0, self.max_blocks, _sp(cs)), "sparse_push")
+        return descs
 
     def _owner_tables(self, rings, sender_scaled, hp=None):
         """OwnerTable per member table, merging the rows at device address rings[i]; the
