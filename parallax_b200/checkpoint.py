@@ -75,6 +75,9 @@ def save_sharded(engine, path, is_chief):
         files = ["sparse-%s-rank%d.pt" % (_safe(name), r) for r in writers]
         manifest["sparse"][name] = {
             "V": t.V, "D": t.D, "nslots": t.nslots, "slot_dim": _table_slot_dim(t),
+            # rows as the master stores them: "bfloat16" for sparse_weights="bf16" (a
+            # manifest without the field holds fp32 rows)
+            "weight_dtype": str(getattr(t, "weight_dtype", torch.float32)).replace("torch.", ""),
             "files": files,
             "placement": [t.layout.P, t.layout.strategy, t.layout.world, t.layout.owners,
                           bool(t.replicated)]}
@@ -190,7 +193,8 @@ def _slot_dim(ent):
 
 def assemble_table(path, name, manifest=None):
     """One sparse variable of a sharded checkpoint as full logical tensors
-    ``{"weight": [V, D], "slots": [[V, D] or [V, 1] (row-wise), ...]}`` — no engine, no GPU:
+    ``{"weight": [V, D], "slots": [[V, D] or [V, 1] (row-wise), ...]}``, fp32 (bf16 weight
+    rows are widened exactly) — no engine, no GPU:
     what an offline tool (`tools/inspect_checkpoint`, an evaluation script on another
     machine) needs."""
     man = manifest or read_manifest(path)
@@ -200,9 +204,9 @@ def assemble_table(path, name, manifest=None):
     for fn in ent["files"]:
         sh = torch.load(os.path.join(path, fn), map_location="cpu", weights_only=False)
         if w is None:
-            w = torch.zeros(V, D, dtype=sh["weight"].dtype)
+            w = torch.zeros(V, D, dtype=torch.float32)
             slots = [torch.zeros(V, _slot_dim(ent), dtype=s_.dtype) for s_ in sh["slots"][:ns]]
-        w[sh["ids"]] = sh["weight"]
+        w[sh["ids"]] = sh["weight"].float()
         for dst, src in zip(slots, sh["slots"]):
             dst[sh["ids"]] = src
         seen += int(sh["ids"].numel())

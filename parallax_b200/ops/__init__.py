@@ -42,7 +42,8 @@ class OwnerTable(ctypes.Structure):
     _fields_ = [("ring", c_void_p), ("table", c_void_p), ("slot0", c_void_p),
                 ("slot1", c_void_p), ("slot2", c_void_p), ("shadow", c_void_p),
                 ("hp", c_void_p), ("D4", c_int), ("kind", c_int), ("avg", c_float),
-                ("D", c_int)]
+                ("D", c_int), ("slot_part", c_void_p), ("seed", ctypes.c_uint32),
+                ("w_bf16", c_int)]
 
 
 _SIGS = {
@@ -86,7 +87,7 @@ _SIGS = {
                                  c_int, c_void_p, ctypes.POINTER(GroupGeom), c_void_p,
                                  c_void_p, c_int, c_void_p]),
     "px_full_softmax_nll": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
-                                    c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
+                                    c_int, c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
                                     c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
     "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PushTable), c_int, c_int,

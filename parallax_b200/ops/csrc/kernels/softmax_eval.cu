@@ -32,7 +32,8 @@ constexpr float EV_LOG2E = 1.4426950408889634f;
 
 struct EvalArgs {
   const __nv_bfloat16* const* w;    // [W] bf16 shadow rows of the weight table on every rank
-  const float* const* b;            // [W] fp32 master rows of the bias table on every rank
+  const void* const* b;             // [W] bias rows on every rank: fp32 master rows, or the bf16
+                                    // master of a sparse_weights="bf16" table
   const int* row_cnt;               // [owners][slots] real rows of the partition in each slot
   const uint32_t* applied;          // this rank's group header: applied[W]
   const SparseCtl* ctl;
@@ -60,6 +61,14 @@ __device__ __forceinline__ bool ev_row_real(const EvalArgs& a, const int* cnt, i
 // Roles as in gemm_tc.cu: warpgroup 0 produces (thread 0 issues the X TMA loads), warpgroups
 // 1 and 2 each own 64 rows of the 128-row X tile and run wgmma m64×BV×16 against the resident
 // table block.  All 384 threads load the table block between work items.
+// bias element 0 of a 16-byte aligned row, widened to fp32
+__device__ __forceinline__ float ev_bias(const float* row) { return __uint_as_float(ld_v4(row).x); }
+__device__ __forceinline__ float ev_bias(const __nv_bfloat16* row) {
+  return __uint_as_float(ld_v4(row).x << 16);
+}
+
+// BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows)
+template <typename BiasT>
 __global__ void __launch_bounds__(THREADS, 1)
 px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs a) {
   constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
@@ -122,7 +131,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs 
       const int lr = r0 + threadIdx.x;
       float bv = -INFINITY;
       if (ev_row_real(a, cnt, lr))
-        bv = __uint_as_float(ld_v4(a.b[owner] + (size_t)lr * a.b_pitch).x);
+        bv = ev_bias(reinterpret_cast<const BiasT*>(a.b[owner]) + (size_t)lr * a.b_pitch);
       s_bias[threadIdx.x] = bv;
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // st.shared -> wgmma reads
@@ -202,11 +211,12 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs 
   }
 }
 
+template <typename BiasT>
 __global__ void __launch_bounds__(256)
 px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, int K,
                                const __nv_bfloat16* __restrict__ X,
                                const __nv_bfloat16* __restrict__ wt, int wt_pitch,
-                               const float* __restrict__ bt, int bt_pitch,
+                               const BiasT* __restrict__ bt, int bt_pitch,
                                const long long* __restrict__ targets, int V,
                                float* __restrict__ nll) {
   const int lane = threadIdx.x & 31;
@@ -234,7 +244,7 @@ px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, i
     d = warp_sum(d);
     if (lane == 0) {
       const long long t = targets[row];
-      nll[row] = (t >= 0 && t < V) ? c.x + logf(c.y) - (d + bt[(size_t)row * bt_pitch])
+      nll[row] = (t >= 0 && t < V) ? c.x + logf(c.y) - (d + (float)bt[(size_t)row * bt_pitch])
                                    : __int_as_float(0x7fc00000);
     }
   }
@@ -250,24 +260,26 @@ extern "C" {
 
 // nll[N] (fp32) of X [N, K] (bf16, K-contiguous) against a (weight, bias) co-lookup group.
 //   w_ptrs / b_ptrs: device arrays of every rank's weight shadow (bf16, row pitch w_pitch) and
-//                    bias master rows (fp32, row pitch b_pitch, a multiple of 4);
+//                    bias master rows (fp32, or bf16 when b_bf16; row pitch b_pitch elements,
+//                    16 bytes apart or a multiple of them);
 //   row_cnt:         [owners][slots] real rows of the partition stored in each slot (owners = 1
 //                    for a replicated layout, else W);
 //   ws:              fp32 [ws_ctas][N][2] scratch, the grid is at most ws_ctas CTAs;
-//   targets:         int64 [N]; wt / bt: the targets' rows from the group lookup (same pitches).
+//   targets:         int64 [N]; wt / bt: the targets' rows from the group lookup (same pitches
+//                    and types).
 // Returns 0, a negative argument error, or a CUDA error code.
 int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
-                        const void* b_ptrs, int b_pitch, const int* row_cnt, int slots,
-                        const GroupGeom* g, int rank, const void* hdr_mine, const void* ctl,
-                        int wait, void* ws, int ws_ctas, const long long* targets, const void* wt,
-                        const float* bt, float* nll, cudaStream_t stream) {
+                        const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                        int slots, const GroupGeom* g, int rank, const void* hdr_mine,
+                        const void* ctl, int wait, void* ws, int ws_ctas, const long long* targets,
+                        const void* wt, const void* bt, float* nll, cudaStream_t stream) {
   using namespace tc;
   if (N <= 0) return 0;
-  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % 4) return -1;
+  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % (b_bf16 ? 8 : 4)) return -1;
   if (ws_ctas < 1 || slots < 1) return -2;
   const GroupGeom G = *g;
   EvalArgs a;
-  a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const float* const*)b_ptrs;
+  a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const void* const*)b_ptrs;
   a.row_cnt = row_cnt;
   a.applied = reinterpret_cast<const uint32_t*>(hdr_mine) + PX_MAX_RANKS;
   a.ctl = (const SparseCtl*)ctl; a.ws = (float2*)ws;
@@ -285,16 +297,25 @@ int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_p
   constexpr int SMEM_MAX = ev_smem_bytes(EV_KMAX / BK);
   static bool set = false;
   if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         SMEM_MAX);
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<float>,
+                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<__nv_bfloat16>,
+                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
     set = true;
   }
-  px_full_softmax_lse_kernel<<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
   int blocks = (N + 7) / 8;
   if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
-  px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
-      (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt, w_pitch,
-      bt, b_pitch, targets, G.V, nll);
+  if (b_bf16) {
+    px_full_softmax_lse_kernel<__nv_bfloat16><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
+    px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
+        (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
+        w_pitch, (const __nv_bfloat16*)bt, b_pitch, targets, G.V, nll);
+  } else {
+    px_full_softmax_lse_kernel<float><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
+    px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
+        (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
+        w_pitch, (const float*)bt, b_pitch, targets, G.V, nll);
+  }
   return (int)cudaGetLastError();
 }
 

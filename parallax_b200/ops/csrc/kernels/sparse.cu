@@ -83,6 +83,49 @@ __device__ __forceinline__ float4 unpack_bf16x4(const uint2& v) {
                      __uint_as_float(v.y << 16), __uint_as_float(v.y & 0xffff0000u));
 }
 
+// ---- stochastic rounding of bf16 master rows (sparse_weights="bf16"); `optim.py` holds the same
+// hash and rounding in torch arithmetic, and the two agree bit for bit.
+// The 16 random bits of element (row, col) are a hash of the table's seed, the global step, the
+// row's GLOBAL id and the column only: replicas, world sizes and partitionings round alike.
+__device__ __forceinline__ uint32_t sr_mix(uint32_t x) {
+  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu;
+  return x ^ (x >> 16);
+}
+__device__ __forceinline__ uint32_t sr_row_key(uint32_t seed, uint32_t step, uint32_t gid) {
+  return sr_mix(sr_mix(seed ^ step) ^ gid);
+}
+// bf16 bits of finite x: the top half of (bits(x) + r), r uniform in [0, 2^16) — x rounds away
+// from zero with probability equal to its fraction of an ulp.  Inf stays Inf, NaN stays NaN.
+__device__ __forceinline__ uint32_t sr_bf16(float x, uint32_t key, uint32_t col) {
+  const uint32_t u = __float_as_uint(x);
+  if ((u & 0x7f800000u) == 0x7f800000u) return (u >> 16) | ((u & 0x7fffffu) ? 0x40u : 0u);
+  return (u + (sr_mix(key ^ col) >> 16)) >> 16;
+}
+// 4 elements, columns col .. col+3 of the row with hash key `key`
+__device__ __forceinline__ uint2 pack_bf16x4_sr(const float4& v, uint32_t key, uint32_t col) {
+  return make_uint2(sr_bf16(v.x, key, col) | (sr_bf16(v.y, key, col + 1) << 16),
+                    sr_bf16(v.z, key, col + 2) | (sr_bf16(v.w, key, col + 3) << 16));
+}
+
+// 4 master elements (float4 group c) of row `row`: fp32 rows of D4 groups, or bf16 rows padded to
+// a multiple of 8 columns (the shadow's layout)
+__device__ __forceinline__ size_t bf16_row_groups(int D4) { return (size_t)((D4 + 1) / 2 * 2); }
+__device__ __forceinline__ float4 ld_master4(const float* t, size_t row, int D4, int c) {
+  return reinterpret_cast<const float4*>(t)[row * D4 + c];
+}
+__device__ __forceinline__ float4 ld_master4(const __nv_bfloat16* t, size_t row, int D4, int c) {
+  return unpack_bf16x4(reinterpret_cast<const uint2*>(t)[row * bf16_row_groups(D4) + c]);
+}
+// ... and their store; a bf16 row is rounded stochastically with the row's hash key
+__device__ __forceinline__ void st_master4(float* t, size_t row, int D4, int c, const float4& w,
+                                           uint32_t) {
+  reinterpret_cast<float4*>(t)[row * D4 + c] = w;
+}
+__device__ __forceinline__ void st_master4(__nv_bfloat16* t, size_t row, int D4, int c,
+                                           const float4& w, uint32_t key) {
+  reinterpret_cast<uint2*>(t)[row * bf16_row_groups(D4) + c] = pack_bf16x4_sr(w, key, 4 * c);
+}
+
 // ------------------------------------------------------------------ lookup
 struct LookupTable {
   const void* const* srcs;      // device array[W]: fp32 tables or bf16 shadows of every rank
@@ -195,55 +238,69 @@ __device__ __forceinline__ void store_shadow4(__nv_bfloat16* shadow, size_t row,
 }
 
 // optimizer on 4 elements of one table row (+ bf16 shadow refresh); used by the owner kernel on
-// local rows and by the async push on remote rows
-template <int FAM>
+// local rows and by the async push on remote rows.  MT: the master rows' type; a bf16 master
+// (no shadow) is rounded stochastically with the row's hash key `key`.
+template <int FAM, typename MT = float>
 __device__ __forceinline__ void px_row_apply4(int kind, const PxHP& h, const float4& g,
-                                              float* table, float* slot0, float* slot1,
+                                              MT* table, float* slot0, float* slot1,
                                               float* slot2, __nv_bfloat16* shadow, size_t row,
-                                              int D4, int c) {
+                                              int D4, int c, uint32_t key = 0) {
   const size_t off = row * D4 + c;
-  float4* pw = reinterpret_cast<float4*>(table) + off;
   float4* p0 = slot0 ? reinterpret_cast<float4*>(slot0) + off : nullptr;
   float4* p1 = slot1 ? reinterpret_cast<float4*>(slot1) + off : nullptr;
   float4* p2 = (FAM == 1 && slot2) ? reinterpret_cast<float4*>(slot2) + off : nullptr;
   const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 w = *pw, s0 = z, s1 = z, s2 = z;
+  float4 w = ld_master4(table, row, D4, c), s0 = z, s1 = z, s2 = z;
   if (p0) s0 = *p0;
   if (p1) s1 = *p1;
   if (p2) s2 = *p2;
   px_rule4<FAM>(kind, h, g, w, s0, s1, s2);
-  *pw = w;
+  st_master4(table, row, D4, c, w, key);
   if (p0) *p0 = s0;
   if (p1) *p1 = s1;
   if (p2) *p2 = s2;
-  if (shadow) store_shadow4(shadow, row, D4, c, w);
+  if (sizeof(MT) == 4 && shadow) store_shadow4(shadow, row, D4, c, w);
 }
 
 // same for 8 consecutive elements (two float4 groups 2*c2, 2*c2+1): every load is issued
 // before the first store (table / slot pointers may alias as far as the compiler knows, so
 // two back-to-back px_row_apply4 calls would serialise load -> store -> load)
-template <int FAM>
+template <int FAM, typename MT = float>
 __device__ __forceinline__ void px_row_apply8(int kind, const PxHP& h, const float* g,
-                                              float* table, float* slot0, float* slot1,
+                                              MT* table, float* slot0, float* slot1,
                                               float* slot2, __nv_bfloat16* shadow, size_t row,
-                                              int D4, int c2) {
+                                              int D4, int c2, uint32_t key = 0) {
   const size_t off = row * D4 + 2 * c2;
-  float4* pw = reinterpret_cast<float4*>(table) + off;
   float4* p0 = slot0 ? reinterpret_cast<float4*>(slot0) + off : nullptr;
   float4* p1 = slot1 ? reinterpret_cast<float4*>(slot1) + off : nullptr;
   float4* p2 = (FAM == 1 && slot2) ? reinterpret_cast<float4*>(slot2) + off : nullptr;
+  float4* pw = reinterpret_cast<float4*>(table) + off;                        // fp32 master
+  uint4* pb = reinterpret_cast<uint4*>(table) + row * ((D4 + 1) / 2) + c2;   // bf16 master
   const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 w[2] = {pw[0], pw[1]}, s0[2] = {z, z}, s1[2] = {z, z}, s2[2] = {z, z};
+  float4 w[2] = {z, z}, s0[2] = {z, z}, s1[2] = {z, z}, s2[2] = {z, z};
+  if constexpr (sizeof(MT) == 4) {
+    w[0] = pw[0]; w[1] = pw[1];
+  } else {
+    float f[8];
+    Vec16<__nv_bfloat16>::unpack(*pb, f);
+    w[0] = make_float4(f[0], f[1], f[2], f[3]);
+    w[1] = make_float4(f[4], f[5], f[6], f[7]);
+  }
   if (p0) { s0[0] = p0[0]; s0[1] = p0[1]; }
   if (p1) { s1[0] = p1[0]; s1[1] = p1[1]; }
   if (p2) { s2[0] = p2[0]; s2[1] = p2[1]; }
   px_rule4<FAM>(kind, h, make_float4(g[0], g[1], g[2], g[3]), w[0], s0[0], s1[0], s2[0]);
   px_rule4<FAM>(kind, h, make_float4(g[4], g[5], g[6], g[7]), w[1], s0[1], s1[1], s2[1]);
-  pw[0] = w[0]; pw[1] = w[1];
+  if constexpr (sizeof(MT) == 4) {
+    pw[0] = w[0]; pw[1] = w[1];
+  } else {
+    const uint2 lo = pack_bf16x4_sr(w[0], key, 8 * c2), hi = pack_bf16x4_sr(w[1], key, 8 * c2 + 4);
+    *pb = make_uint4(lo.x, lo.y, hi.x, hi.y);
+  }
   if (p0) { p0[0] = s0[0]; p0[1] = s0[1]; }
   if (p1) { p1[0] = s1[0]; p1[1] = s1[1]; }
   if (p2) { p2[0] = s2[0]; p2[1] = s2[1]; }
-  if (shadow) {
+  if (sizeof(MT) == 4 && shadow) {
     const float f[8] = {w[0].x, w[0].y, w[0].z, w[0].w, w[1].x, w[1].y, w[1].z, w[1].w};
     st_v4(reinterpret_cast<uint4*>(shadow) + row * ((D4 + 1) / 2) + c2,
           Vec16<__nv_bfloat16>::pack(f));
@@ -638,13 +695,17 @@ px_sparse_push_kernel(const int32_t* __restrict__ pend_ids, int n, PushArgs a, G
 // ------------------------------------------------------------------ owner
 struct OwnerTable {
   char* ring;                   // my receive ring: [W_src][cap][D4*4] WireT
-  float* table; float* slot0; float* slot1; float* slot2;
+  void* table;                  // master rows: fp32 [rows][D4*4], or bf16 [rows][Dps] (w_bf16)
+  float* slot0; float* slot1; float* slot2;
   __nv_bfloat16* shadow;        // bf16 copy read by lookups (or null)
   const float* hp;
   int D4, kind;
   float avg;                    // 1/num_workers (average_sparse) × owner-side gradient scale
   int D;                        // true row width, read by family 2 only (the row-wise rule
                                 // averages Σg² over it); fills the 8-byte alignment tail
+  const int32_t* slot_part;     // bf16 master: partition held in each of my slots (global ids)
+  uint32_t seed;                // bf16 master: the table's stochastic-rounding seed
+  int w_bf16;                   // 1: bf16 master rows, stochastically rounded; no shadow
 };
 struct OwnerArgs {
   OwnerTable t[PX_GRP_MAX];
@@ -769,10 +830,21 @@ __device__ __forceinline__ void owner_walk(const OwnerArgs& a, const int* s_pre,
 // it into L2).  Padding columns carry zero gradient and stay unchanged.
 #define PX_RW_REG_F4 2
 
+template <typename MT>
 __device__ __forceinline__ void px_store_row4(const OwnerTable& T, size_t row, int c,
-                                              const float4& w) {
-  reinterpret_cast<float4*>(T.table)[row * T.D4 + c] = w;
-  if (T.shadow) store_shadow4(T.shadow, row, T.D4, c, w);
+                                              const float4& w, uint32_t key) {
+  st_master4(reinterpret_cast<MT*>(T.table), row, T.D4, c, w, key);
+  if (sizeof(MT) == 4 && T.shadow) store_shadow4(T.shadow, row, T.D4, c, w);
+}
+
+// the global id of my local row r (a bf16 master's rounding is keyed by it): the inverse of
+// geom_map for the partition T.slot_part holds in r's slot
+__device__ __forceinline__ uint32_t owner_gid(const GroupGeom& g, const OwnerTable& T, int r) {
+  if (g.replicated) return (uint32_t)r;
+  const int slot = r / g.rows_per_part, idx = r - slot * g.rows_per_part;
+  const int p = __ldg(T.slot_part + slot);
+  if (g.strategy == 0) return (uint32_t)(idx * g.P + p);
+  return (uint32_t)(p < g.extras ? p * (g.base + 1) + idx : p * g.base + g.extras + idx);
 }
 
 __device__ __forceinline__ void px_sgd4(float step, const float4& g, float4& w) {
@@ -780,14 +852,15 @@ __device__ __forceinline__ void px_sgd4(float step, const float4& g, float4& w) 
   w.z = fmaf(-step, g.z, w.z); w.w = fmaf(-step, g.w, w.w);
 }
 
-template <typename WireT>
+template <typename WireT, typename MT>
 __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const OwnerTable& T, int e,
-                                                 int r, int lane, unsigned hmask) {
+                                                 int r, int lane, unsigned hmask, uint32_t key) {
   const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
   const float gmul = T.avg * T.hp[HP_GSCALE];
   const float s_old = lane == 0 ? T.slot0[r] : 0.f;
   const bool in_regs = T.D4 <= 16 * PX_RW_REG_F4;
-  const float4* wrow = reinterpret_cast<const float4*>(T.table) + (size_t)r * T.D4;
+  const MT* wtab = reinterpret_cast<const MT*>(T.table);
+  const float4* wrow = reinterpret_cast<const float4*>(T.table) + (size_t)r * T.D4;   // fp32
   float4 gk[PX_RW_REG_F4], wk[PX_RW_REG_F4];
   float ss = 0.f;
   if (in_regs) {
@@ -795,7 +868,8 @@ __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const Owner
     for (int k = 0; k < PX_RW_REG_F4; ++k) {
       const int c = lane + 16 * k;
       if (c < T.D4) {
-        wk[k] = wrow[c];
+        if constexpr (sizeof(MT) == 4) wk[k] = wrow[c];
+        else wk[k] = ld_master4(wtab, (size_t)r, T.D4, c);
         gk[k] = ld_merged4<WireT>(a, T, row_bytes, e, c);
       }
     }
@@ -829,16 +903,18 @@ __device__ __forceinline__ void px_rowwise_apply(const OwnerArgs& a, const Owner
       const int c = lane + 16 * k;
       if (c < T.D4) {
         px_sgd4(step, gk[k], wk[k]);
-        px_store_row4(T, (size_t)r, c, wk[k]);
+        px_store_row4<MT>(T, (size_t)r, c, wk[k], key);
       }
     }
   } else {
     for (int c = lane; c < T.D4; c += 16) {
       float4 g = ld_merged4<WireT>(a, T, row_bytes, e, c);
       g.x *= gmul; g.y *= gmul; g.z *= gmul; g.w *= gmul;
-      float4 w = wrow[c];
+      float4 w;
+      if constexpr (sizeof(MT) == 4) w = wrow[c];
+      else w = ld_master4(wtab, (size_t)r, T.D4, c);
       px_sgd4(step, g, w);
-      px_store_row4(T, (size_t)r, c, w);
+      px_store_row4<MT>(T, (size_t)r, c, w, key);
     }
   }
 }
@@ -857,8 +933,8 @@ __global__ void px_sparse_wait_kernel(const uint32_t* hdr, const SparseCtl* ctl,
 
 // ONE launch: wait for every source, merge rows that several sources touched, apply the sparse
 // optimizer once per touched row, publish `applied`.  Launched cooperatively when use_merge (one
-// grid barrier between linking and applying).
-template <typename WireT, int FAM>
+// grid barrier between linking and applying).  MT: the type of the master rows.
+template <typename WireT, int FAM, typename MT = float>
 __global__ void __launch_bounds__(256, FAM == 1 ? 2 : 4)
 px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
   __shared__ bool s_last;
@@ -890,7 +966,13 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
       const size_t off = (size_t)rn * T.D4 * 16;             // row offset in bytes
       const int lines = (T.D4 * 16 + 127) / 128;
       for (int l = lane; l < lines; l += 16) {
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) + off + l * 128));
+        if constexpr (sizeof(MT) == 4) {
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) + off + l * 128));
+        } else if (l < ((T.D4 + 1) / 2 * 16 + 127) / 128) {
+          // a bf16 master row is (D4 + 1) / 2 16-byte vectors long
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(T.table) +
+                                                        (size_t)rn * ((T.D4 + 1) / 2) * 16 + l * 128));
+        }
         if (FAM == 2) {
           // one fp32 accumulator per row: its pitch is 4 bytes, not the row's
           if (l == 0)
@@ -908,8 +990,11 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
 #pragma unroll 1
     for (int t = 0; t < a.nt; ++t) {
       const OwnerTable& T = a.t[t];
+      uint32_t key = 0;             // the row's rounding key (bf16 master)
+      if constexpr (sizeof(MT) == 2)
+        key = sr_row_key(T.seed, (uint32_t)T.hp[HP_STEP], owner_gid(g, T, r));
       if (FAM == 2) {
-        px_rowwise_apply<WireT>(a, T, e, r, lane, hmask);
+        px_rowwise_apply<WireT, MT>(a, T, e, r, lane, hmask, key);
         continue;
       }
       const size_t row_bytes = (size_t)T.D4 * 4 * sizeof(WireT);
@@ -921,16 +1006,16 @@ px_sparse_owner_kernel(OwnerArgs a, GroupGeom g, SparseCtl* ctl) {
           ld_merged8(a, T, row_bytes, e, c2, f);
 #pragma unroll
           for (int q = 0; q < 8; ++q) f[q] *= gmul;
-          px_row_apply8<FAM>(T.kind, hp, f, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
-                             (size_t)r, T.D4, c2);
+          px_row_apply8<FAM>(T.kind, hp, f, reinterpret_cast<MT*>(T.table), T.slot0, T.slot1, T.slot2, T.shadow,
+                             (size_t)r, T.D4, c2, key);
         }
         continue;
       }
       for (int cidx = lane; cidx < T.D4; cidx += 16) {
         float4 gv = ld_merged4<WireT>(a, T, row_bytes, e, cidx);
         gv.x *= gmul; gv.y *= gmul; gv.z *= gmul; gv.w *= gmul;
-        px_row_apply4<FAM>(T.kind, hp, gv, T.table, T.slot0, T.slot1, T.slot2, T.shadow,
-                           (size_t)r, T.D4, cidx);
+        px_row_apply4<FAM>(T.kind, hp, gv, reinterpret_cast<MT*>(T.table), T.slot0, T.slot1, T.slot2, T.shadow,
+                           (size_t)r, T.D4, cidx, key);
       }
     }
   };
@@ -971,6 +1056,16 @@ static const void* const kPushKernels[2][2][2] = {
       (const void*)px_sparse_push_kernel<float, float, true, 1>},
      {(const void*)px_sparse_push_kernel<__nv_bfloat16, float, true, 0>,
       (const void*)px_sparse_push_kernel<__nv_bfloat16, float, true, 1>}}};
+
+// The owner instantiations, [bf16 master][bf16 wire][optimizer family]
+#define PX_OWNER_FAMS(WireT, MT)                                                          \
+  {(const void*)px_sparse_owner_kernel<WireT, 0, MT>,                                     \
+   (const void*)px_sparse_owner_kernel<WireT, 1, MT>,                                     \
+   (const void*)px_sparse_owner_kernel<WireT, 2, MT>}
+static const void* const kOwnerKernels[2][2][3] = {
+    {PX_OWNER_FAMS(float, float), PX_OWNER_FAMS(__nv_bfloat16, float)},
+    {PX_OWNER_FAMS(float, __nv_bfloat16), PX_OWNER_FAMS(__nv_bfloat16, __nv_bfloat16)}};
+#undef PX_OWNER_FAMS
 
 // The most CTAs of 256 threads of `fn` the device keeps resident at once: the largest grid a
 // cooperative launch of `fn` may have.  Cached per kernel.
@@ -1038,7 +1133,8 @@ const char* px_sparse_abi() {
     SIZE(OwnerTable); FIELD(OwnerTable, ring); FIELD(OwnerTable, table); FIELD(OwnerTable, slot0);
     FIELD(OwnerTable, slot1); FIELD(OwnerTable, slot2); FIELD(OwnerTable, shadow);
     FIELD(OwnerTable, hp); FIELD(OwnerTable, D4); FIELD(OwnerTable, kind); FIELD(OwnerTable, avg);
-    FIELD(OwnerTable, D);
+    FIELD(OwnerTable, D); FIELD(OwnerTable, slot_part); FIELD(OwnerTable, seed);
+    FIELD(OwnerTable, w_bf16);
 #undef SIZE
 #undef FIELD
     return s;
@@ -1133,18 +1229,14 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
   a.nt = nt; a.ring_ids = ring_ids; a.hdr = (uint32_t*)hdr; a.hdrs = (uint32_t* const*)hdrs_dev;
   a.slotmap = slotmap; a.next = next; a.cap = cap; a.rank = rank; a.use_merge = use_merge;
   const int fam = PX_KIND_FAMILY(tabs[0].kind);
+  const int w_bf16 = tabs[0].w_bf16 != 0;
   for (int t = 0; t < nt; ++t) {
     if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
+    if ((tabs[t].w_bf16 != 0) != w_bf16) return -8;   // members share one master type
     a.t[t] = tabs[t];
   }
   SparseCtl* C = (SparseCtl*)ctl;
-  const void* fn;
-  if (wire_dtype == 0) fn = fam == 0 ? (const void*)px_sparse_owner_kernel<float, 0>
-                          : fam == 1 ? (const void*)px_sparse_owner_kernel<float, 1>
-                                     : (const void*)px_sparse_owner_kernel<float, 2>;
-  else fn = fam == 0 ? (const void*)px_sparse_owner_kernel<__nv_bfloat16, 0>
-          : fam == 1 ? (const void*)px_sparse_owner_kernel<__nv_bfloat16, 1>
-                     : (const void*)px_sparse_owner_kernel<__nv_bfloat16, 2>;
+  const void* fn = kOwnerKernels[w_bf16][wire_dtype != 0][fam];
   void* args[] = {&a, &G, &C};
   // Merge grids are also held to the residency of px_sparse_owner_kernel<float, 1> (3 CTAs per
   // SM on the H100): a tuning cap, under which the benchmark numbers were taken.

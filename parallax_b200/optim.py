@@ -68,11 +68,65 @@ def slot_width(kind, D):
     return 1 if kind in ROWWISE_KINDS else D
 
 
-def table_row_bytes(kind, D):
-    """Bytes one row of a sparse variable of width D takes on its owner: the fp32 master row
-    and the fp32 slots, every D-wide row padded to a multiple of 4 columns."""
+def table_row_bytes(kind, D, weight_dtype=torch.float32):
+    """Bytes one row of a sparse variable of width D takes on its owner: the master row and
+    the fp32 slots, every D-wide row padded to a multiple of 4 columns.  A bf16 master row
+    (``sess_config["sparse_weights"] = "bf16"``) is padded to a multiple of 8 columns."""
     Dp = (D + 3) // 4 * 4
-    return 4 * Dp + 4 * NUM_SLOTS[kind] * slot_width(kind, Dp)
+    w = 4 * Dp if weight_dtype == torch.float32 else 2 * ((Dp // 4 + 1) // 2 * 8)
+    return w + 4 * NUM_SLOTS[kind] * slot_width(kind, Dp)
+
+
+# ---------------------------------------------------------------------------
+# bf16 master rows: stochastic rounding (`ops/csrc/kernels/sparse.cu` holds the same hash and
+# rounding; the two agree bit for bit)
+# ---------------------------------------------------------------------------
+SPARSE_WEIGHTS = {"fp32": torch.float32, "bf16": torch.bfloat16}
+_M32 = 0xffffffff
+
+
+def sparse_weight_dtype(value):
+    """torch dtype of ``sess_config["sparse_weights"]``: "fp32" (default) or "bf16"."""
+    if value not in SPARSE_WEIGHTS:
+        raise ValueError("sess_config['sparse_weights'] must be 'fp32' or 'bf16', not %r"
+                         % (value,))
+    return SPARSE_WEIGHTS[value]
+
+
+def sr_seed(name):
+    """The stochastic-rounding seed of sparse variable `name` (a 32-bit constant)."""
+    import zlib
+    return zlib.crc32(name.encode("utf-8")) & _M32
+
+
+def _mul32(x, c):
+    """(x · c) mod 2^32 for x in [0, 2^32) (int64 tensors or ints) without int64 overflow."""
+    return ((x & 0xffff) * c + ((((x >> 16) * (c & 0xffff)) & 0xffff) << 16)) & _M32
+
+
+def sr_mix(x):
+    """32-bit integer hash (a 32-bit finaliser: xor-shift, multiply, twice)."""
+    x = x ^ (x >> 16)
+    x = _mul32(x, 0x7feb352d)
+    x = x ^ (x >> 15)
+    x = _mul32(x, 0x846ca68b)
+    return x ^ (x >> 16)
+
+
+def round_bf16_stochastic(x, seed, step, gids):
+    """bf16 [n, D] of fp32 rows `x` [n, D] of global ids `gids` [n], rounded stochastically at
+    global step `step`: element (i, j) takes the top 16 bits of ``bits(x) + r`` with
+    ``r = sr_mix(sr_mix(sr_mix(seed ^ step) ^ gid) ^ j) >> 16``, so it rounds away from zero
+    with probability equal to its fraction of a bf16 ulp.  Inf and NaN pass through."""
+    x = x.to(torch.float32).contiguous()
+    n, D = x.shape
+    u = x.view(torch.int32).to(torch.int64) & _M32
+    key = sr_mix(sr_mix(int(seed) ^ int(step)) ^ (gids.to(x.device, torch.int64) & _M32))
+    r = sr_mix(key[:, None] ^ torch.arange(D, dtype=torch.int64, device=x.device)[None, :]) >> 16
+    finite = (u & 0x7f800000) != 0x7f800000
+    special = (u >> 16) | torch.where((u & 0x7fffff) != 0, 0x40, 0)
+    b = torch.where(finite, (u + r) >> 16, special) & 0xffff
+    return ((b ^ 0x8000) - 0x8000).to(torch.int16).view(torch.bfloat16)
 
 
 def check_table_slots(name, kind, V, D, slots):
@@ -388,19 +442,23 @@ def apply_dense_(kind, w, g, slots, hp):
     return w
 
 
-def apply_sparse_rows_(kind, w, rows, g, slots, hp):
+def apply_sparse_rows_(kind, w, rows, g, slots, hp, seed=None, gids=None):
     """Row-sparse update: `rows` (int64, unique) index dim 0 of `w`/`slots`;
     `g` is [len(rows), D] — the *summed* gradient of each row.  `weight_decay` is a
     dense-variable setting: sparse rows are not decayed (TF's SparseApply* ops have no
-    L2 term either, and the fused `sparse_update4` kernel takes none)."""
+    L2 term either, and the fused `sparse_update4` kernel takes none).  A bf16 `w` is
+    widened, updated in fp32 and stored with `round_bf16_stochastic` (the table's `seed`,
+    hp[HP_STEP] and the rows' global ids `gids`)."""
     if rows.numel() == 0:
         return w
     if hp[HP_WD] != 0.0:
         hp = list(hp)
         hp[HP_WD] = 0.0
-    w_r = w.index_select(0, rows)
+    w_r = w.index_select(0, rows).to(torch.float32)
     s_r = tuple(s.index_select(0, rows) for s in slots)
     apply_dense_(kind, w_r, g, s_r, hp)
+    if w.dtype == torch.bfloat16:
+        w_r = round_bf16_stochastic(w_r, seed, int(hp[HP_STEP]), gids)
     w.index_copy_(0, rows, w_r)
     for s, sr in zip(slots, s_r):
         s.index_copy_(0, rows, sr)

@@ -235,6 +235,7 @@ class TrainEngine(object):
         self.step_times = []
         self._check_joint_clip(sync)
         self._check_rowwise(sync)
+        self._check_sparse_weights(sync)
         self._build()
         self._consistency_check()
         self._start_aux()
@@ -267,7 +268,8 @@ class TrainEngine(object):
                 info = self.analysis.variables[path + ".weight" if path else "weight"]
                 rows = (int(mod.weight.shape[0]) + info.partitions - 1) // info.partitions
                 items.append((path, info.partitions,
-                              rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]))))
+                              rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]),
+                                                            self.sparse_weight_dtype)))
             placed = assign_owners(items, comm.world) \
                 if bool(cfg.communication_config.ps_config.boundary_among_servers) else {}
             for path, mod in self.analysis.sparse_modules.items():
@@ -280,7 +282,7 @@ class TrainEngine(object):
                     g.sparse_optimizer, comm, self.route, g, cfg,
                     init={"seed": getattr(mod, "init_seed", 1234),
                           "scale": getattr(mod, "init_scale", 0.05)}, device=dev,
-                    owners=placed.get(path))
+                    owners=placed.get(path), weight_dtype=self.sparse_weight_dtype)
                 adapter = _HostTableAdapter(t)
                 self.tables[pname] = adapter
                 _set_submodule(self.model, path, ShardedEmbedding(adapter))
@@ -330,6 +332,25 @@ class TrainEngine(object):
                 raise ValueError(
                     "co-lookup group %s: its tables must all be clipped by the same "
                     "ClipByGlobalNorm(include_sparse=True) rule or all by none" % paths)
+
+    def _check_sparse_weights(self, sync):
+        """``sess_config["sparse_weights"]``: "fp32" (default) or "bf16" master rows for every
+        sparse variable.  Refuses at build, before anything is allocated, what bf16 masters
+        cannot do; sets `self.sparse_weight_dtype`."""
+        value = self.config.sess_option("sparse_weights", "fp32")
+        self.sparse_weight_dtype = _optim.sparse_weight_dtype(value)
+        if value != "bf16":
+            return
+        if not sync:
+            raise ValueError(
+                "sparse_weights='bf16' needs sync=True: the asynchronous push applies rows "
+                "into fp32 master tables on their owners")
+        if self.backend == "nvlink":
+            cdt = self.config.sess_option("compute_dtype")
+            if cdt not in ("bf16", "bfloat16", torch.bfloat16):
+                raise ValueError(
+                    "sparse_weights='bf16' on the NVLink fabric needs compute_dtype='bf16' "
+                    "(got %r): lookups read bf16 master rows into bf16 outputs only" % (cdt,))
 
     def _check_rowwise(self, sync):
         """Refuse at build, before anything is allocated, what a row-wise optimizer
@@ -689,7 +710,7 @@ class TrainEngine(object):
                 new = _HostTableAdapter(HostSparseTable(
                     name, weight, num_partitions, old.layout.strategy,
                     self.graph.sparse_optimizer, self.comm, self.route, self.graph,
-                    self.config, device=old.t.device))
+                    self.config, device=old.t.device, weight_dtype=old.t.weight_dtype))
                 new.load_full(weight, slots)
                 self.tables[name] = new
                 if holder is not None:
@@ -717,7 +738,7 @@ class TrainEngine(object):
                 continue
             state = [(t.full_weight(), t.full_slots()) for t in olds]
             nbytes = sum(((t.V + num_partitions - 1) // num_partitions) *
-                         _optim.table_row_bytes(t.kind, t.D) for t in olds)
+                         _optim.table_row_bytes(t.kind, t.D, t.weight_dtype) for t in olds)
             owners = assign_owners([("g", num_partitions, nbytes)], self.comm.world)["g"] \
                 if bool(ps_cfg.boundary_among_servers) else None
             cap = grp.cap

@@ -175,7 +175,8 @@ class HostSparseTable(object):
     """One sparse variable (embedding table) on the host fabric."""
 
     def __init__(self, name, weight, num_partitions, strategy, optimizer, comm,
-                 route, graph, config, init=None, device=None, owners=None):
+                 route, graph, config, init=None, device=None, owners=None,
+                 weight_dtype=torch.float32):
         self.name = name
         self.device = torch.device("cpu") if device is None else torch.device(device)
         self.comm = comm
@@ -192,8 +193,15 @@ class HostSparseTable(object):
         self.clip_rule = graph.joint_clip_index(name)
         self.merged = []
         L = self.layout
+        # bf16 master rows (sparse_weights="bf16"): every update is applied in fp32 on the
+        # widened rows and rounded stochastically (`optim.round_bf16_stochastic`), keyed by
+        # the rows' global ids
+        self.weight_dtype = weight_dtype
+        self.sr_seed = _optim.sr_seed(name)
         shard = torch.zeros(L.rows_local, self.D, dtype=torch.float32)
         g, l = L.global_ids_of_owner(comm.rank)
+        self._gid = torch.zeros(L.rows_local, dtype=torch.int64)
+        self._gid[l] = g
         if weight.device.type == "meta":
             gen = torch.Generator().manual_seed(init["seed"])
             full = torch.empty(self.V, self.D).uniform_(
@@ -201,7 +209,7 @@ class HostSparseTable(object):
             shard[l] = full[g]
         else:
             shard[l] = weight.detach().to(torch.float32).cpu()[g]
-        self.shard = shard.to(self.device)
+        self.shard = shard.to(self.device, weight_dtype)
         self.slots = _slots_like(self.shard, optimizer)
         self.nslots = len(self.slots)
         self.slot_dim = _optim.slot_width(optimizer.kind, self.D)
@@ -215,14 +223,14 @@ class HostSparseTable(object):
         """rows = table[ids] for arbitrary global ids (ids: 1-D int64)."""
         L, W, me = self.layout, self.comm.world, self.comm.rank
         if self.replicated or W == 1:
-            return self.shard[L.local_row_of(ids)]
+            return self.shard[L.local_row_of(ids)].float()
         # PS-style request/response all-to-all: ids travel to their owners, rows
         # travel back; O(n) traffic per rank instead of an all-gather of every id
         owners = L.owner_of(ids)
         order = torch.argsort(owners, stable=True)
         counts = torch.bincount(owners, minlength=W).tolist()
         req, req_counts = self.comm.all_to_all_varlen(ids[order], counts)
-        rows = self.shard[L.local_row_of(req)]
+        rows = self.shard[L.local_row_of(req)].float()
         resp, _ = self.comm.all_to_all_varlen(rows, req_counts)
         out = torch.empty(ids.numel(), self.D, dtype=torch.float32, device=self.device)
         out[order] = resp
@@ -303,7 +311,8 @@ class HostSparseTable(object):
             if scale != 1.0:
                 g = g * scale
             _optim.apply_sparse_rows_(self.optimizer.kind, self.shard, rows, g,
-                                      self.slots, hp)
+                                      self.slots, hp, self.sr_seed,
+                                      self._gid[rows.cpu()])
         self.merged = []
 
     # -- checkpoint / inspection -------------------------------------------------
@@ -312,9 +321,9 @@ class HostSparseTable(object):
         if self.replicated or W == 1:
             g, l = L.global_ids_of_owner(0 if self.replicated else self.comm.rank)
             out = torch.zeros(self.V, local.shape[1])
-            out[g] = local.cpu()[l]
+            out[g] = local.cpu()[l].float()
             return out
-        shards = self.comm.all_gather_tensors(local)
+        shards = self.comm.all_gather_tensors(local.float())
         out = torch.zeros(self.V, local.shape[1])
         for o in range(W):
             g, l = L.global_ids_of_owner(o)
@@ -333,7 +342,7 @@ class HostSparseTable(object):
         g, l = self.layout.global_ids_of_owner(
             0 if self.replicated else self.comm.rank)
         l = l.to(self.device)
-        self.shard[l] = weight.to(torch.float32)[g].to(self.device)
+        self.shard[l] = weight.to(torch.float32)[g].to(self.device, self.shard.dtype)
         if slots is not None:
             for s, full in zip(self.slots, slots):
                 s[l] = full.to(torch.float32)[g].to(self.device)

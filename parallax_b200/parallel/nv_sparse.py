@@ -2,7 +2,8 @@
 
 `NVSparseTable` is the storage of one row-partitioned variable (fp32 master rows,
 optimizer slots and — for bf16 models — a bf16 *shadow* copy that lookups read, all
-in symmetric memory).  `NVSparseGroup` is the machinery of one *group* of tables
+in symmetric memory; with ``sess_config["sparse_weights"] = "bf16"`` the master rows
+themselves are bf16, in the shadow's layout, and there is no second copy).  `NVSparseGroup` is the machinery of one *group* of tables
 that are looked up with the same ids (LM1B: ``softmax_w`` + ``softmax_b``; every
 other table is a group of one): per step ONE remote-gather lookup kernel per
 lookup call, ONE push kernel (SMEM local aggregation + P2P stores + flag) and ONE
@@ -129,11 +130,30 @@ class NVSparseTable(object):
         self.out_dtype = out_dtype or torch.float32
         self.anchor_device = self.device
         self.capacity_hint = (opts.get("sparse_capacity") or {}).get(name)
+        self.weight_dtype = _optim.sparse_weight_dtype(opts.get("sparse_weights", "fp32"))
+        if self.weight_dtype == torch.bfloat16 and self.out_dtype != torch.bfloat16:
+            raise ValueError(
+                "sparse variable %r: sparse_weights='bf16' needs bf16 lookups "
+                "(compute_dtype='bf16'): the lookup kernel copies bf16 rows into bf16 outputs"
+                % name)
+        self.sr_seed = _optim.sr_seed(name)
         L = self.layout
         rows = L.rows_local
         heap = self.heap
-        self.tab_buf = heap.alloc(rows * self.Dp * 4, "table:" + name)
-        self.table = self.tab_buf.tensor(torch.float32, rows * self.Dp).view(rows, self.Dp)
+        self.Dps = (self.D4 + 1) // 2 * 8          # shadow row length (16-byte vectors)
+        if self.weight_dtype == torch.bfloat16:
+            # bf16 master rows in the shadow's layout: lookups and the full-softmax evaluation
+            # read them through the shadow descriptors; the owner kernel rounds every update
+            # stochastically.  No fp32 copy exists.
+            self.tab_buf = heap.alloc(rows * self.Dps * 2, "table:" + name)
+            self.table = self.tab_buf.tensor(torch.bfloat16, rows * self.Dps) \
+                .view(rows, self.Dps)
+            self.table.zero_()
+            self.shadow = None
+            self._init_weights(weight, init)
+        else:
+            self.tab_buf = heap.alloc(rows * self.Dp * 4, "table:" + name)
+            self.table = self.tab_buf.tensor(torch.float32, rows * self.Dp).view(rows, self.Dp)
         # a row-wise rule keeps one fp32 per row: a dense [rows_local] array (the kernels
         # address it with a 4-byte pitch); every other rule keeps padded rows like the table
         self.slot_dim = _optim.slot_width(self.kind, self.D)
@@ -146,17 +166,21 @@ class NVSparseTable(object):
             self.slot_bufs.append(sb)
             self.slots.append(t)
         # bf16 shadow rows for bf16 models: lookups move half the bytes over NVLink / HBM;
-        # the owner kernel refreshes the shadow row together with the fp32 master row
-        self.Dps = (self.D4 + 1) // 2 * 8          # shadow row length (16-byte vectors)
+        # the owner kernel refreshes the shadow row together with the fp32 master row.  A
+        # bf16 master is its own shadow (`sparse_shadow` has no effect).
         want = opts.get("sparse_shadow", "auto")
-        self.use_shadow = (self.out_dtype == torch.bfloat16 and bool(want) and
-                           (want is True or rows * self.Dps * 2 <= (16 << 30)))
-        self.shadow_buf = self.shadow = None
-        if self.use_shadow:
-            self.shadow_buf = heap.alloc(rows * self.Dps * 2, "shadow:" + name)
-            self.shadow = self.shadow_buf.tensor(torch.bfloat16, rows * self.Dps) \
-                .view(rows, self.Dps)
-        self._init_weights(weight, init)
+        if self.weight_dtype == torch.bfloat16:
+            self.use_shadow = True
+            self.shadow_buf, self.shadow = self.tab_buf, self.table
+        else:
+            self.shadow_buf = self.shadow = None
+            self.use_shadow = (self.out_dtype == torch.bfloat16 and bool(want) and
+                               (want is True or rows * self.Dps * 2 <= (16 << 30)))
+            if self.use_shadow:
+                self.shadow_buf = heap.alloc(rows * self.Dps * 2, "shadow:" + name)
+                self.shadow = self.shadow_buf.tensor(torch.bfloat16, rows * self.Dps) \
+                    .view(rows, self.Dps)
+            self._init_weights(weight, init)
         self._ptrs = {}
         self.ring_buf = None
         self.staging = None
@@ -173,17 +197,26 @@ class NVSparseTable(object):
             gen = torch.Generator(device=self.device)
             gen.manual_seed(int(init["seed"]) * 1000003 + (0 if self.replicated
                                                            else self.rank))
+            if self.weight_dtype == torch.bfloat16:
+                # the fp32 initialisation, rounded to nearest even (runs before the slots
+                # are allocated, and returns its fp32 scratch to the device)
+                w = torch.empty(self.table.shape[0], self.Dp, device=self.device)
+                w[:, :self.D].uniform_(-init["scale"], init["scale"], generator=gen)
+                self.table[:, :self.D] = w[:, :self.D]
+                del w
+                torch.cuda.empty_cache()
+                return
             self.table[:, :self.D].uniform_(-init["scale"], init["scale"], generator=gen)
             if self.Dp != self.D:
                 self.table[:, self.D:].zero_()
         else:
             w = weight.detach().to(torch.float32)
             for g, l in L.owner_chunks(0 if self.replicated else self.rank):
-                self.table[l.to(self.device), :self.D] = w[g].to(self.device)
+                self.table[l.to(self.device), :self.D] = w[g].to(self.device, self.table.dtype)
         self.refresh_shadow()
 
     def refresh_shadow(self):
-        if self.shadow is not None:
+        if self.shadow is not None and self.shadow is not self.table:
             self.shadow.zero_()
             self.shadow[:, :self.Dp].copy_(self.table)
 
@@ -259,7 +292,7 @@ class NVSparseTable(object):
             gs.append(g)
             rows.append(src[l.to(self.device), :d].cpu())
         if not gs:
-            return torch.zeros(0, dtype=torch.int64), torch.zeros(0, d)
+            return torch.zeros(0, dtype=torch.int64), torch.zeros(0, d, dtype=src.dtype)
         return torch.cat(gs), torch.cat(rows)
 
     def _gather_full(self, local, d):
@@ -268,12 +301,12 @@ class NVSparseTable(object):
         out = torch.zeros(self.V, d)
         if self.replicated or W == 1:
             g, l = L.global_ids_of_owner(0 if self.replicated else self.rank)
-            out[g] = local.cpu()[l]
+            out[g] = local.cpu()[l].float()
             return out
         shards = self.comm.all_gather_tensors(local)
         for o in range(W):
             g, l = L.global_ids_of_owner(o)
-            out[g] = shards[o].cpu()[l]
+            out[g] = shards[o].cpu()[l].float()
         return out
 
     def full_weight(self):
@@ -289,7 +322,7 @@ class NVSparseTable(object):
             _optim.check_table_slots(self.name, self.kind, self.V, self.D, slots)
         for g, l in self.layout.owner_chunks(0 if self.replicated else self.rank):
             l = l.to(self.device)
-            self.table[l, :self.D] = weight.float()[g].to(self.device)
+            self.table[l, :self.D] = weight.float()[g].to(self.device, self.table.dtype)
             if slots is not None:
                 for s, full in zip(self.slots, slots):
                     s[l, :self.slot_dim] = full.float()[g].to(self.device)
@@ -310,7 +343,7 @@ class NVSparseTable(object):
         if own.any():
             l = L.local_row_of(ids[own]).to(self.device)
             dst = self.table if what == "weight" else self.slots[int(what)]
-            dst[l, :d] = rows[own].float().to(self.device)
+            dst[l, :d] = rows[own].float().to(self.device, dst.dtype)
 
     def release(self):
         """Free this table's symmetric segments (collective)."""
@@ -319,7 +352,8 @@ class NVSparseTable(object):
             self.comm.barrier()
         if self.group is not None:
             self.group.release_shared()
-        for b in [self.tab_buf, self.shadow_buf, self.ring_buf] + list(self.slot_bufs):
+        shadow = self.shadow_buf if self.shadow_buf is not self.tab_buf else None
+        for b in [self.tab_buf, shadow, self.ring_buf] + list(self.slot_bufs):
             if b is not None:
                 self.heap.free(b)
         self.table = self.shadow = None
@@ -374,6 +408,15 @@ class NVSparseGroup(object):
         g.part_owner = self._owners_dev.data_ptr()
         g.part_slot = self._slots_dev.data_ptr()
         self.geom = g
+        # the partition held in each of my slots (-1: none): a bf16 master's owner kernel keys
+        # its stochastic rounding by global row ids
+        slot_part = [-1] * max(lay.parts_per_owner, 1)
+        for p_ in range(lay.P):
+            if not lay.replicated and lay.owners[p_] == self.rank:
+                slot_part[lay.slots[p_]] = p_
+        self._slot_part_dev = torch.tensor(slot_part, dtype=torch.int32, device=self.device)
+        if len({t.weight_dtype for t in tables}) != 1:
+            raise ValueError("co-lookup group %s mixes fp32 and bf16 master rows" % self.name)
         self.ctl = torch.zeros(abi["ctl_bytes"] // 4, dtype=torch.int32, device=self.device)
         self.hdr_buf = self.heap.alloc(abi["hdr_words"] * 4, "hdr:" + self.name)
         self.ids_buf = None
@@ -543,10 +586,13 @@ class NVSparseGroup(object):
         wait = self._wait
         stream = _sp(torch.cuda.current_stream(self.device))
         w_t = torch.empty((n, tw.Dps), dtype=torch.bfloat16, device=self.device)
-        b_t = torch.empty((n, tb.Dp), dtype=torch.float32, device=self.device)
-        # target bias from the fp32 master like every bias row the eval kernel reads
+        # target bias from the master rows like every bias row the eval kernel reads: fp32, or
+        # bf16 rows of the shadow's layout with bf16 masters (widened where they are added)
+        b_bf16 = tb.weight_dtype == torch.bfloat16
+        b_src, b_pitch = ("shadow", tb.Dps) if b_bf16 else ("table", tb.Dp)
+        b_t = torch.empty((n, b_pitch), dtype=tb.weight_dtype, device=self.device)
         descs = (ops.LookupTable * 2)(_lookup_table(tw, "shadow", w_t),
-                                      _lookup_table(tb, "table", b_t))
+                                      _lookup_table(tb, b_src, b_t))
         _count()
         ops.check(L.px_sparse_lookup(
             _vp(ids.data_ptr()), 1, n, descs, 2, _vp(0), ctypes.byref(self.geom),
@@ -557,7 +603,7 @@ class NVSparseGroup(object):
         _count(2)
         ops.check(L.px_full_softmax_nll(
             _vp(x.data_ptr()), n, K, _vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps,
-            _vp(tb.dev_ptrs("table").data_ptr()), tb.Dp, _vp(cnt.data_ptr()),
+            _vp(tb.dev_ptrs(b_src).data_ptr()), b_pitch, int(b_bf16), _vp(cnt.data_ptr()),
             int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
             _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), wait, _vp(ws.data_ptr()),
             consts.NUM_SMS, _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
@@ -800,8 +846,10 @@ class NVSparseGroup(object):
             d.slot0 = t.slots[0].data_ptr() if t.nslots > 0 else 0
             d.slot1 = t.slots[1].data_ptr() if t.nslots > 1 else 0
             d.slot2 = t.slots[2].data_ptr() if t.nslots > 2 else 0
-            d.shadow = t.shadow.data_ptr() if t.use_shadow else 0
+            bf16 = t.weight_dtype == torch.bfloat16
+            d.shadow = t.shadow.data_ptr() if t.use_shadow and not bf16 else 0
             d.hp, d.D4, d.D, d.kind = hp_ptr, t.D4, t.D, _optim.KIND_ID[t.kind]
+            d.w_bf16, d.seed, d.slot_part = int(bf16), t.sr_seed, self._slot_part_dev.data_ptr()
             avg = (1.0 / self.world) if t.average else 1.0
             d.avg = avg if sender_scaled else avg * t.scale
         return descs

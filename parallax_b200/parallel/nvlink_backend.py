@@ -633,7 +633,8 @@ def build_nvlink(engine):
     def item_bytes(path, mod):
         info = engine.analysis.variables[pname_of(path)]
         rows = (int(mod.weight.shape[0]) + info.partitions - 1) // info.partitions
-        return info.partitions, rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]))
+        return info.partitions, rows * _optim.table_row_bytes(kind, int(mod.weight.shape[1]),
+                                                              engine.sparse_weight_dtype)
     mods = dict(sparse_items)
     place_items, seen = [], set()
     for path, mod in sparse_items:
