@@ -31,6 +31,12 @@ def add_flags(ap):
     ap.add_argument("--export_graph_path", default=None)
     ap.add_argument("--compute_dtype", default=None, help="bf16 | float32")
     ap.add_argument("--cuda_graph", action="store_true")
+    # K forward/backward passes per optimizer step: every feed of a step is split into K
+    # equal micro-batches along dim 0, so the per-worker batch a driver feeds is K·b.  Give
+    # graph builders that take a batch size the per-worker K·b: `lm1b_graph(batch_size=...)`
+    # scales the embedding gradients by it (ScaleGradients), and its 1/K weighting expects it.
+    ap.add_argument("--micro_batches", type=int, default=1,
+                    help="forward/backward passes per optimizer step (gradient accumulation)")
     return ap
 
 
@@ -53,6 +59,8 @@ def build_config(FLAGS):
         sc["compute_dtype"] = FLAGS.compute_dtype
     if FLAGS.cuda_graph:
         sc["cuda_graph"] = True
+    if getattr(FLAGS, "micro_batches", 1) != 1:
+        sc["micro_batches"] = FLAGS.micro_batches
     cfg = parallax.Config()
     cfg.run_option = FLAGS.run_option
     cfg.average_sparse = FLAGS.average_sparse

@@ -74,7 +74,7 @@ _SIGS = {
                              c_int, c_int, c_void_p]),
     "px_dense_step": (c_int, [PP, PP, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
-                              c_float, c_float, c_int, c_int, c_int, c_void_p,
+                              c_float, c_float, c_int, c_int, c_int, c_int, c_void_p,
                               c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                               c_void_p]),
     "px_clip_scale": (c_int, [c_void_p, c_float, c_void_p, c_void_p, c_void_p,

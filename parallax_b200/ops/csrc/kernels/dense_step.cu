@@ -18,6 +18,13 @@
 // MODE 1 REDUCE_ONLY  : barrier, reduce → fp32 scratch + Σg² (for global-norm
 //                       clipping the norm must be known before any update)
 // MODE 2 UPDATE_PUSH  : scratch·clip → update, push params, barrier
+// MODE 3 ACCUMULATE   : barrier, reduce → fp32 scratch (= or +=), barrier; no update.  One
+//                       micro-batch of a step that accumulates several: the end barrier is
+//                       there because peers pull from this rank's gradient bucket, which the
+//                       next micro-batch's backward overwrites.
+// "Accumulator in" (PX_DS_ACC_IN, modes 0, 1 and 3): the fp32 scratch holds the scaled sum of
+// the step's earlier micro-batches and is added to this reduction before anything else, so
+// the last micro-batch of a step runs mode 0 or 1 with the flag and mode 2 is unchanged.
 // World 1 degenerates to a fused multi-tensor optimizer (also used as the
 // local update after a plain all-reduce in "replicated" AR mode).
 #include "common.cuh"
@@ -32,16 +39,18 @@ struct DenseStepArgs {
   float* slot1;      // [slice] or null
   float* slot2;      // [slice] or null (centered RMSProp)
   float* ema;        // [slice] or null
-  float* red;        // [slice] fp32 scratch (modes 1/2) or null
+  float* red;        // [slice] fp32 scratch (modes 1/2/3, accumulator in) or null
   const float* hp;   // device hyper-parameters (8 floats)
   const float* clip; // device scalar multiplier or null
   float* sumsq;      // device scalar accumulator or null
   size_t n;          // bucket elements, multiple of W * VN
   float avg;         // 1/num_workers (or 1)
   float ema_decay;
-  int rank, ch_start, ch_end, kind, mode;
+  int rank, ch_start, ch_end, kind, mode;   // mode | PX_DS_ACC_IN in the ACC kernels
   int use_mc;        // 1: grads.p[0] / params.p[0] are NVSwitch multicast addresses
 };
+
+constexpr int PX_DS_ACC_IN = 4;
 
 // NVLS: the switch reduces (fp32 accumulate) / broadcasts; see collectives.cu
 template <typename T>
@@ -99,11 +108,16 @@ __device__ __forceinline__ void px_rank_wait(uint32_t* const* pads, int slot, in
   __syncthreads();
 }
 
-template <typename T, int W, int FAM>
-__global__ void __launch_bounds__(512, (W == 1 && FAM == 0) ? 2 : 1)
+// ACC: the instantiation that runs mode 3 and the accumulator-in flag.  A step of one
+// micro-batch launches only ACC = false, whose code is that of a kernel without either.  The
+// ACC kernels keep one CTA per SM: the accumulator's 8 extra loads in flight spill at the
+// 64 registers of two.
+template <typename T, int W, int FAM, bool ACC>
+__global__ void __launch_bounds__(512, (W == 1 && FAM == 0 && !ACC) ? 2 : 1)
 px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr) {
   constexpr int VN = Vec16<T>::N;
-  const int mode = a.mode, kind = a.kind;
+  const int mode = ACC ? (a.mode & 3) : a.mode, kind = a.kind;
+  const bool acc_in = ACC && (a.mode & PX_DS_ACC_IN);
   const int slot_s = a.ch_start * PX_MAX_BLOCKS, slot_e = a.ch_end * PX_MAX_BLOCKS;
   // profiling aid: %globaltimer stamps of the last launch in the (otherwise unused) epoch slots
   // of the last channel: [0] CTA 0 start, [1] CTA 0 past the start wait, [2] CTA 0 loop done,
@@ -147,8 +161,10 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
       for (int p = 0; p < W; ++p)
         in[p] = ld_v4_stream(reinterpret_cast<const T*>(a.grads.p[p]) + base + e);
     }
+    float r[ACC ? VN : 1];
+    if (acc_in) ld_f32<VN>(a.red + e, r);
     float w[VN], s0[VN], s1[VN], s2[FAM == 1 ? VN : 1], m[VN];
-    if (mode != 1) {
+    if (mode != 1 && !(ACC && mode == 3)) {
       ld_f32<VN>(a.master + e, w);
       if (a.slot0) ld_f32<VN>(a.slot0 + e, s0);
       if (a.slot1) ld_f32<VN>(a.slot1 + e, s1);
@@ -173,6 +189,14 @@ px_dense_step_kernel(DenseStepArgs a, uint32_t* const* pads, uint32_t* epoch_ctr
     }
 #pragma unroll
     for (int i = 0; i < VN; ++i) g[i] *= gmul;
+    if (acc_in) {
+#pragma unroll
+      for (int i = 0; i < VN; ++i) g[i] += r[ACC ? i : 0];
+    }
+    if (ACC && mode == 3) {
+      st_f32<VN>(a.red + e, g);
+      continue;
+    }
     if (mode == 1) {
 #pragma unroll
       for (int i = 0; i < VN; ++i) ss += g[i] * g[i];
@@ -316,12 +340,16 @@ extern "C" {
 int px_dense_step(const void* const* grads, const void* const* params, float* master,
                   float* slot0, float* slot1, float* slot2, float* ema, float* red, const float* hp,
                   const float* clip, float* sumsq, size_t n, float avg, float ema_decay,
-                  int kind, int mode, int dtype, void* pads_dev, void* epoch_ctr, int ch_start,
-                  int ch_end, int rank, int world, int max_blocks, int use_mc,
+                  int kind, int mode, int acc_in, int dtype, void* pads_dev, void* epoch_ctr,
+                  int ch_start, int ch_end, int rank, int world, int max_blocks, int use_mc,
                   cudaStream_t stream) {
   if (world < 1 || world > 8) return -3;
   const int vn = dtype == 0 ? 4 : 8;
   if (n % ((size_t)world * vn) != 0) return -1;
+  // mode 3 and the accumulator need the fp32 scratch; the clip multiplier belongs to mode 2
+  const bool acc = mode == 3 || acc_in;
+  if (mode < 0 || mode > 3 || (acc && (red == nullptr || clip != nullptr || mode == 2)))
+    return -2;
   DenseStepArgs a;
   a.use_mc = use_mc;
   if (use_mc) {            // entry 0 = multicast address; no peer pointers needed
@@ -334,24 +362,31 @@ int px_dense_step(const void* const* grads, const void* const* params, float* ma
   }
   a.master = master; a.slot0 = slot0; a.slot1 = slot1; a.slot2 = slot2; a.ema = ema; a.red = red;
   a.hp = hp; a.clip = clip; a.sumsq = sumsq; a.n = n; a.avg = avg; a.ema_decay = ema_decay;
-  a.rank = rank; a.ch_start = ch_start; a.ch_end = ch_end; a.kind = kind; a.mode = mode;
+  a.rank = rank; a.ch_start = ch_start; a.ch_end = ch_end; a.kind = kind;
+  a.mode = mode | (acc_in ? PX_DS_ACC_IN : 0);
   const int threads = 512;
   // rank-level barriers: the grid is sized for HBM bandwidth, not by barrier slots
   size_t b = (n / world / vn + threads - 1) / threads;
   const size_t cap = world == 1 ? PX_NUM_SMS * 4 : (size_t)(max_blocks > 0 ? max_blocks : PX_NUM_SMS);
   int blocks = (int)(b < 1 ? 1 : (b > cap ? cap : b));
-#define LAUNCH(T, W)                                                                       \
+#define LAUNCH_FAM(T, W, FAM)                                                              \
   do {                                                                                     \
-    if (PX_KIND_FAMILY(kind) == 0)                                                         \
-      px_dense_step_kernel<T, W, 0><<<blocks, threads, 0, stream>>>(                       \
+    if (acc)                                                                               \
+      px_dense_step_kernel<T, W, FAM, true><<<blocks, threads, 0, stream>>>(               \
           a, (uint32_t* const*)pads_dev, (uint32_t*)epoch_ctr);                            \
     else                                                                                   \
-      px_dense_step_kernel<T, W, 1><<<blocks, threads, 0, stream>>>(                       \
+      px_dense_step_kernel<T, W, FAM, false><<<blocks, threads, 0, stream>>>(              \
           a, (uint32_t* const*)pads_dev, (uint32_t*)epoch_ctr);                            \
+  } while (0)
+#define LAUNCH(T, W)                                                                       \
+  do {                                                                                     \
+    if (PX_KIND_FAMILY(kind) == 0) LAUNCH_FAM(T, W, 0);                                    \
+    else LAUNCH_FAM(T, W, 1);                                                              \
   } while (0)
   if (dtype == 0) { PX_DISPATCH_WORLD(world, LAUNCH, float); }
   else { PX_DISPATCH_WORLD(world, LAUNCH, __nv_bfloat16); }
 #undef LAUNCH
+#undef LAUNCH_FAM
   return (int)cudaGetLastError();
 }
 

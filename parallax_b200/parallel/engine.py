@@ -236,6 +236,7 @@ class TrainEngine(object):
         self._check_joint_clip(sync)
         self._check_rowwise(sync)
         self._check_sparse_weights(sync)
+        self._check_micro_batches(sync)
         self._build()
         self._consistency_check()
         self._start_aux()
@@ -292,7 +293,8 @@ class TrainEngine(object):
                            not getattr(p, "_parallax_skip", False)]
             if g.trainable():
                 self.dense = HostDenseGroup(dense_named, g.optimizer, comm,
-                                            self.route, g)
+                                            self.route, g,
+                                            micro_batches=self.micro_batches)
                 self._link_joint_tables()
         elif self.backend == "nvlink":
             from .nvlink_backend import build_nvlink
@@ -351,6 +353,70 @@ class TrainEngine(object):
                 raise ValueError(
                     "sparse_weights='bf16' on the NVLink fabric needs compute_dtype='bf16' "
                     "(got %r): lookups read bf16 master rows into bf16 outputs only" % (cdt,))
+
+    def _check_micro_batches(self, sync):
+        """``sess_config["micro_batches"]``: forward/backward passes per optimizer step
+        (default 1).  Refuses at build, before anything is allocated, what cannot
+        accumulate; sets `self.micro_batches`."""
+        k = self.config.sess_option("micro_batches", 1)
+        if isinstance(k, bool) or not isinstance(k, int) or k < 1:
+            raise ValueError("sess_config['micro_batches'] must be a positive int, got %r "
+                             "(1 runs one forward/backward pass per step)" % (k,))
+        self.micro_batches = k
+        if k == 1:
+            return
+        if not sync:
+            raise ValueError(
+                "micro_batches=%d needs sync=True: an asynchronous PS applies every "
+                "gradient as it arrives and has no step to accumulate into; use "
+                "micro_batches=1" % k)
+        if self.backend == "nvlink":
+            if self.config.sess_option("dense_update", "sharded") == "replicated" or \
+                    self.config.communication_config.ps_config.protocol == "nccl":
+                raise ValueError(
+                    "micro_batches=%d is not implemented on the NVLink fabric with "
+                    "dense_update='replicated' or PSConfig(protocol='nccl'): those reduce in "
+                    "place with an all-reduce per step.  Use the default sharded update, or "
+                    "sess_config={'fabric': 'library'} to accumulate over library "
+                    "collectives" % k)
+
+    def _split_feeds(self, feeds):
+        """The `micro_batches` parts of a step's feeds: every tensor feed with a dim 0 as
+        K equal views along it, everything else unchanged in every part."""
+        K = self.micro_batches
+        parts = [dict() for _ in range(K)]
+        for name, v in feeds.items():
+            if torch.is_tensor(v) and v.dim() > 0:
+                if v.shape[0] % K:
+                    raise ValueError(
+                        "feed %r: dim 0 (%d) is not divisible by micro_batches=%d"
+                        % (name, v.shape[0], K))
+                n = v.shape[0] // K
+                for k in range(K):
+                    parts[k][name] = v[k * n:(k + 1) * n]
+            else:
+                for k in range(K):
+                    parts[k][name] = v
+        return parts
+
+    @staticmethod
+    def _combine_outputs(outs):
+        """One step's outputs from its micro-batches': floating-point 0-dim tensors (the loss)
+        averaged, integer 0-dim tensors (counts, e.g. NMT's `word_count`) summed, other tensors
+        with a dim 0 concatenated along it, anything else (0-dim booleans included) from the
+        last micro-batch."""
+        res = {}
+        for k, v in outs[-1].items():
+            vals = [o[k] for o in outs]
+            if not torch.is_tensor(v) or v.dtype == torch.bool and v.dim() == 0:
+                res[k] = v
+            elif v.dim() == 0 and (v.is_floating_point() or v.is_complex()):
+                res[k] = torch.stack(vals).mean()
+            elif v.dim() == 0:
+                res[k] = torch.stack(vals).sum().to(v.dtype)
+            else:
+                res[k] = torch.cat(vals)
+        return res
 
     def _check_rowwise(self, sync):
         """Refuse at build, before anything is allocated, what a row-wise optimizer
@@ -456,12 +522,11 @@ class TrainEngine(object):
             nvops.stamp(st.data_ptr() + 0)
             if self.dense is not None:
                 self.dense.stamp_before = st.data_ptr() + 40
-        out = self.forward(feeds)
-        loss = out[self.graph.loss]
-        if self.graph.loss_scale != 1.0:
-            (loss * self.graph.loss_scale).backward()
+        if self.micro_batches == 1:
+            out = self.forward(feeds)
+            self._backward(out)
         else:
-            loss.backward()
+            out = self._accumulate(feeds)
         if ev is not None:
             ev["bwd"].record()
         if st is not None:
@@ -490,6 +555,36 @@ class TrainEngine(object):
         return {k: (v.detach() if torch.is_tensor(v) else v)
                 for k, v in out.items()}
 
+    def _backward(self, out):
+        loss = out[self.graph.loss]
+        if self.graph.loss_scale != 1.0:
+            (loss * self.graph.loss_scale).backward()
+        else:
+            loss.backward()
+
+    def _accumulate(self, feeds):
+        """Forward and backward of every micro-batch of the step.  The fabric reduces each
+        micro-batch's gradients into the owners' fp32 accumulators; only the last one's
+        are followed by the optimizer (`finish_step`)."""
+        K, outs = self.micro_batches, []
+        groups = [g for g in [self.dense] + list(getattr(self, "sparse_groups", ()))
+                  if hasattr(g, "micro_batch")]
+        for k, part in enumerate(self._split_feeds(feeds)):
+            for grp in groups:
+                grp.micro_batch(k, K)
+            out = self.forward(part)
+            if k > 0 and self.backend == "nvlink":
+                # the gradient buckets are rewritten from here on: the previous micro-batch's
+                # reductions, which read them (on this rank and, through the kernel's end
+                # barrier, on every peer), must be complete.  The forward pass overlaps them.
+                torch.cuda.current_stream(self.comm.device).wait_stream(
+                    self.fabric.comm_stream)
+            self._backward(out)
+            if k < K - 1 and self.dense is not None:
+                self.dense.end_micro_batch()
+            outs.append(out)
+        return self._combine_outputs(outs)
+
     def train_step(self, feeds):
         """One synchronous (or async-PS) training step.
 
@@ -501,6 +596,8 @@ class TrainEngine(object):
         need (barrier epochs, step counters, hyper-parameters) lives in device
         memory, so a replay is exactly a re-execution."""
         t0 = time.perf_counter()
+        if self.micro_batches > 1:
+            self._split_feeds(feeds)        # a feed that cannot be split fails before the step
         step = self.global_step + 1
         tl = self.timeline.enabled()
         tuning = self.autotuner is not None and not self.autotuner.done

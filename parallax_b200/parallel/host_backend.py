@@ -34,7 +34,7 @@ class HostDenseGroup(object):
     """All dense variables of the graph on the host fabric."""
 
     def __init__(self, named_params, optimizer, comm, route, graph,
-                 options=None):
+                 options=None, micro_batches=1):
         self.comm = comm
         self.route = route
         self.optimizer = optimizer
@@ -55,6 +55,10 @@ class HostDenseGroup(object):
         # sparse tables clipped jointly with dense variables (`HostSparseTable.clip_rule`):
         # aggregated before this group's step, applied by `_clip` with the rule's scale
         self.joint_tables = []
+        # micro_batches > 1: every micro-batch's gradient is widened and summed in fp32
+        # (`end_micro_batch`); the step applies the sum × 1/K
+        self.micro_batches = micro_batches
+        self.acc = None
         # make every replica start from rank 0's values
         # (reference `mpi/runner.py:134-139` broadcast of global variables)
         for m, p in zip(self.master, self.params):
@@ -66,14 +70,31 @@ class HostDenseGroup(object):
         for p in self.params:
             p.grad = None
 
+    def end_micro_batch(self):
+        """Add this micro-batch's gradients, widened to fp32, into the step's
+        accumulators and clear them."""
+        if self.acc is None:
+            self.acc = [torch.zeros_like(p, dtype=torch.float32) for p in self.params]
+        for a, p in zip(self.acc, self.params):
+            if p.grad is not None:
+                a.add_(p.grad.detach().to(torch.float32))
+        self.zero_grad()
+
     def finish_step(self, step):
         W = self.comm.world
+        acc = None
+        if self.micro_batches > 1:
+            self.end_micro_batch()
+            acc, self.acc = self.acc, None
         grads = []
-        for p, s in zip(self.params, self.scales):
-            g = p.grad
-            if g is None:
-                g = torch.zeros_like(p)
-            g = g.detach().to(torch.float32)
+        for i, (p, s) in enumerate(zip(self.params, self.scales)):
+            if acc is not None:
+                g = acc[i] * (1.0 / self.micro_batches)
+            else:
+                g = p.grad
+                if g is None:
+                    g = torch.zeros_like(p)
+                g = g.detach().to(torch.float32)
             if s != 1.0:
                 g = g * s
             grads.append(g)
@@ -187,6 +208,8 @@ class HostSparseTable(object):
         self.layout = TableLayout(self.V, num_partitions, comm.world, strategy,
                                   replicated=self.replicated, owners=owners)
         self.average = bool(config.average_sparse)
+        # the rows of every micro-batch of a step are pending together and weighted 1/K
+        self.micro_batches = int(config.sess_option("micro_batches", 1))
         self.local_aggregation = bool(
             config.communication_config.ps_config.local_aggregation)
         self.scale = graph.scale_for(name)
@@ -298,6 +321,8 @@ class HostSparseTable(object):
             g.index_add_(0, inv, seg_rows)
             if self.average and self.route.sync:
                 g.div_(W)
+            if self.micro_batches > 1:
+                g.mul_(1.0 / self.micro_batches)
             self.merged.append((L.local_row_of(u), g))
 
     def sumsq(self):

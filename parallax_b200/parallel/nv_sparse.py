@@ -394,6 +394,10 @@ class NVSparseGroup(object):
         self.protocol = opts.get("_protocol", "nvlink")
         self.max_blocks = int(opts.get("sparse_blocks", consts.NUM_SMS * 2))
         self.early_push = bool(opts.get("sparse_early_push", True))
+        # sess_config["micro_batches"] = K: the rows of all K micro-batches of a step are
+        # pushed together, after the last one's backward, and weighted 1/K on the owner
+        self.micro_batches = int(opts.get("micro_batches", 1))
+        self._last_mb = True
         hints = [t.capacity_hint for t in tables if t.capacity_hint]
         self.capacity_hint = max(hints) if hints else None
         self.hp = hp_stage(self.fabric, t0.optimizer)
@@ -625,7 +629,7 @@ class NVSparseGroup(object):
         self.calls.append((token, gs))
         self._bwd_calls += 1
         if self.early_push and self._bwd_calls == self._fwd_calls and self._cur_step > 0 \
-                and self.ring_ready():
+                and self._last_mb and self.ring_ready():
             self._run_step(self._cur_step)
 
     def ring_ready(self):
@@ -721,6 +725,11 @@ class NVSparseGroup(object):
         self.hp.upload(step)
         self._cur_step = step
         self._fwd_calls = self._bwd_calls = 0
+
+    def micro_batch(self, k, K):
+        """The engine runs micro-batch `k` of `K` of the step next: only the last one's
+        backward may push."""
+        self._last_mb = k == K - 1
 
     def finish_step(self, step, stream=None):
         if self._done_step == step and not self.calls:
@@ -851,6 +860,8 @@ class NVSparseGroup(object):
             d.hp, d.D4, d.D, d.kind = hp_ptr, t.D4, t.D, _optim.KIND_ID[t.kind]
             d.w_bf16, d.seed, d.slot_part = int(bf16), t.sr_seed, self._slot_part_dev.data_ptr()
             avg = (1.0 / self.world) if t.average else 1.0
+            if self.micro_batches > 1:
+                avg /= self.micro_batches
             d.avg = avg if sender_scaled else avg * t.scale
         return descs
 

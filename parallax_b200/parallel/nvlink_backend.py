@@ -27,7 +27,7 @@ from .layout import TableLayout, assign_owners
 from .nv_sparse import NVSparseTable, NVSparseGroup, hp_stage     # noqa: F401 (re-export)
 from .symmetric import (SymmetricHeap, IpcExchange, CH_COMM, CH_MAIN, CH_SMALL)
 
-MODE_FUSED, MODE_REDUCE, MODE_UPDATE = 0, 1, 2
+MODE_FUSED, MODE_REDUCE, MODE_UPDATE, MODE_ACCUMULATE = 0, 1, 2, 3
 _ES = {torch.float32: 4, torch.bfloat16: 2}
 
 
@@ -121,6 +121,11 @@ class NVDenseGroup(object):
         # been pushed (`finish_step`): it becomes ready right when backward reaches the
         # embedding gradients, and must not sit in front of their push on the comm stream
         self.defer_last = bool(opts.get("dense_defer_last", True))
+        # sess_config["micro_batches"] = K: micro-batch k < K-1 of a step reduces every bucket
+        # into its fp32 accumulator `red` (MODE_ACCUMULATE); the last one runs the step's
+        # usual kernels with the accumulator folded in.  Every gradient is weighted 1/(W·K).
+        self.micro_batches = int(opts.get("micro_batches", 1))
+        self._mb = 0
         self._build_buckets()
         self._install_hooks()
         self._next = 0
@@ -271,7 +276,7 @@ class NVDenseGroup(object):
                 self.ema_rule.applies_to(n) for n, _, _, _ in b.items):
             b.ema = mk(src=b.master)
         b.red = torch.empty(b.slice, dtype=torch.float32, device=dev) \
-            if (b.clip >= 0 and sharded) else None
+            if ((b.clip >= 0 or self.micro_batches > 1) and sharded) else None
 
     def _install_hooks(self):
         for b in self.buckets:
@@ -341,7 +346,8 @@ class NVDenseGroup(object):
         last = len(self.buckets) - 1
         while self._next < len(self.buckets) and \
                 getattr(self.buckets[self._next], "is_ready", False):
-            if self._next == last and self.defer_last and not final:
+            if self._next == last and self.defer_last and not final and \
+                    self._mb == self.micro_batches - 1:
                 break
             b = self.buckets[self._next]
             self._launch(b)
@@ -371,19 +377,27 @@ class NVDenseGroup(object):
         s1 = b.slots[1] if self.nslots > 1 else None
         s2 = b.slots[2] if self.nslots > 2 else None
         st = self.clip_state.get(b.clip)
-        if self.update == "sharded":
+        K = self.micro_batches
+        avg = 1.0 / (W * K)
+        acc_in = self._mb > 0
+        if self.update == "sharded" and self._mb < K - 1:
+            nvops.dense_step(heap, self._grad_sources(b), self._param_targets(b),
+                             b.master, s0, s1, b.ema, b.red, self.hp, None, None, b.n, avg,
+                             ema_decay, self.kind, MODE_ACCUMULATE, b.dtype, CH_COMM,
+                             max_blocks=mb, stream=cs, use_mc=b.mc, slot2=s2, acc_in=acc_in)
+        elif self.update == "sharded":
             if st is None:
                 nvops.dense_step(heap, self._grad_sources(b), self._param_targets(b),
-                                 b.master, s0, s1, b.ema, None, self.hp, None,
-                                 None, b.n, 1.0 / W, ema_decay, self.kind,
+                                 b.master, s0, s1, b.ema, b.red if acc_in else None,
+                                 self.hp, None, None, b.n, avg, ema_decay, self.kind,
                                  MODE_FUSED, b.dtype, CH_COMM, max_blocks=mb,
-                                 stream=cs, use_mc=b.mc, slot2=s2)
+                                 stream=cs, use_mc=b.mc, slot2=s2, acc_in=acc_in)
             else:
                 nvops.dense_step(heap, self._grad_sources(b), self._param_targets(b),
                                  b.master, s0, s1, b.ema, b.red, self.hp, None,
-                                 st.local, b.n, 1.0 / W, ema_decay, self.kind,
+                                 st.local, b.n, avg, ema_decay, self.kind,
                                  MODE_REDUCE, b.dtype, CH_COMM, max_blocks=mb,
-                                 stream=cs, use_mc=b.mc, slot2=s2)
+                                 stream=cs, use_mc=b.mc, slot2=s2, acc_in=acc_in)
                 self.contributed(st, cs)
         elif self.update == "replicated":
             # classic AR: all-reduce (mean) then every replica updates itself
@@ -458,7 +472,7 @@ class NVDenseGroup(object):
                 nvops.dense_step(self.heap, self._grad_sources(bb),
                                  self._param_targets(bb), bb.master, t0, t1,
                                  bb.ema, bb.red, self.hp, st.scale, None,
-                                 bb.n, 1.0 / W, ema_decay, self.kind,
+                                 bb.n, 1.0 / (W * self.micro_batches), ema_decay, self.kind,
                                  MODE_UPDATE, bb.dtype, CH_COMM,
                                  max_blocks=mb, stream=cs, use_mc=bb.mc, slot2=t2)
             else:
@@ -503,18 +517,36 @@ class NVDenseGroup(object):
     def close(self):
         _sinks.unregister_all(self.params)
 
-    def finish_step(self, step):
-        # buckets whose parameters received no gradient this step
+    def micro_batch(self, k, K):
+        """The engine runs micro-batch `k` of `K` of the step next."""
+        self._mb = k
+
+    def end_micro_batch(self):
+        """After the backward pass of a micro-batch that is not the step's last: every
+        bucket has been reduced into its accumulator (MODE_ACCUMULATE) or is now; the
+        bucket state starts over for the next micro-batch."""
+        self._flush_buckets()
+        self._reset_buckets()
+
+    def _flush_buckets(self):
+        # buckets whose parameters received no gradient this (micro-)step
         for b in self.buckets:
             if not getattr(b, "is_ready", False):
                 self._bucket_ready(b)
         self._drain(final=True)
         assert self._next == len(self.buckets)
-        torch.cuda.current_stream(self.device).wait_stream(self.fabric.comm_stream)
+
+    def _reset_buckets(self):
         for b in self.buckets:
             b.ready, b.is_ready, b.launched = 0, False, False
             b.async_events = []
         self._next = 0
+
+    def finish_step(self, step):
+        self._flush_buckets()
+        torch.cuda.current_stream(self.device).wait_stream(self.fabric.comm_stream)
+        self._reset_buckets()
+        self._mb = 0
 
     def zero_grad(self):
         for p in self.params:

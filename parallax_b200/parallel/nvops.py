@@ -82,13 +82,15 @@ def allgather(heap, buf_cptrs, slice_bytes, channels, max_blocks=32, stream=None
 def dense_step(heap, grads_cptrs, params_cptrs, master, slot0, slot1, ema, red,
                hp, clip, sumsq, n, avg, ema_decay, kind, mode, dtype, channels,
                rank=None, world=None, max_blocks=32, stream=None, use_mc=False,
-               slot2=None):
+               slot2=None, acc_in=False):
+    """One fused dense step (`kernels/dense_step.cu`).  `acc_in`: `red` holds the scaled
+    gradient sum of the step's earlier micro-batches; modes 0, 1 and 3 add it first."""
     L = ops.lib()
     _count()
     ops.check(L.px_dense_step(
         grads_cptrs, params_cptrs, _p(master), _p(slot0), _p(slot1), _p(slot2), _p(ema),
         _p(red), _p(hp), _p(clip), _p(sumsq), n, avg, ema_decay, KIND_ID[kind],
-        mode, DT[dtype], _p(heap.pads_dev()) if heap is not None else _vp(0),
+        mode, 1 if acc_in else 0, DT[dtype], _p(heap.pads_dev()) if heap is not None else _vp(0),
         _p(heap.epoch) if heap is not None else _vp(0), channels[0], channels[1],
         heap.rank if rank is None else rank,
         heap.world if world is None else world, max_blocks, 1 if use_mc else 0,
