@@ -29,6 +29,9 @@ ap.add_argument("--batch_size", type=int, default=16)
 ap.add_argument("--seq_len", type=int, default=512)
 ap.add_argument("--mlm_fraction", type=float, default=0.15)
 ap.add_argument("--learning_rate", type=float, default=1e-4)
+ap.add_argument("--optimizer", default="adam", choices=["adam", "lamb"],
+                help="lamb: LAMB for the dense variables (the large-batch recipe), Adam for "
+                     "the word embedding")
 ap.add_argument("--num_partitions", type=int, default=8)
 ap.add_argument("--max_steps", type=int, default=100)
 ap.add_argument("--log_frequency", type=int, default=10)
@@ -38,7 +41,7 @@ FLAGS = ap.parse_args()
 def main():
     model = Bert(vocab=FLAGS.vocab_size, max_len=FLAGS.seq_len,
                  num_partitions=FLAGS.num_partitions, **SIZES[FLAGS.size])
-    graph = bert_graph(model, FLAGS.learning_rate)
+    graph = bert_graph(model, FLAGS.learning_rate, optimizer=FLAGS.optimizer)
     sess, num_workers, worker_id, _ = parallax.parallel_run(
         graph, FLAGS.resource_info_file, sync=FLAGS.sync,
         parallax_config=parallax_config.build_config(FLAGS))

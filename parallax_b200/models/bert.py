@@ -60,7 +60,23 @@ def bert_large(**kw):
     return Bert(hidden=1024, layers=24, heads=16, ff=4096, **kw)
 
 
-def bert_graph(model, learning_rate=1e-4):
+# the parameters BERT's LAMB recipe neither decays nor adapts: LayerNorm gains and biases
+LAMB_EXCLUDE = [r"(^|\.)(ln\d*|mlm_ln)\.", r"(^|\.)bias$"]
+
+
+def bert_graph(model, learning_rate=1e-4, optimizer="adam"):
+    """`optimizer="adam"` trains every variable with Adam.  `optimizer="lamb"` is the
+    large-batch recipe: LAMB with weight decay 0.01, LayerNorm and bias parameters excluded
+    from the decay and the trust ratio, for the dense variables, and Adam for the
+    `word_emb` table."""
     dense = lambda n: n != "word_emb.weight"
-    return Graph(model, optimizer=optim.Adam(learning_rate, weight_decay=0.0),
-                 grad_rules=[ClipByGlobalNorm(1.0, params=dense)], name="bert")
+    clip = [ClipByGlobalNorm(1.0, params=dense)]
+    if optimizer == "adam":
+        return Graph(model, optimizer=optim.Adam(learning_rate, weight_decay=0.0),
+                     grad_rules=clip, name="bert")
+    if optimizer == "lamb":
+        return Graph(model, optimizer=optim.Lamb(learning_rate, weight_decay=0.01,
+                                                 exclude_from_weight_decay=LAMB_EXCLUDE),
+                     sparse_optimizer=optim.Adam(learning_rate, weight_decay=0.0),
+                     grad_rules=clip, name="bert")
+    raise ValueError("bert_graph: optimizer must be 'adam' or 'lamb', not %r" % (optimizer,))

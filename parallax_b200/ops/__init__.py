@@ -83,6 +83,13 @@ _SIGS = {
                                c_size_t, c_int, c_int, c_int, c_int, c_int,
                                c_void_p]),
     "px_sumsq": (c_int, [c_void_p, c_size_t, c_int, c_float, c_void_p, c_void_p]),
+    "px_layerwise_norm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                  c_void_p, c_int, c_int, c_int, c_void_p]),
+    "px_layerwise_update": (c_int, [PP, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                    c_void_p, c_size_t, c_float, c_int, c_int, c_void_p,
+                                    c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "px_sparse_lookup": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(LookupTable),
                                  c_int, c_void_p, ctypes.POINTER(GroupGeom), c_void_p,
                                  c_void_p, c_int, c_void_p]),

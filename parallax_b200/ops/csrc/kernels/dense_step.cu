@@ -334,6 +334,186 @@ px_sumsq_kernel(const T* __restrict__ x, size_t n, float mul, float* out) {
   block_atomic_sum(ss, out);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Layer-wise rules (family 3: LARS, LAMB).  A bucket's step scales every tensor's update by a
+// trust ratio of two norms over the WHOLE tensor, which may straddle several owners' slices:
+//   MODE 1 (unchanged)  : reduce → `red` (+ Σg² under a clip rule)
+//   px_lw_norm_kernel   : per chunk of this slice, Σw² and Σx² (x = g for LARS, r for LAMB)
+//                         → partials[chunk]; no atomics
+//   px_lw_combine_kernel: per segment (tensor), its chunks' partials in chunk order → sums
+//   one-shot all-reduce : sums → total, bitwise identical on every rank (W > 1 only)
+//   px_lw_update_kernel : trust ratio per segment, rule, EMA, push of the parameters, end barrier
+// The chunk table is built once per bucket and rank on the host (nvlink_backend.py): a chunk
+// lies inside one tensor, in units of the bucket's 16-byte vectors relative to the slice start;
+// padding vectors belong to no chunk and are never touched.  `ne` counts the chunk's elements
+// that belong to the tensor: the tail of a tensor's last vector is left out of its sums.
+struct LwChunk { int v0, nv, seg, ne; };
+
+struct LayerwiseArgs {
+  const float* red;      // [slice] reduced gradient (1/W and micro-batch weights applied)
+  float* master;         // [slice]
+  float* slot0;          // LARS momentum / LAMB m
+  float* slot1;          // LAMB v or null
+  float* ema;            // [slice] or null
+  const float* hp;       // device hyper-parameters (10 floats)
+  const float* clip;     // device scalar multiplier or null
+  const LwChunk* chunks; // [nchunks]
+  const int* seg_flags;  // [nseg] PX_LW_* bits
+  const int* seg_chunks; // [nseg, 2] first / end chunk of each segment in this slice
+  float* partials;       // [nchunks, 2]
+  float* sums;           // [nseg, 2] this rank's Σw², Σx² (zero outside the slice)
+  const float* total;    // [nseg, 2] sums over every rank
+  int nchunks, nseg, kind;
+};
+
+__device__ __forceinline__ float2 lw_block_sum2(float a, float b) {
+  __shared__ float2 s_part[32];
+  a = warp_sum(a); b = warp_sum(b);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) s_part[wid] = make_float2(a, b);
+  __syncthreads();
+  float2 t = make_float2(0.f, 0.f);
+  if (wid == 0) {
+    if (lane < (int)(blockDim.x + 31) / 32) t = s_part[lane];
+    t.x = warp_sum(t.x); t.y = warp_sum(t.y);
+  }
+  __syncthreads();          // s_part is reused by the next chunk
+  return t;
+}
+
+template <int VN>
+__global__ void __launch_bounds__(512)
+px_lw_norm_kernel(LayerwiseArgs a) {
+  // the decay is read per chunk, next to its flag: held across the chunk loop (and the
+  // sqrt / division slow-path calls inside it), ptxas spilled it at the fp32 width
+  const float b1 = a.hp[HP_A], b2 = a.hp[HP_B], eps = a.hp[HP_EPS];
+  const float bc1 = a.hp[HP_BC1], bc2 = a.hp[HP_BC2];
+  const float gmul = a.clip != nullptr ? *a.clip : 1.f;
+  for (int c = blockIdx.x; c < a.nchunks; c += gridDim.x) {
+    const LwChunk ch = a.chunks[c];
+    const float wd = (a.seg_flags[ch.seg] & PX_LW_DECAY) ? a.hp[HP_WD] : 0.f;
+    float sw = 0.f, sx = 0.f;
+    for (int v = threadIdx.x; v < ch.nv; v += blockDim.x) {
+      const size_t e = (size_t)(ch.v0 + v) * VN;
+      const int lim = ch.ne - v * VN;
+      float g[VN], w[VN], s0[VN], s1[VN];
+      ld_f32<VN>(a.red + e, g);
+      ld_f32<VN>(a.master + e, w);
+      if (a.kind == PX_LAMB) {
+        ld_f32<VN>(a.slot0 + e, s0);
+        ld_f32<VN>(a.slot1 + e, s1);
+      }
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        float x = g[i] * gmul;
+        if (a.kind == PX_LAMB) x = px_lamb_r(b1, b2, eps, bc1, bc2, wd, x, w[i], s0[i], s1[i]);
+        if (i < lim) {
+          sw = fmaf(w[i], w[i], sw);
+          sx = fmaf(x, x, sx);
+        }
+      }
+    }
+    const float2 t = lw_block_sum2(sw, sx);
+    if (threadIdx.x == 0) { a.partials[2 * c] = t.x; a.partials[2 * c + 1] = t.y; }
+  }
+}
+
+// one thread per segment: its chunks' partials in chunk order (fixed, so the sums — and with
+// them the parameters — are reproducible run to run)
+__global__ void __launch_bounds__(256)
+px_lw_combine_kernel(LayerwiseArgs a) {
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < a.nseg; s += gridDim.x * blockDim.x) {
+    double sw = 0.0, sx = 0.0;
+    for (int c = a.seg_chunks[2 * s]; c < a.seg_chunks[2 * s + 1]; ++c) {
+      sw += a.partials[2 * c];
+      sx += a.partials[2 * c + 1];
+    }
+    a.sums[2 * s] = (float)sw;
+    a.sums[2 * s + 1] = (float)sx;
+  }
+}
+
+__device__ __forceinline__ float px_lw_trust(int kind, const PxHP& h, int flags, float sw,
+                                             float sx) {
+  const float wn = sqrtf(sw), xn = sqrtf(sx);
+  if (!(flags & PX_LW_ADAPT) || !(wn > 0.f && xn > 0.f)) return 1.f;
+  return kind == PX_LARS ? h.b * wn / (xn + h.wd * wn + h.eps) : wn / xn;
+}
+
+template <typename T, int W>
+__global__ void __launch_bounds__(512)
+px_lw_update_kernel(LayerwiseArgs a, PeerPtrs params, size_t n, float ema_decay, int rank,
+                    int ch_end, int use_mc, uint32_t* const* pads, uint32_t* epoch_ctr) {
+  constexpr int VN = Vec16<T>::N;
+  const PxHP h = px_load_hp(a.hp);
+  const float bc1 = a.hp[HP_BC1], bc2 = a.hp[HP_BC2];
+  const float gmul = a.clip != nullptr ? *a.clip : 1.f;
+  const size_t base = (size_t)rank * (n / W);
+  for (int c = blockIdx.x; c < a.nchunks; c += gridDim.x) {
+    const LwChunk ch = a.chunks[c];
+    const int flags = a.seg_flags[ch.seg];
+    const float lr_t = h.lr * px_lw_trust(a.kind, h, flags, a.total[2 * ch.seg],
+                                          a.total[2 * ch.seg + 1]);
+    const float wd = (flags & PX_LW_DECAY) ? h.wd : 0.f;
+    for (int v = threadIdx.x; v < ch.nv; v += blockDim.x) {
+      const size_t e = (size_t)(ch.v0 + v) * VN;
+      float g[VN], w[VN], s0[VN], s1[VN], m[VN];
+      ld_f32<VN>(a.red + e, g);
+      ld_f32<VN>(a.master + e, w);
+      ld_f32<VN>(a.slot0 + e, s0);
+      if (a.kind == PX_LAMB) ld_f32<VN>(a.slot1 + e, s1);
+      if (a.ema) ld_f32<VN>(a.ema + e, m);
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        const float gi = g[i] * gmul;
+        if (a.kind == PX_LARS) {
+          s0[i] = fmaf(h.a, s0[i], gi);
+          w[i] = fmaf(-lr_t, (flags & PX_LW_NESTEROV) ? fmaf(h.a, s0[i], gi) : s0[i], w[i]);
+        } else {
+          const float r = px_lamb_r(h.a, h.b, h.eps, bc1, bc2, wd, gi, w[i], s0[i], s1[i]);
+          w[i] = fmaf(-lr_t, r, w[i]);
+        }
+      }
+      st_f32<VN>(a.master + e, w);
+      st_f32<VN>(a.slot0 + e, s0);
+      if (a.kind == PX_LAMB) st_f32<VN>(a.slot1 + e, s1);
+      if (a.ema) {
+#pragma unroll
+        for (int i = 0; i < VN; ++i) m[i] -= (1.f - ema_decay) * (m[i] - w[i]);
+        st_f32<VN>(a.ema + e, m);
+      }
+      const uint4 out = Vec16<T>::pack(w);
+      if (use_mc) {
+        ds_mm_st(reinterpret_cast<T*>(params.p[0]) + base + e, out);
+      } else {
+#pragma unroll
+        for (int p = 0; p < W; ++p) st_v4_stream(reinterpret_cast<T*>(params.p[p]) + base + e, out);
+      }
+    }
+  }
+  // MODE 2's end barrier: the last CTA announces that this rank's parameter stores are out and
+  // waits for the same from every peer
+  if (W > 1) {
+    const int slot_e = ch_end * PX_MAX_BLOCKS;
+    __shared__ bool s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence_system();
+      s_last = atomicAdd(epoch_ctr + slot_e + 1, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (s_last) {
+      const uint32_t e_end = ld_volatile_u32(epoch_ctr + slot_e) + 1;
+      px_rank_signal(pads, slot_e, rank, W, e_end);
+      px_rank_wait(pads, slot_e, rank, W, e_end);
+      if (threadIdx.x == 0) {
+        epoch_ctr[slot_e] = e_end;
+        epoch_ctr[slot_e + 1] = 0;
+      }
+    }
+  }
+}
+
 extern "C" {
 
 // dtype 0 fp32 / 1 bf16.  grads/params: `world` pointers in natural order.
@@ -350,6 +530,8 @@ int px_dense_step(const void* const* grads, const void* const* params, float* ma
   const bool acc = mode == 3 || acc_in;
   if (mode < 0 || mode > 3 || (acc && (red == nullptr || clip != nullptr || mode == 2)))
     return -2;
+  // modes 0 and 2 apply an elementwise rule: the layer-wise and row-wise kinds have none here
+  if ((mode == 0 || mode == 2) && (kind < 0 || kind > PX_CENTERED_RMSPROP)) return -4;
   DenseStepArgs a;
   a.use_mc = use_mc;
   if (use_mc) {            // entry 0 = multicast address; no peer pointers needed
@@ -409,6 +591,7 @@ int px_dense_async(const void* my_grads, void* my_params, const void* const* mas
   if (world < 1 || world > 8) return -3;
   const int vn = dtype == 0 ? 4 : 8;
   if (n % ((size_t)world * vn) != 0) return -1;
+  if (kind < 0 || kind > PX_CENTERED_RMSPROP) return -4;     // elementwise rules only
   PeerPtrs M{}, S0{}, S1{}, S2{};
   for (int i = 0; i < world; ++i) {
     M.p[i] = const_cast<void*>(master[i]);
@@ -437,6 +620,75 @@ int px_sumsq(const void* x, size_t n, int dtype, float mul, float* out, cudaStre
   const int blocks = px_clamp_blocks(n / vn, 512 * 4, PX_NUM_SMS * 2);
   if (dtype == 0) px_sumsq_kernel<float><<<blocks, 512, 0, stream>>>((const float*)x, n, mul, out);
   else px_sumsq_kernel<__nv_bfloat16><<<blocks, 512, 0, stream>>>((const __nv_bfloat16*)x, n, mul, out);
+  return (int)cudaGetLastError();
+}
+
+// Layer-wise passes of one bucket (kind PX_LARS / PX_LAMB, sharded update).  `chunks`,
+// `seg_flags`, `seg_chunks`: the bucket's segment map for this rank (device); `red`, `master`,
+// slots and `ema` are this rank's slices.
+//   px_layerwise_norm  : norm pass and per-segment combine → sums [nseg, 2]
+//   px_layerwise_update: trust ratios from `total` (the all-reduced sums; `sums` itself at
+//                        W = 1), the update, the push to `params` and the end barrier
+static int lw_args(LayerwiseArgs& a, int kind, const float* red, float* master, float* slot0,
+                   float* slot1, float* ema, const float* hp, const float* clip,
+                   const void* chunks, int nchunks, const int* seg_flags, const int* seg_chunks,
+                   int nseg, float* partials, float* sums, const float* total) {
+  if (kind != PX_LARS && kind != PX_LAMB) return -4;
+  if (red == nullptr || master == nullptr || slot0 == nullptr ||
+      (kind == PX_LAMB && slot1 == nullptr) || nchunks < 0 || nseg < 0) return -2;
+  a.red = red; a.master = master; a.slot0 = slot0; a.slot1 = slot1; a.ema = ema; a.hp = hp;
+  a.clip = clip; a.chunks = (const LwChunk*)chunks; a.nchunks = nchunks; a.seg_flags = seg_flags;
+  a.seg_chunks = seg_chunks; a.nseg = nseg; a.partials = partials; a.sums = sums;
+  a.total = total; a.kind = kind;
+  return 0;
+}
+
+int px_layerwise_norm(const float* red, const float* master, const float* slot0,
+                      const float* slot1, const float* hp, const float* clip, const void* chunks,
+                      int nchunks, const int* seg_flags, const int* seg_chunks, int nseg,
+                      float* partials, float* sums, int kind, int dtype, int max_blocks,
+                      cudaStream_t stream) {
+  LayerwiseArgs a;
+  const int rc = lw_args(a, kind, red, const_cast<float*>(master), const_cast<float*>(slot0),
+                         const_cast<float*>(slot1), nullptr, hp, clip, chunks, nchunks,
+                         seg_flags, seg_chunks, nseg, partials, sums, nullptr);
+  if (rc != 0) return rc;
+  if (nseg == 0) return 0;
+  const int cap = max_blocks > 0 ? max_blocks : PX_NUM_SMS * 4;
+  const int blocks = nchunks < 1 ? 1 : (nchunks > cap ? cap : nchunks);
+  if (nchunks > 0) {
+    if (dtype == 0) px_lw_norm_kernel<4><<<blocks, 512, 0, stream>>>(a);
+    else px_lw_norm_kernel<8><<<blocks, 512, 0, stream>>>(a);
+  }
+  px_lw_combine_kernel<<<(nseg + 255) / 256, 256, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+int px_layerwise_update(const void* const* params, const float* red, float* master, float* slot0,
+                        float* slot1, float* ema, const float* hp, const float* clip,
+                        const void* chunks, int nchunks, const int* seg_flags, int nseg,
+                        const float* total, size_t n, float ema_decay, int kind, int dtype,
+                        void* pads_dev, void* epoch_ctr, int ch_end, int rank, int world,
+                        int max_blocks, int use_mc, cudaStream_t stream) {
+  if (world < 1 || world > 8) return -3;
+  const int vn = dtype == 0 ? 4 : 8;
+  if (n % ((size_t)world * vn) != 0) return -1;
+  LayerwiseArgs a;
+  const int rc = lw_args(a, kind, red, master, slot0, slot1, ema, hp, clip, chunks, nchunks,
+                         seg_flags, nullptr, nseg, nullptr, nullptr, total);
+  if (rc != 0) return rc;
+  PeerPtrs P{};
+  if (use_mc) P.p[0] = const_cast<void*>(params[0]);
+  else P = px_rotate(params, rank, world);
+  const int cap = world == 1 ? PX_NUM_SMS * 4 : (max_blocks > 0 ? max_blocks : PX_NUM_SMS);
+  const int blocks = nchunks < 1 ? 1 : (nchunks > cap ? cap : nchunks);
+#define LAUNCH(T, W)                                                                       \
+  px_lw_update_kernel<T, W><<<blocks, 512, 0, stream>>>(a, P, n, ema_decay, rank, ch_end,  \
+                                                        use_mc, (uint32_t* const*)pads_dev, \
+                                                        (uint32_t*)epoch_ctr)
+  if (dtype == 0) { PX_DISPATCH_WORLD(world, LAUNCH, float); }
+  else { PX_DISPATCH_WORLD(world, LAUNCH, __nv_bfloat16); }
+#undef LAUNCH
   return (int)cudaGetLastError();
 }
 

@@ -11,6 +11,9 @@
 //   family 2: row-wise adagrad — one accumulator per table row, fed by the row's mean g²;
 //             sparse owner kernel only (`px_sparse_owner_kernel<.., 2>` in sparse.cu), since
 //             the rule needs the whole row before it can update any element of it
+//   family 3: layer-wise rules, LARS and LAMB — the step of each dense tensor is scaled by a
+//             trust ratio of two norms over the whole tensor; dense only, run by the norm and
+//             update passes of dense_step.cu (`px_layerwise_norm` / `px_layerwise_update`)
 // Numerics oracle: `parallax_b200/optim.py::apply_dense_` / `apply_sparse_rows_`.
 #pragma once
 #include <cuda_runtime.h>
@@ -18,13 +21,17 @@
 enum {
   PX_SGD = 0, PX_MOMENTUM = 1, PX_ADAGRAD = 2, PX_ADAM = 3, PX_RMSPROP = 4,
   PX_ADADELTA = 5, PX_FTRL = 6, PX_PROX_SGD = 7, PX_PROX_ADAGRAD = 8, PX_ADAGRAD_DA = 9,
-  PX_CENTERED_RMSPROP = 10, PX_ROWWISE_ADAGRAD = 11
+  PX_CENTERED_RMSPROP = 10, PX_ROWWISE_ADAGRAD = 11, PX_LARS = 12, PX_LAMB = 13
 };
 #define PX_KIND_FAMILY(kind) \
-  ((kind) <= PX_RMSPROP ? 0 : (kind) <= PX_CENTERED_RMSPROP ? 1 : 2)
+  ((kind) <= PX_RMSPROP ? 0 : (kind) <= PX_CENTERED_RMSPROP ? 1 \
+   : (kind) == PX_ROWWISE_ADAGRAD ? 2 : 3)
 
-// device hyper-parameter vector (8 floats), see optim.py
-enum { HP_LR = 0, HP_A, HP_B, HP_EPS, HP_WD, HP_STEP, HP_GSCALE, HP_FLAGS };
+// device hyper-parameter vector (10 floats), see optim.py; HP_BC1 / HP_BC2 are LAMB's bias
+// corrections 1/(1-β1ᵗ), 1/(1-β2ᵗ), read by the layer-wise passes only
+enum { HP_LR = 0, HP_A, HP_B, HP_EPS, HP_WD, HP_STEP, HP_GSCALE, HP_FLAGS, HP_BC1, HP_BC2 };
+// per-tensor flags of the layer-wise rules (optim.py LW_*)
+enum { PX_LW_NESTEROV = 1, PX_LW_DECAY = 2, PX_LW_ADAPT = 4 };
 
 struct PxHP { float lr, a, b, eps, wd, step, flags; };
 __device__ __forceinline__ PxHP px_load_hp(const float* hp) {
@@ -120,4 +127,13 @@ __device__ __forceinline__ void px_rule4(int kind, const PxHP& h, const float4& 
   px_rule<FAM>(kind, h, g.y, w.y, s0.y, s1.y, s2.y);
   px_rule<FAM>(kind, h, g.z, w.z, s0.z, s1.z, s2.z);
   px_rule<FAM>(kind, h, g.w, w.w, s0.w, s1.w, s2.w);
+}
+
+// LAMB's update direction r for one element, and the new moments m, v (a = β1, b = β2).  The
+// norm pass and the update pass of dense_step.cu both call it, so they agree on r bit for bit.
+__device__ __forceinline__ float px_lamb_r(float a, float b, float eps, float bc1, float bc2,
+                                           float wd, float g, float w, float& m, float& v) {
+  m = fmaf(a, m, (1.f - a) * g);
+  v = fmaf(b, v, (1.f - b) * g * g);
+  return fmaf(wd, w, (m * bc1) / (sqrtf(v * bc2) + eps));
 }

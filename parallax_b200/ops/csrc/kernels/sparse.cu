@@ -1183,6 +1183,11 @@ static inline int push_hbits(int n, int blocks) {
 
 // grad_dtype / wire_dtype: 0 fp32, 1 bf16.  async: 1 = remote optimizer application (Hogwild).
 // All member tables of a group use the same optimizer kind family.
+// The kinds the sparse kernels implement: the elementwise families 0 and 1 and the row-wise
+// family 2.  Any other kind (the dense-only layer-wise rules among them) is refused, never
+// applied as nothing or as another family's rule.
+static bool px_sparse_kind(int kind) { return kind >= PX_SGD && kind <= PX_ROWWISE_ADAGRAD; }
+
 int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt,
                    int grad_dtype, int wire_dtype, int async, void* ring_ids_dev, void* hdrs_dev,
                    int cap, const GroupGeom* g, void* ctl, int rank, int dedup, int max_blocks,
@@ -1194,6 +1199,7 @@ int px_sparse_push(const int32_t* pend_ids, int n, const PushTable* tabs, int nt
   a.cap = cap; a.rank = rank;
   const int fam = PX_KIND_FAMILY(tabs[0].kind);
   for (int t = 0; t < nt; ++t) {
+    if (!px_sparse_kind(tabs[t].kind)) return -9;
     if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
     a.t[t] = tabs[t];
   }
@@ -1231,6 +1237,7 @@ int px_sparse_owner(const OwnerTable* tabs, int nt, int wire_dtype, const int32_
   const int fam = PX_KIND_FAMILY(tabs[0].kind);
   const int w_bf16 = tabs[0].w_bf16 != 0;
   for (int t = 0; t < nt; ++t) {
+    if (!px_sparse_kind(tabs[t].kind)) return -9;
     if (PX_KIND_FAMILY(tabs[t].kind) != fam) return -6;
     if ((tabs[t].w_bf16 != 0) != w_bf16) return -8;   // members share one master type
     a.t[t] = tabs[t];

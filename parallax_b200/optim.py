@@ -23,6 +23,10 @@ Update rules (g = aggregated gradient):
 * rmsprop  : ms = ρ·ms+(1-ρ)g² ; mom = μ·mom + lr·g/sqrt(ms+ε) ; w -= mom
 * rowwise_adagrad (sparse variables only): one accumulator per row,
              s += mean_j(g_j²) ; w -= lr·g / (sqrt(s) + ε)
+* lars     (dense only, layer-wise): trust = η‖w‖/(‖g‖ + λ‖w‖ + ε) per tensor ;
+             mom = μ·mom + g ; w -= lr·trust·mom
+* lamb     (dense only, layer-wise): m, v as Adam ; r = m̂/(sqrt(v̂)+ε) + λw ;
+             w -= lr·(‖w‖/‖r‖)·r, the norms over the whole tensor
 
 Sparse variants touch only the rows present in the aggregated gradient
 ("lazy" Adam/momentum, exactly like TF's sparse apply ops).
@@ -43,11 +47,16 @@ HOST_KINDS = EXT_KINDS            # historical name
 # family 2: rules that keep one fp32 slot value per table ROW (sparse variables only; the
 # sparse owner kernel merges a whole row before it applies it)
 ROWWISE_KINDS = ("rowwise_adagrad",)
-KIND_ID = {k: i for i, k in enumerate(KINDS + EXT_KINDS + ROWWISE_KINDS)}
+# family 3: layer-wise rules, whose step is scaled by a trust ratio of norms over each whole
+# dense tensor (dense variables only; `dense_step.cu` runs them as a norm pass, an all-reduce
+# of the per-tensor sums and an update pass)
+LAYERWISE_KINDS = ("lars", "lamb")
+KIND_ID = {k: i for i, k in enumerate(KINDS + EXT_KINDS + ROWWISE_KINDS + LAYERWISE_KINDS)}
 # number of fp32 state slots per kind
 NUM_SLOTS = {"sgd": 0, "momentum": 1, "adagrad": 1, "adam": 2, "rmsprop": 2,
              "adadelta": 2, "ftrl": 2, "proximal_sgd": 0, "proximal_adagrad": 1,
-             "adagrad_da": 2, "centered_rmsprop": 3, "rowwise_adagrad": 1}
+             "adagrad_da": 2, "centered_rmsprop": 3, "rowwise_adagrad": 1,
+             "lars": 1, "lamb": 2}
 SLOT_NAMES = {
     "sgd": (), "momentum": ("momentum",), "adagrad": ("accumulator",),
     "adam": ("m", "v"), "rmsprop": ("ms", "mom"),
@@ -55,11 +64,15 @@ SLOT_NAMES = {
     "proximal_adagrad": ("accumulator",),
     "adagrad_da": ("gradient_accumulator", "gradient_squared_accumulator"),
     "centered_rmsprop": ("ms", "mg", "mom"), "rowwise_adagrad": ("accumulator",),
+    "lars": ("momentum",), "lamb": ("m", "v"),
 }
 
 
 def kind_family(kind):
-    """Kernel template family of `kind` (`optim_rules.cuh`): 0, 1 or 2 (row-wise)."""
+    """Kernel template family of `kind` (`optim_rules.cuh`): 0, 1, 2 (row-wise) or 3
+    (layer-wise)."""
+    if kind in LAYERWISE_KINDS:
+        return 3
     return 0 if kind in KINDS else 1 if kind in EXT_KINDS else 2
 
 
@@ -146,9 +159,14 @@ def require_fused(kind, where):
             "optimizer kind %r has no fused kernel (%s).  Fused kinds: %s"
             % (kind, where, ", ".join(KIND_ID)))
 
-# layout of the device-side hyper-parameter vector read by the kernels
-HP_LR, HP_A, HP_B, HP_EPS, HP_WD, HP_STEP, HP_GSCALE, HP_FLAGS = range(8)
-HP_SIZE = 8
+# layout of the device-side hyper-parameter vector read by the kernels; HP_BC1 / HP_BC2 are
+# LAMB's bias corrections 1/(1-β1ᵗ) and 1/(1-β2ᵗ), folded on the host in double
+HP_LR, HP_A, HP_B, HP_EPS, HP_WD, HP_STEP, HP_GSCALE, HP_FLAGS, HP_BC1, HP_BC2 = range(10)
+HP_SIZE = 10
+# bits of hp[HP_FLAGS] for the layer-wise rules (the same bits as their per-tensor flags in
+# the dense step's segment map): nesterov (LARS), weight decay applies (LAMB), trust ratio
+# applies (both)
+LW_NESTEROV, LW_DECAY, LW_ADAPT = 1, 2, 4
 
 
 class Optimizer(object):
@@ -170,7 +188,7 @@ class Optimizer(object):
         return tuple(0.0 for _ in range(NUM_SLOTS[self.kind]))
 
     def hyper(self, step):
-        """Vector [lr, a, b, eps, wd, step, gscale, flags] for step `step`
+        """Vector [lr, a, b, eps, wd, step, gscale, flags, bc1, bc2] for step `step`
         (1-based count of the update being applied)."""
         hp = [0.0] * HP_SIZE
         hp[HP_LR] = self.lr_at(step)
@@ -182,6 +200,12 @@ class Optimizer(object):
 
     def _fill(self, hp, step):
         pass
+
+    def hyper_for(self, name, step):
+        """`hyper(step)` for the dense parameter `name`: a layer-wise rule clears the
+        weight-decay and trust-ratio bits of hp[HP_FLAGS] that its exclude lists remove
+        (`layer_flags`); every other rule has no per-name setting."""
+        return self.hyper(step)
 
     def describe(self):
         d = {k: v for k, v in vars(self).items() if not callable(v)}
@@ -349,7 +373,97 @@ class RowWiseAdagrad(Optimizer):
         hp[HP_EPS] = self.epsilon
 
 
+class Lars(Optimizer):
+    """`tf.contrib.opt.LARSOptimizer`: momentum with a layer-wise learning rate (You et al.,
+    2017).  For each dense parameter tensor, with g its gradient (after averaging,
+    `ScaleGradients` and clipping) and w its fp32 master before the update::
+
+        trust = eeta·‖w‖ / (‖g‖ + weight_decay·‖w‖ + epsilon)   if ‖w‖ > 0 and ‖g‖ > 0, else 1
+        mom   = momentum·mom + g
+        w    -= learning_rate·trust·mom       (nesterov: learning_rate·trust·(g + momentum·mom))
+
+    The norms are over the whole tensor.  `weight_decay` enters only the trust ratio, as in
+    the reference: no λw term is added to the gradient.  A parameter whose name contains an
+    entry of `skip_list` as a substring takes trust = 1.  A *dense-variable* optimizer, for
+    sync training only; the engine refuses it for sparse variables."""
+    kind = "lars"
+
+    def __init__(self, learning_rate, momentum=0.9, weight_decay=1e-4, eeta=0.001,
+                 epsilon=0.0, skip_list=None, use_nesterov=False, name=None):
+        super().__init__(learning_rate, weight_decay=weight_decay, name=name)
+        self.momentum, self.eeta, self.epsilon = float(momentum), float(eeta), float(epsilon)
+        self.skip_list = list(skip_list) if skip_list is not None else None
+        self.use_nesterov = bool(use_nesterov)
+
+    def _fill(self, hp, step):
+        hp[HP_A], hp[HP_B], hp[HP_EPS] = self.momentum, self.eeta, self.epsilon
+        hp[HP_FLAGS] = float((LW_NESTEROV if self.use_nesterov else 0) | LW_ADAPT)
+
+    def layer_flags(self, name):
+        """The per-tensor flags of `name`: LW_NESTEROV with `use_nesterov`, and LW_ADAPT
+        unless an entry of `skip_list` is a substring of `name`.  The dense step reads every
+        flag of the rule from these (its segment map), not from hp[HP_FLAGS]."""
+        skip = self.skip_list is not None and any(s in name for s in self.skip_list)
+        return (LW_NESTEROV if self.use_nesterov else 0) | (0 if skip else LW_ADAPT)
+
+    def hyper_for(self, name, step):
+        hp = self.hyper(step)
+        hp[HP_FLAGS] = float(self.layer_flags(name))
+        return hp
+
+
+class Lamb(Optimizer):
+    """LAMB (You et al., 2019; `tfa.optimizers.LAMB`): Adam moments with a layer-wise trust
+    ratio.  For each dense parameter tensor::
+
+        m = β1·m + (1−β1)·g ;  v = β2·v + (1−β2)·g²
+        r = (m/(1−β1ᵗ)) / (sqrt(v/(1−β2ᵗ)) + epsilon)  [+ weight_decay·w]
+        trust = ‖w‖/‖r‖  if ‖w‖ > 0 and ‖r‖ > 0, else 1
+        w -= learning_rate·trust·r
+
+    Weight decay is decoupled (added to r, not to g).  `exclude_from_weight_decay` and
+    `exclude_from_layer_adaptation` are lists of regexes, matched with `re.search` against
+    the dotted parameter name, that turn off the decay term and the trust ratio (trust = 1)
+    of the parameters they match; `exclude_from_layer_adaptation=None` means "the same as
+    `exclude_from_weight_decay`".  A *dense-variable* optimizer, for sync training only."""
+    kind = "lamb"
+
+    def __init__(self, learning_rate=0.001, beta1=0.9, beta2=0.999, epsilon=1e-6,
+                 weight_decay=0.0, exclude_from_weight_decay=None,
+                 exclude_from_layer_adaptation=None, name=None):
+        super().__init__(learning_rate, weight_decay=weight_decay, name=name)
+        self.beta1, self.beta2, self.epsilon = float(beta1), float(beta2), float(epsilon)
+        self.exclude_from_weight_decay = list(exclude_from_weight_decay or [])
+        self.exclude_from_layer_adaptation = list(
+            exclude_from_layer_adaptation if exclude_from_layer_adaptation is not None
+            else self.exclude_from_weight_decay)
+
+    def _fill(self, hp, step):
+        hp[HP_A], hp[HP_B], hp[HP_EPS] = self.beta1, self.beta2, self.epsilon
+        t = max(int(step), 1)
+        hp[HP_BC1] = 1.0 / (1.0 - self.beta1 ** t)
+        hp[HP_BC2] = 1.0 / (1.0 - self.beta2 ** t)
+        hp[HP_FLAGS] = float(LW_DECAY | LW_ADAPT)
+
+    def layer_flags(self, name):
+        """LW_DECAY and LW_ADAPT, each unless one of its exclude patterns matches `name`."""
+        import re
+        f = 0
+        if self.weight_decay != 0.0 and \
+                not any(re.search(p, name) for p in self.exclude_from_weight_decay):
+            f |= LW_DECAY
+        if not any(re.search(p, name) for p in self.exclude_from_layer_adaptation):
+            f |= LW_ADAPT
+        return f
+
+    def hyper_for(self, name, step):
+        hp = self.hyper(step)
+        hp[HP_FLAGS] = float(self.layer_flags(name))
+        return hp
+
+
 # TF-style aliases
+LARSOptimizer = Lars
 AdadeltaOptimizer = Adadelta
 FtrlOptimizer = Ftrl
 ProximalGradientDescentOptimizer = ProximalGradientDescent
@@ -365,11 +479,37 @@ RMSPropOptimizer = RMSProp
 # ---------------------------------------------------------------------------
 # fp32 torch reference math (host fabric + test oracle)
 # ---------------------------------------------------------------------------
+def lamb_direction(g, w, m, v, hp):
+    """LAMB's (new m, new v, r) for gradient g, master w and moments m, v, all fp32; r
+    includes the decoupled weight-decay term when hp[HP_FLAGS] has LW_DECAY."""
+    a, b, eps = hp[HP_A], hp[HP_B], hp[HP_EPS]
+    m = m * a + g * (1.0 - a)
+    v = v * b + g * g * (1.0 - b)
+    r = (m * hp[HP_BC1]) / ((v * hp[HP_BC2]).sqrt() + eps)
+    if int(hp[HP_FLAGS]) & LW_DECAY:
+        r = r + hp[HP_WD] * w
+    return m, v, r
+
+
+def trust_ratio(kind, wn, xn, hp):
+    """Layer-wise trust ratio from ‖w‖ and ‖x‖ (x = g for LARS, r for LAMB): 1 when the
+    rule's LW_ADAPT bit is clear or either norm is 0."""
+    if not int(hp[HP_FLAGS]) & LW_ADAPT or not (wn > 0.0 and xn > 0.0):
+        return 1.0
+    if kind == "lars":
+        return hp[HP_B] * wn / (xn + hp[HP_WD] * wn + hp[HP_EPS])
+    return wn / xn
+
+
 def apply_dense_(kind, w, g, slots, hp):
     """In-place update of fp32 tensor `w` with gradient `g` (already
-    aggregated); `slots` is a tuple of fp32 state tensors shaped like `w`."""
+    aggregated); `slots` is a tuple of fp32 state tensors shaped like `w`.  A layer-wise rule
+    (`LAYERWISE_KINDS`) treats `w` as one whole tensor: its norms are taken over all of it,
+    and its per-tensor flags come from hp[HP_FLAGS] (`Optimizer.hyper_for`)."""
     lr, a, b, eps, wd = hp[HP_LR], hp[HP_A], hp[HP_B], hp[HP_EPS], hp[HP_WD]
     g = g.to(torch.float32) * hp[HP_GSCALE]
+    if kind in LAYERWISE_KINDS:           # weight decay is the rule's own term
+        return _apply_layerwise_(kind, w, g, slots, hp)
     if wd != 0.0:
         g = g + wd * w
     if kind == "sgd":
@@ -439,6 +579,27 @@ def apply_dense_(kind, w, g, slots, hp):
         w.addcdiv_(g, acc.sqrt().add_(eps), value=-lr)
     else:  # pragma: no cover
         raise ValueError(kind)
+    return w
+
+
+def _apply_layerwise_(kind, w, g, slots, hp):
+    lr = hp[HP_LR]
+    wn = float(w.double().norm())
+    if kind == "lars":
+        (mom,) = slots
+        trust = trust_ratio(kind, wn, float(g.double().norm()), hp)
+        mom.mul_(hp[HP_A]).add_(g)
+        if int(hp[HP_FLAGS]) & LW_NESTEROV:
+            w.add_(g + hp[HP_A] * mom, alpha=-lr * trust)
+        else:
+            w.add_(mom, alpha=-lr * trust)
+    else:
+        m, v = slots
+        m_new, v_new, r = lamb_direction(g, w, m, v, hp)
+        trust = trust_ratio(kind, wn, float(r.double().norm()), hp)
+        m.copy_(m_new)
+        v.copy_(v_new)
+        w.add_(r, alpha=-lr * trust)
     return w
 
 

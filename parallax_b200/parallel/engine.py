@@ -235,6 +235,7 @@ class TrainEngine(object):
         self.step_times = []
         self._check_joint_clip(sync)
         self._check_rowwise(sync)
+        self._check_layerwise(sync)
         self._check_sparse_weights(sync)
         self._check_micro_batches(sync)
         self._build()
@@ -434,6 +435,34 @@ class TrainEngine(object):
                 "%s needs sync=True: the asynchronous push applies every worker's rows "
                 "element by element on the owner, without the merged row a row-wise rule "
                 "needs" % type(sparse_opt).__name__)
+
+    def _check_layerwise(self, sync):
+        """Refuse at build, before anything is allocated, what a layer-wise optimizer
+        (`optim.LAYERWISE_KINDS`: LARS, LAMB — a trust ratio per dense tensor) cannot do."""
+        g = self.graph
+        opt, sparse_opt = g.optimizer, g.sparse_optimizer
+        if sparse_opt is not None and sparse_opt.kind in _optim.LAYERWISE_KINDS and \
+                self.analysis.sparse:
+            raise ValueError(
+                "%s scales each dense tensor's step by a trust ratio over the whole tensor and "
+                "has no rule for the rows of sparse variables, but the model has sparse "
+                "variables: give them their own optimizer, e.g. "
+                "Graph(..., sparse_optimizer=Momentum(...)) (the reference LARS's own sparse "
+                "fallback) or Adam(...)" % type(sparse_opt).__name__)
+        if opt is None or opt.kind not in _optim.LAYERWISE_KINDS:
+            return
+        name = type(opt).__name__
+        if not sync:
+            raise ValueError(
+                "%s needs sync=True: its trust ratio is a norm over the whole aggregated "
+                "gradient of a tensor, which an asynchronous PS never forms" % name)
+        if self.backend == "nvlink" and (
+                self.config.sess_option("dense_update", "sharded") == "replicated" or
+                self.config.communication_config.ps_config.protocol == "nccl"):
+            raise ValueError(
+                "%s is not implemented on the NVLink fabric with dense_update='replicated' or "
+                "PSConfig(protocol='nccl'): use the default sharded update, or "
+                "sess_config={'fabric': 'library'} to run it over library collectives" % name)
 
     def grad_norm(self, i):
         """Pre-clip global norm of clip rule `i` (index in the graph's

@@ -113,8 +113,10 @@ class HostDenseGroup(object):
                     grads[i] = flat[off:off + n].view_as(g)
                     off += n
             self._clip(grads, step)
+            per_name = kind in _optim.LAYERWISE_KINDS     # exclude lists act per tensor
             for i, g in enumerate(grads):
-                _optim.apply_dense_(kind, self.master[i], g, self.slots[i], hp)
+                hp_i = self.optimizer.hyper_for(self.names[i], step) if per_name else hp
+                _optim.apply_dense_(kind, self.master[i], g, self.slots[i], hp_i)
         else:
             # asynchronous PS: every worker's gradient is applied on its own,
             # un-averaged.  The host fabric serialises them in rank order.

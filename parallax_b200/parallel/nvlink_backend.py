@@ -29,6 +29,9 @@ from .symmetric import (SymmetricHeap, IpcExchange, CH_COMM, CH_MAIN, CH_SMALL)
 
 MODE_FUSED, MODE_REDUCE, MODE_UPDATE, MODE_ACCUMULATE = 0, 1, 2, 3
 _ES = {torch.float32: 4, torch.bfloat16: 2}
+# segments (tensors) of one layer-wise bucket: its [nseg, 2] fp32 sums must fit one half of the
+# fabric's one-shot stage (2 × 64 KiB)
+LW_MAX_SEGMENTS = 65536 // 8
 
 
 class NVFabric(object):
@@ -112,6 +115,9 @@ class NVDenseGroup(object):
         _optim.require_fused(optimizer.kind, "NVLink fabric")
         self.kind = optimizer.kind
         self.nslots = _optim.NUM_SLOTS[self.kind]
+        # LARS / LAMB: every bucket reduces with MODE_REDUCE, then runs the norm pass, the
+        # all-reduce of its per-tensor sums and the update pass (`_layerwise_update`)
+        self.layerwise = self.kind in _optim.LAYERWISE_KINDS
         self.clip_rules = graph.clip_rules()
         self.ema_rule = graph.ema
         self.last_grad_norm = {}
@@ -155,7 +161,8 @@ class NVDenseGroup(object):
             off = b.n
             b.items.append((name, p, off, p.numel()))
             b.n = off + (p.numel() + vn - 1) // vn * vn
-            if b.n * _ES[p.dtype] >= self.bucket_bytes:
+            if b.n * _ES[p.dtype] >= self.bucket_bytes or \
+                    (self.layerwise and len(b.items) >= LW_MAX_SEGMENTS):
                 del open_b[key]
         self.buckets = buckets
         heap = self.heap
@@ -276,7 +283,13 @@ class NVDenseGroup(object):
                 self.ema_rule.applies_to(n) for n, _, _, _ in b.items):
             b.ema = mk(src=b.master)
         b.red = torch.empty(b.slice, dtype=torch.float32, device=dev) \
-            if ((b.clip >= 0 or self.micro_batches > 1) and sharded) else None
+            if ((b.clip >= 0 or self.micro_batches > 1 or self.layerwise) and sharded) else None
+        b.lw = None
+        if self.layerwise and sharded:
+            b.lw = nvops.LayerwiseMap([(off, numel) for _, _, off, numel in b.items], lo,
+                                      b.slice, 16 // _ES[b.dtype],
+                                      [self.optimizer.layer_flags(n) for n, _, _, _ in b.items],
+                                      dev)
 
     def _install_hooks(self):
         for b in self.buckets:
@@ -386,7 +399,13 @@ class NVDenseGroup(object):
                              ema_decay, self.kind, MODE_ACCUMULATE, b.dtype, CH_COMM,
                              max_blocks=mb, stream=cs, use_mc=b.mc, slot2=s2, acc_in=acc_in)
         elif self.update == "sharded":
-            if st is None:
+            if st is None and self.layerwise:
+                nvops.dense_step(heap, self._grad_sources(b), self._param_targets(b),
+                                 b.master, s0, s1, b.ema, b.red, self.hp, None, None, b.n,
+                                 avg, ema_decay, self.kind, MODE_REDUCE, b.dtype, CH_COMM,
+                                 max_blocks=mb, stream=cs, use_mc=b.mc, acc_in=acc_in)
+                self._layerwise_update(b, None, cs)
+            elif st is None:
                 nvops.dense_step(heap, self._grad_sources(b), self._param_targets(b),
                                  b.master, s0, s1, b.ema, b.red if acc_in else None,
                                  self.hp, None, None, b.n, avg, ema_decay, self.kind,
@@ -465,7 +484,9 @@ class NVDenseGroup(object):
         W, mb = self.world, self.fabric.dense_blocks
         ema_decay = self.ema_rule.decay if self.ema_rule is not None else 0.0
         for bb in st.buckets:
-            if self.update == "sharded":
+            if self.update == "sharded" and self.layerwise:
+                self._layerwise_update(bb, st.scale, cs)
+            elif self.update == "sharded":
                 t0 = bb.slots[0] if self.nslots > 0 else None
                 t1 = bb.slots[1] if self.nslots > 1 else None
                 t2 = bb.slots[2] if self.nslots > 2 else None
@@ -479,6 +500,25 @@ class NVDenseGroup(object):
                 self._local_update(bb, st.scale, cs)
         for grp, hp in zip(st.groups, hps):
             grp.stage_apply(grp._cur_step, cs, hp=hp)
+
+    def _layerwise_update(self, b, clip, cs):
+        """Passes 2-4 of a layer-wise bucket whose gradient is in `b.red`: the norm pass over
+        this rank's slice, the one-shot all-reduce of the [nseg, 2] sums (bitwise identical
+        on every rank, so a tensor split across owners gets one trust ratio), the update
+        pass with the push of the parameters and the end barrier."""
+        s0 = b.slots[0]
+        s1 = b.slots[1] if self.nslots > 1 else None
+        lw, W = b.lw, self.world
+        nvops.layerwise_norm(b.red, b.master, s0, s1, self.hp, clip, lw, self.kind, b.dtype,
+                             stream=cs)
+        if W > 1:
+            nvops.allreduce_oneshot(self.heap, lw.sums, lw.total, self.fabric.small_stage,
+                                    2 * lw.nseg, torch.float32, 1.0, CH_SMALL, stream=cs)
+        ema_decay = self.ema_rule.decay if self.ema_rule is not None else 0.0
+        nvops.layerwise_update(self.heap, self._param_targets(b), b.red, b.master, s0, s1,
+                               b.ema, self.hp, clip, lw, lw.total if W > 1 else lw.sums, b.n,
+                               ema_decay, self.kind, b.dtype, CH_COMM,
+                               max_blocks=self.fabric.dense_blocks, stream=cs, use_mc=b.mc)
 
     def _finish_clip(self, st, cs):
         rule = self.clip_rules[st.index]
