@@ -33,11 +33,26 @@ ap.add_argument("--num_steps", type=int, default=20)
 ap.add_argument("--vocab_size", type=int, default=793470)
 ap.add_argument("--max_batches", type=int, default=100)
 ap.add_argument("--tiny", action="store_true")
+ap.add_argument("--top_k", type=int, default=0,
+                help="also report accuracy@1 and accuracy@K of the K most likely next words "
+                     "(parallax.nn.full_softmax_topk); this reads the softmax table a second "
+                     "time per batch, after the perplexity's pass")
 FLAGS = ap.parse_args()
 
 
+def topk_hits(top, y, w):
+    """(Σ w where the target is the first prediction, Σ w where it is among all k) of one
+    batch: `top` [B, T, k] predicted ids, `y` [B, T] targets, `w` [B, T] weights."""
+    top = torch.as_tensor(top).cpu()
+    y = torch.as_tensor(np.asarray(y)).to(torch.int64)
+    w = torch.as_tensor(np.asarray(w, dtype=np.float32))
+    eq = top == y[..., None]
+    return float((eq[..., 0].float() * w).sum()), float((eq.any(-1).float() * w).sum())
+
+
 def main():
-    kw = dict(vocab_size=FLAGS.vocab_size, num_steps=FLAGS.num_steps, lazy=True)
+    kw = dict(vocab_size=FLAGS.vocab_size, num_steps=FLAGS.num_steps, lazy=True,
+              eval_top_k=FLAGS.top_k)
     if FLAGS.tiny:
         kw.update(vocab_size=min(FLAGS.vocab_size, 10000), emb_size=32, state_size=64,
                   projected_size=32, num_sampled=64, lazy=False)
@@ -67,18 +82,28 @@ def main():
         ds = Dataset(vocab, os.path.join(FLAGS.datadir, "heldout-monolingual.tokenized.shuffled/*"),
                      deterministic=True)
         batches = ds.iterate_once(FLAGS.batch_size, FLAGS.num_steps)
-    tot, cnt = 0.0, 0.0
+    tot, cnt, hit1, hitk = 0.0, 0.0, 0.0, 0.0
     for i, (x, y, w) in enumerate(batches):
         if i >= FLAGS.max_batches:
             break
-        loss = sess.run("loss", {"x": [x], "y": [y], "w": [w]})[0]
+        feeds = {"x": [x], "y": [y], "w": [w]}
+        if FLAGS.top_k > 0:
+            loss, top = sess.run(["loss", "top_k_ids"], feeds)
+            hit1_, hitk_ = topk_hits(top[0], y, w)
+            hit1 += hit1_
+            hitk += hitk_
+        else:
+            loss = sess.run("loss", feeds)
         n = float(np.sum(w))
-        tot += float(loss) * x.size        # `loss` is the mean over batch×steps of loss·w
+        tot += float(loss[0]) * x.size     # `loss` is the mean over batch×steps of loss·w
         cnt += n
     ppl = math.exp(tot / max(cnt, 1.0))
     parallax.log.info("checkpoint %s (global_step %d): perplexity = %.3f over %d words",
                       path, eng.global_step, ppl, int(cnt))
     print("perplexity %.3f" % ppl)
+    if FLAGS.top_k > 0:
+        print("accuracy@1 %.4f accuracy@%d %.4f" % (hit1 / max(cnt, 1.0), FLAGS.top_k,
+                                                    hitk / max(cnt, 1.0)))
     sess.close()
 
 

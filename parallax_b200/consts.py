@@ -105,6 +105,9 @@ NUM_ITERATIONS_FOR_TEST = 100
 
 # streaming multiprocessors of the target GPU (H100 SXM); grid sizes of the native kernels
 NUM_SMS = 132
+# bound on the per-CTA top-k lists of one fused full-softmax top-k launch (NUM_SMS · rows · k
+# 8-byte entries); larger batches are evaluated in row chunks, each reading the table once
+TOPK_WS_BYTES = 48 << 20
 
 RUN_OPTIONS = ("PS", "MPI", "HYBRID")
 # "AR" is accepted as a modern alias of the reference's "MPI" run option.

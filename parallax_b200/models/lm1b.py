@@ -88,8 +88,11 @@ class LM1B(nn.Module):
 
     def __init__(self, vocab_size=793470, emb_size=512, state_size=2048,
                  projected_size=512, num_sampled=8192, num_steps=20,
-                 num_shards=32, keep_prob=0.9, lazy=False):
+                 num_shards=32, keep_prob=0.9, lazy=False, eval_top_k=0):
+        """`eval_top_k` = k > 0: in eval mode `forward` also returns ``"top_k_ids"``, the k
+        most likely next words of every position (`parallax.nn.full_softmax_topk`)."""
         super().__init__()
+        self.eval_top_k = int(eval_top_k)
         self.vocab_size, self.emb_size = vocab_size, emb_size
         self.state_size, self.projected_size = state_size, projected_size
         self.num_sampled, self.num_steps = num_sampled, num_steps
@@ -148,7 +151,12 @@ class LM1B(nn.Module):
             if row_w is not None:
                 loss = loss * row_w.to(loss.dtype)
             loss = loss.mean()
-        return {"loss": loss, "final_state_c": c.detach(), "final_state_h": h.detach()}
+        out = {"loss": loss, "final_state_c": c.detach(), "final_state_h": h.detach()}
+        if self.eval_top_k > 0 and not self.training:
+            _, ids = pnn.full_softmax_topk(inputs, self.softmax_w, self.softmax_b,
+                                           self.eval_top_k)
+            out["top_k_ids"] = ids.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
+        return out
 
     def prefetch_softmax(self, y):
         """Time-major targets, negative sampling, one fused lookup of (softmax_w, softmax_b)

@@ -146,11 +146,38 @@ def full_softmax_nll(inputs, targets, weight, bias):
                          % (inputs.shape[0], tuple(targets.shape)))
     if targets.dtype.is_floating_point or targets.dtype == torch.bool:
         raise ValueError("targets must be integer ids, got %s" % targets.dtype)
+    _check_full_softmax(inputs, weight, bias)
+    from .parallel.engine import full_softmax_nll as _fs
+    return _fs(inputs, targets, weight, bias)
+
+
+def full_softmax_topk(inputs, weight, bias, k):
+    """The k most likely rows of a partitioned output table for every row of `inputs`:
+    ``(log_probs, ids)``, both ``[N, k]``, where `log_probs` (fp32) is ::
+
+        log_softmax(inputs @ weight.weight.T + bias.weight.T)
+
+    at `ids` (int64 global row ids in [0, V), never a padding row, no duplicates in a row).
+    Within a row the order is logit descending, equal logits by ascending id, so the result
+    does not depend on the partitioning, the world size or the path taken.  `inputs`, `weight`
+    and `bias` are those of `full_softmax_nll`; `k` is an int with 1 <= k <= V.  Under the
+    conditions of `full_softmax_nll`'s fused path and with k <= 32, one fused kernel keeps each
+    row's k best (logit, id) pairs where the rows live (no gathered table, no [N, V] logits);
+    otherwise the table is gathered and the logits materialised, which also carries gradients
+    into `log_probs`."""
+    if inputs.dim() != 2:
+        raise ValueError("inputs must be [N, K], got shape %s" % (tuple(inputs.shape),))
+    _check_full_softmax(inputs, weight, bias)
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= weight.num_embeddings:
+        raise ValueError("k must be an int in [1, %d], got %r" % (weight.num_embeddings, k))
+    from .parallel.engine import full_softmax_topk as _ft
+    return _ft(inputs, weight, bias, k)
+
+
+def _check_full_softmax(inputs, weight, bias):
     if weight.embedding_dim != inputs.shape[1]:
         raise ValueError("weight rows have %d columns, inputs have %d"
                          % (weight.embedding_dim, inputs.shape[1]))
     if bias.embedding_dim != 1 or bias.num_embeddings != weight.num_embeddings:
         raise ValueError("bias must be a [%d, 1] embedding, got [%d, %d]"
                          % (weight.num_embeddings, bias.num_embeddings, bias.embedding_dim))
-    from .parallel.engine import full_softmax_nll as _fs
-    return _fs(inputs, targets, weight, bias)

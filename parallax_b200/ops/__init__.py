@@ -97,6 +97,10 @@ _SIGS = {
                                     c_int, c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
                                     c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p]),
+    "px_full_softmax_topk": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                     c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(GroupGeom),
+                                     c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,
+                                     c_void_p, c_void_p, c_void_p, c_void_p]),
     "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PushTable), c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_int,
                                ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int, c_int,

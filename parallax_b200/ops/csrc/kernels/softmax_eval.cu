@@ -16,6 +16,12 @@
 //                                   subtract the target logit, whose rows come from the group's
 //                                   lookup kernel.
 //
+// Top-k (px_full_softmax_topk): the same GEMM kernel with a list capacity KC > 0 also keeps, per
+// row, the k best (logit, global id) pairs it has seen — logit descending, equal logits by
+// ascending id — in the CTA's slice of a [grid, N, k] workspace, and
+// px_full_softmax_topk_combine_kernel merges the grid's sorted lists and the (max, Σexp) pairs
+// into log-probabilities and int64 ids.
+//
 // One-sided like the lookup: peers' rows are read over NVLink with 16-byte loads; nothing is
 // exchanged, so a rank may evaluate alone.  In sync mode the kernel first waits applied[o] >=
 // completed steps on the group header (the lookup's freshness rule).
@@ -23,12 +29,18 @@
 #include "sparse_group.cuh"
 #include "wgmma.cuh"
 
+#include <type_traits>
+
 namespace tc {
 
 constexpr int EV_BV = 128;          // table rows per work item = wgmma N
 constexpr int EV_STAGES = 4;        // X ring depth (16 KB per stage)
 constexpr int EV_KMAX = 512;
 constexpr float EV_LOG2E = 1.4426950408889634f;
+
+// one top-k list entry; the order key is (v descending, id ascending).  An empty entry is
+// (−inf, INT_MAX), which every real row beats; real logits are never −inf.
+struct __align__(8) TopkEntry { float v; int id; };
 
 struct EvalArgs {
   const __nv_bfloat16* const* w;    // [W] bf16 shadow rows of the weight table on every rank
@@ -43,6 +55,19 @@ struct EvalArgs {
   int W, rank, replicated, owners, slots, rows_per_part, nblk;
   int wait;
 };
+
+// the top-k kernels' arguments (KC > 0); the log-sum-exp kernels take EvalArgs alone
+struct TopkArgs : EvalArgs {
+  TopkEntry* tk;                    // [grid][N][k] per-CTA lists, sorted by the order key
+  const int* part_idx;              // [owners][slots] partition held in each slot (-1: none)
+  GroupGeom g;                      // for the global ids of the partitions' rows
+  int k;
+};
+template <int KC> using EvalParams = typename std::conditional<KC == 0, EvalArgs, TopkArgs>::type;
+
+__device__ __forceinline__ bool tk_beats(float v, int id, float v2, int id2) {
+  return v > v2 || (v == v2 && id < id2);
+}
 
 // (m, s) ⊕ (m2, s2) for s = Σ exp(l − m); s == 0 marks an empty pair (m = −inf)
 __device__ __forceinline__ void lse_merge(float2& c, float m2, float s2) {
@@ -67,10 +92,74 @@ __device__ __forceinline__ float ev_bias(const __nv_bfloat16* row) {
   return __uint_as_float(ld_v4(row).x << 16);
 }
 
-// BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows)
-template <typename BiasT>
+// Top-k epilogue of one row h of the quad's two (all four lanes call it; the row is < N).  A lane
+// holds 32 of the block's BV logits at acc[j·4 + 2h + e], column j·8 + cq + e; s_gid has their
+// global ids.  The list of the CTA is skipped unless the block's row maximum mx can enter it.
+// Otherwise up to k rounds of quad-wide arg-max extract, best first, the block's entries that
+// beat the list's (k − r)-th entry in round r.  The list is copied to shared memory (lbuf) by the
+// four lanes at once, the candidates are staged in cand, and both are merged into the list from
+// its tail, so entries ahead of the first insertion are not rewritten.
+template <int KC>
+__device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, int cq, float mx,
+                                         const int* s_gid, TopkEntry* cand, TopkEntry* lbuf,
+                                         TopkEntry* list, bool first) {
+  const TopkEntry none = {-INFINITY, INT_MAX};
+  const int k = a.k;
+  const unsigned qmask = 0xfu << (threadIdx.x & 28);
+  const bool q0 = (threadIdx.x & 3) == 0;
+  if (!first && (mx == -INFINITY || mx < list[k - 1].v)) return;
+  for (int i = threadIdx.x & 3; i < k; i += 4) lbuf[i] = first ? none : list[i];
+  __syncwarp(qmask);
+  int m = 0;
+  for (; m < k; ++m) {
+    float bv = -INFINITY;
+    int bc = 0, bid = INT_MAX;
+#pragma unroll
+    for (int j = 0; j < EV_BV / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float v = acc[j * 4 + 2 * h + e];
+        const int c = j * 8 + cq + e;
+        if (v > bv || (v == bv && v != -INFINITY && s_gid[c] < bid)) { bv = v; bc = c; bid = s_gid[c]; }
+      }
+    float wv = bv;
+    int wid = bid;
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      const float v2 = __shfl_xor_sync(qmask, wv, o);
+      const int id2 = __shfl_xor_sync(qmask, wid, o);
+      if (tk_beats(v2, id2, wv, wid)) { wv = v2; wid = id2; }
+    }
+    const TopkEntry t = lbuf[k - 1 - m];
+    if (wv == -INFINITY || !tk_beats(wv, wid, t.v, t.id)) break;
+    if (q0) cand[m] = TopkEntry{wv, wid};
+    if (bid == wid && bv == wv) {            // the lane that holds the winner takes it out
+#pragma unroll
+      for (int j = 0; j < EV_BV / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (j * 8 + cq + e == bc) acc[j * 4 + 2 * h + e] = -INFINITY;
+    }
+  }
+  __syncwarp(qmask);
+  if (q0) {
+    // merge from the tail: the worse of (list[i], cand[j]) goes to position o; once every
+    // candidate is placed, list[0 .. i] is already where it belongs
+    int i = k - 1 - m, j = m - 1;
+    for (int o = k - 1; o >= 0 && (j >= 0 || first); --o) {
+      const TopkEntry l = i >= 0 ? lbuf[i] : none;
+      if (j >= 0 && (i < 0 || tk_beats(l.v, l.id, cand[j].v, cand[j].id))) list[o] = cand[j--];
+      else { list[o] = l; --i; }
+    }
+  }
+  __syncwarp(qmask);
+}
+
+// BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows).  KC: top-k list
+// capacity (0: log-sum-exp only; else k <= KC and the top-k epilogue runs)
+template <typename BiasT, int KC>
 __global__ void __launch_bounds__(THREADS, 1)
-px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs a) {
+px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParams<KC> a) {
   constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -79,6 +168,8 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs 
   float* s_bias = reinterpret_cast<float*>(sX + EV_STAGES * X_BYTES);   // [BV], −inf = padding
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + BV);
   uint64_t* empty_bar = full_bar + EV_STAGES;
+  int* s_gid = reinterpret_cast<int*>(empty_bar + EV_STAGES);      // [BV] (KC > 0)
+  TopkEntry* s_cand = reinterpret_cast<TopkEntry*>(s_gid + BV);   // [256 / 4 quads][2][KC]
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
@@ -133,6 +224,15 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs 
       if (ev_row_real(a, cnt, lr))
         bv = ev_bias(reinterpret_cast<const BiasT*>(a.b[owner]) + (size_t)lr * a.b_pitch);
       s_bias[threadIdx.x] = bv;
+      if constexpr (KC > 0) {
+        int gid = INT_MAX;
+        if (bv != -INFINITY) {
+          const int slot = lr / a.rows_per_part;
+          gid = geom_gid(a.g, __ldg(a.part_idx + (a.replicated ? 0 : owner) * a.slots + slot),
+                         lr - slot * a.rows_per_part);
+        }
+        s_gid[threadIdx.x] = gid;
+      }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // st.shared -> wgmma reads
     __syncthreads();
@@ -204,6 +304,12 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalArgs 
             lse_merge(c, mx, sum);
             *p = c;
           }
+          if constexpr (KC > 0) {
+            if (row < a.N)
+              topk_row<KC>(a, acc, h, cq, mx, s_gid, s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC,
+                           s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC + KC,
+                           a.tk + ((size_t)blockIdx.x * a.N + row) * a.k, first);
+          }
         }
       }
     }
@@ -250,11 +356,127 @@ px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, i
   }
 }
 
+// one warp per row: merge the grid's (max, Σexp) pairs, then the grid's sorted top-k lists in k
+// rounds of warp-wide arg-max over the lists' heads (lane l holds the heads of lists l, l + 32,
+// ...), and write log_probs = logit − lse and the ids of the row's k best entries
+constexpr int TK_LISTS_PER_LANE = 8;       // grid <= 256
+
+__global__ void __launch_bounds__(256)
+px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
+                                    const TopkEntry* __restrict__ tk, int grid, int N, int k,
+                                    float* __restrict__ log_probs, long long* __restrict__ ids) {
+  const int lane = threadIdx.x & 31;
+  for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
+    float2 c = make_float2(-INFINITY, 0.f);
+    for (int g = lane; g < grid; g += 32) {
+      const float2 p = ws[(size_t)g * N + row];
+      lse_merge(c, p.x, p.y);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, c.x, o);
+      const float s2 = __shfl_xor_sync(0xffffffffu, c.y, o);
+      lse_merge(c, m2, s2);
+    }
+    const float lse = c.x + logf(c.y);
+    int pos[TK_LISTS_PER_LANE];
+    TopkEntry head[TK_LISTS_PER_LANE];
+#pragma unroll
+    for (int s = 0; s < TK_LISTS_PER_LANE; ++s) {
+      const int g = lane + 32 * s;
+      pos[s] = 0;
+      head[s] = g < grid ? tk[((size_t)g * N + row) * k] : TopkEntry{-INFINITY, INT_MAX};
+    }
+    TopkEntry mine = {-INFINITY, INT_MAX};
+    for (int o = 0; o < k; ++o) {
+      TopkEntry b = {-INFINITY, INT_MAX};
+      int bs = -1;
+#pragma unroll
+      for (int s = 0; s < TK_LISTS_PER_LANE; ++s)
+        if (tk_beats(head[s].v, head[s].id, b.v, b.id)) { b = head[s]; bs = s; }
+      TopkEntry w = b;
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) {
+        const float v2 = __shfl_xor_sync(0xffffffffu, w.v, off);
+        const int id2 = __shfl_xor_sync(0xffffffffu, w.id, off);
+        if (tk_beats(v2, id2, w.v, w.id)) w = TopkEntry{v2, id2};
+      }
+      if (lane == o) mine = w;
+      if (bs >= 0 && b.id == w.id) {
+#pragma unroll
+        for (int s = 0; s < TK_LISTS_PER_LANE; ++s)
+          if (s == bs) {
+            head[s] = ++pos[s] < k ? tk[((size_t)(lane + 32 * s) * N + row) * k + pos[s]]
+                                   : TopkEntry{-INFINITY, INT_MAX};
+          }
+      }
+    }
+    if (lane < k) {
+      log_probs[(size_t)row * k + lane] = mine.v - lse;
+      ids[(size_t)row * k + lane] = mine.id;
+    }
+  }
+}
+
 constexpr int ev_smem_bytes(int kb) {
   return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8;
 }
+// the top-k kernels add the block's global ids, and a candidate list and a copy of the row's list
+// per consumer quad (231 104 bytes at K = 512, KC = 32)
+constexpr int ev_smem_bytes(int kb, int kc) {
+  return ev_smem_bytes(kb) + EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry);
+}
+static_assert(ev_smem_bytes(EV_KMAX / BK, 32) <= 227 * 1024, "top-k shared memory");
 
 }  // namespace tc
+
+namespace {
+
+// EvalArgs and the X tensor map shared by both entry points; returns 0, a negative argument error
+// or a CUDA error code
+int ev_setup(tc::EvalArgs& a, CUtensorMap& tx, int& grid, const void* X, int N, int K,
+             const void* w_ptrs, int w_pitch, const void* b_ptrs, int b_pitch, int b_bf16,
+             const int* row_cnt, int slots, const GroupGeom* g, int rank, const void* hdr_mine,
+             const void* ctl, int wait, void* ws, int ws_ctas) {
+  using namespace tc;
+  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % (b_bf16 ? 8 : 4)) return -1;
+  if (ws_ctas < 1 || slots < 1) return -2;
+  const GroupGeom G = *g;
+  a = EvalArgs{};
+  a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const void* const*)b_ptrs;
+  a.row_cnt = row_cnt;
+  a.applied = reinterpret_cast<const uint32_t*>(hdr_mine) + PX_MAX_RANKS;
+  a.ctl = (const SparseCtl*)ctl; a.ws = (float2*)ws;
+  a.N = N; a.K = K; a.kb = (K + BK - 1) / BK;
+  a.w_pitch = w_pitch; a.b_pitch = b_pitch;
+  a.W = G.W; a.rank = rank; a.replicated = G.replicated; a.owners = G.replicated ? 1 : G.W;
+  a.slots = slots; a.rows_per_part = G.rows_per_part;
+  a.nblk = (slots * G.rows_per_part + EV_BV - 1) / EV_BV;
+  a.wait = wait;
+  const int items = a.owners * a.nblk;
+  grid = items < ws_ctas ? items : ws_ctas;
+  return make_tmap(&tx, X, N, K, BM);
+}
+
+int ev_combine_blocks(int N) {
+  const int blocks = (N + 7) / 8;
+  return blocks > PX_NUM_SMS * 8 ? PX_NUM_SMS * 8 : blocks;
+}
+
+template <typename BiasT, int KC>
+void ev_topk_launch(int grid, const CUtensorMap& tx, const tc::TopkArgs& a, cudaStream_t stream) {
+  using namespace tc;
+  static bool set = false;
+  if (!set) {
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC>,
+                         cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         ev_smem_bytes(EV_KMAX / BK, KC));
+    set = true;
+  }
+  px_full_softmax_lse_kernel<BiasT, KC><<<grid, THREADS, ev_smem_bytes(a.kb, KC), stream>>>(tx, a);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -275,47 +497,70 @@ int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_p
                         const void* wt, const void* bt, float* nll, cudaStream_t stream) {
   using namespace tc;
   if (N <= 0) return 0;
-  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % (b_bf16 ? 8 : 4)) return -1;
-  if (ws_ctas < 1 || slots < 1) return -2;
-  const GroupGeom G = *g;
   EvalArgs a;
-  a.w = (const __nv_bfloat16* const*)w_ptrs; a.b = (const void* const*)b_ptrs;
-  a.row_cnt = row_cnt;
-  a.applied = reinterpret_cast<const uint32_t*>(hdr_mine) + PX_MAX_RANKS;
-  a.ctl = (const SparseCtl*)ctl; a.ws = (float2*)ws;
-  a.N = N; a.K = K; a.kb = (K + BK - 1) / BK;
-  a.w_pitch = w_pitch; a.b_pitch = b_pitch;
-  a.W = G.W; a.rank = rank; a.replicated = G.replicated; a.owners = G.replicated ? 1 : G.W;
-  a.slots = slots; a.rows_per_part = G.rows_per_part;
-  a.nblk = (slots * G.rows_per_part + EV_BV - 1) / EV_BV;
-  a.wait = wait;
-  const int items = a.owners * a.nblk;
-  const int grid = items < ws_ctas ? items : ws_ctas;
   CUtensorMap tx;
-  int rc = make_tmap(&tx, X, N, K, BM);
+  int grid;
+  int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                    slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
   if (rc) return rc;
   constexpr int SMEM_MAX = ev_smem_bytes(EV_KMAX / BK);
   static bool set = false;
   if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<float>,
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<float, 0>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<__nv_bfloat16>,
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<__nv_bfloat16, 0>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
     set = true;
   }
-  int blocks = (N + 7) / 8;
-  if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
+  const int blocks = ev_combine_blocks(N);
   if (b_bf16) {
-    px_full_softmax_lse_kernel<__nv_bfloat16><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
+    px_full_softmax_lse_kernel<__nv_bfloat16, 0><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
     px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
         (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
-        w_pitch, (const __nv_bfloat16*)bt, b_pitch, targets, G.V, nll);
+        w_pitch, (const __nv_bfloat16*)bt, b_pitch, targets, g->V, nll);
   } else {
-    px_full_softmax_lse_kernel<float><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
+    px_full_softmax_lse_kernel<float, 0><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
     px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
         (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
-        w_pitch, (const float*)bt, b_pitch, targets, G.V, nll);
+        w_pitch, (const float*)bt, b_pitch, targets, g->V, nll);
   }
+  return (int)cudaGetLastError();
+}
+
+// The k largest logits of each row of X [N, K] against a (weight, bias) co-lookup group:
+// log_probs fp32 [N, k] (logit − logsumexp of the row) and ids int64 [N, k], logit descending and
+// equal logits by ascending id.  Arguments as px_full_softmax_nll, without targets, plus
+//   part_idx: [owners][slots] partition held in each slot (-1: none; [1][1] = {0} replicated);
+//   k:        1 <= k <= 32; the kernel's list capacity is k rounded up to 8, 16 or 32;
+//   tk:       [ws_ctas][N][k] 8-byte (fp32 logit, int32 id) scratch.  ws_ctas <= 256.
+// Returns 0, a negative argument error (-3: k out of range), or a CUDA error code.
+int px_full_softmax_topk(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                         const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                         const int* part_idx, int slots, const GroupGeom* g, int rank,
+                         const void* hdr_mine, const void* ctl, int wait, void* ws, int ws_ctas,
+                         int k, void* tk, float* log_probs, long long* ids, cudaStream_t stream) {
+  using namespace tc;
+  if (k < 1 || k > 32) return -3;
+  if (N <= 0) return 0;
+  if (ws_ctas > 32 * TK_LISTS_PER_LANE) return -2;
+  TopkArgs a;
+  CUtensorMap tx;
+  int grid;
+  int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                    slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
+  if (rc) return rc;
+  a.tk = (TopkEntry*)tk; a.part_idx = part_idx; a.g = *g; a.k = k;
+  if (b_bf16) {
+    if (k <= 8) ev_topk_launch<__nv_bfloat16, 8>(grid, tx, a, stream);
+    else if (k <= 16) ev_topk_launch<__nv_bfloat16, 16>(grid, tx, a, stream);
+    else ev_topk_launch<__nv_bfloat16, 32>(grid, tx, a, stream);
+  } else {
+    if (k <= 8) ev_topk_launch<float, 8>(grid, tx, a, stream);
+    else if (k <= 16) ev_topk_launch<float, 16>(grid, tx, a, stream);
+    else ev_topk_launch<float, 32>(grid, tx, a, stream);
+  }
+  px_full_softmax_topk_combine_kernel<<<ev_combine_blocks(N), 256, 0, stream>>>(
+      (const float2*)ws, (const TopkEntry*)tk, grid, N, k, log_probs, ids);
   return (int)cudaGetLastError();
 }
 

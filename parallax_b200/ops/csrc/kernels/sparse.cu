@@ -842,9 +842,7 @@ __device__ __forceinline__ void px_store_row4(const OwnerTable& T, size_t row, i
 __device__ __forceinline__ uint32_t owner_gid(const GroupGeom& g, const OwnerTable& T, int r) {
   if (g.replicated) return (uint32_t)r;
   const int slot = r / g.rows_per_part, idx = r - slot * g.rows_per_part;
-  const int p = __ldg(T.slot_part + slot);
-  if (g.strategy == 0) return (uint32_t)(idx * g.P + p);
-  return (uint32_t)(p < g.extras ? p * (g.base + 1) + idx : p * g.base + g.extras + idx);
+  return (uint32_t)geom_gid(g, __ldg(T.slot_part + slot), idx);
 }
 
 __device__ __forceinline__ void px_sgd4(float step, const float4& g, float4& w) {

@@ -16,6 +16,13 @@ struct GroupGeom {
   const int* part_slot;         // [P] index of partition p among its owner's partitions
 };
 
+// the global id of row idx of partition p: the inverse of the (partition, index) split of an id
+// (`geom_part` in sparse.cu); a replicated layout is one "mod" partition, so this is the identity
+__device__ __forceinline__ int geom_gid(const GroupGeom& g, int p, int idx) {
+  if (g.strategy == 0) return idx * g.P + p;
+  return p < g.extras ? p * (g.base + 1) + idx : p * g.base + g.extras + idx;
+}
+
 // per-rank control block of a group (local memory)
 struct SparseCtl {
   uint32_t step;                // completed steps

@@ -123,13 +123,11 @@ def lookup_many(modules, ids, defer=False):
     return PendingLookup(outs) if defer else outs
 
 
-def full_softmax_nll(inputs, targets, weight, bias):
-    """Per-row ``cross_entropy(inputs @ W.T + b, targets, reduction="none")`` over every row
-    of the (weight, bias) embedding modules.  When the modules form a co-lookup group on the
-    NVLink fabric (protocol nvlink) whose weight table keeps a bf16 shadow, `inputs` is bf16
-    with K % 8 == 0 and K <= 512, and no gradient is wanted, the group's fused kernel computes
-    it where the rows live; everything else runs the gather + matmul + cross_entropy
-    composition (which also gives the tables their gradients in training)."""
+def _fused_eval_group(inputs, weight, bias):
+    """The co-lookup group whose fused full-softmax kernels can evaluate `inputs` against the
+    (weight, bias) embedding modules, else None: the modules form a group on the NVLink fabric
+    (protocol nvlink) whose weight table keeps a bf16 shadow, `inputs` is bf16 on the group's
+    device with K % 8 == 0 and K <= 512, and no gradient is wanted."""
     tabs = [getattr(m, "table", None) for m in (weight, bias)]
     grp = getattr(tabs[0], "group", None) if tabs[0] is not None else None
     K = int(inputs.shape[-1])
@@ -139,8 +137,33 @@ def full_softmax_nll(inputs, targets, weight, bias):
             (not torch.is_grad_enabled() or not (inputs.requires_grad or
                                                  weight._anchor.requires_grad or
                                                  bias._anchor.requires_grad)):
+        return grp
+    return None
+
+
+def full_softmax_nll(inputs, targets, weight, bias):
+    """Per-row ``cross_entropy(inputs @ W.T + b, targets, reduction="none")`` over every row
+    of the (weight, bias) embedding modules.  Where `_fused_eval_group` finds a group, its
+    fused kernel computes it where the rows live; everything else runs the gather + matmul +
+    cross_entropy composition (which also gives the tables their gradients in training)."""
+    grp = _fused_eval_group(inputs, weight, bias)
+    if grp is not None:
         return grp.full_softmax_nll(inputs, targets)
     return full_softmax_composition(inputs, targets, weight, bias)
+
+
+# largest k of the fused top-k kernel (its per-row list capacity)
+FUSED_TOPK_MAX = 32
+
+
+def full_softmax_topk(inputs, weight, bias, k):
+    """``(log_probs [N, k], ids [N, k])`` of the k largest full-softmax logits of each row,
+    logit descending and equal logits by ascending id.  Fused where `_fused_eval_group` finds a
+    group and k <= 32; everything else (and training) runs `full_softmax_topk_composition`."""
+    grp = _fused_eval_group(inputs, weight, bias)
+    if grp is not None and k <= FUSED_TOPK_MAX:
+        return grp.full_softmax_topk(inputs, k)
+    return full_softmax_topk_composition(inputs, weight, bias, k)
 
 
 def full_softmax_composition(inputs, targets, weight, bias):
@@ -150,6 +173,31 @@ def full_softmax_composition(inputs, targets, weight, bias):
     w, b = w.to(inputs.dtype), b.squeeze(-1).float()
     logits = (inputs @ w.t()).float() + b
     return torch.nn.functional.cross_entropy(logits, targets, reduction="none")
+
+
+def full_softmax_topk_composition(inputs, weight, bias, k):
+    """The unfused top-k: gather every row, materialise the [N, V] logits, `log_softmax`, then
+    the k best of each row by (logit descending, id ascending).  `torch.topk` leaves the order
+    of equal values open, so it only finds each row's k-th value; the rows' candidates at or
+    above it are then sorted stably (ascending id within equal values).  Gradients flow into
+    `log_probs`."""
+    ids = torch.arange(weight.num_embeddings, device=inputs.device)
+    w, b = lookup_many([weight, bias], ids)
+    w, b = w.to(inputs.dtype), b.squeeze(-1).float()
+    lp = torch.log_softmax((inputs @ w.t()).float() + b, dim=-1)
+    n = lp.shape[0]
+    with torch.no_grad():
+        kth = torch.topk(lp, k, dim=1).values[:, -1:]
+        r, c = (lp >= kth).nonzero(as_tuple=True)   # row-major: ids ascend within a row
+        o = torch.sort(lp[r, c], descending=True, stable=True).indices
+        o = o[torch.sort(r[o], stable=True).indices]
+        r, c = r[o], c[o]
+        cnt = torch.bincount(r, minlength=n)
+        rank = torch.arange(r.numel(), device=r.device) - (torch.cumsum(cnt, 0) - cnt)[r]
+        keep = rank < k
+        top = torch.empty(n, k, dtype=torch.int64, device=lp.device)
+        top[r[keep], rank[keep]] = c[keep]
+    return lp.gather(1, top), top
 
 
 class ShardedEmbedding(tnn.Module):

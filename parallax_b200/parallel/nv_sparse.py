@@ -437,6 +437,7 @@ class NVSparseGroup(object):
         self._done_step = -1
         self._last_n = 1
         self._row_cnt = None
+        self._part_idx = None
         # ClipByGlobalNorm(include_sparse=True): (dense group, clip state) of the rule this
         # group contributes to, and the group's private hyper-parameters for the clipped apply
         self.joint_clip = None
@@ -567,6 +568,30 @@ class NVSparseGroup(object):
             self._row_cnt = (lay, cnt.to(self.device))
         return self._row_cnt[1]
 
+    def _part_index(self):
+        """int32 [owners, slots] on the device: the partition held in each (owner, slot) of the
+        layout (-1: none), from which the top-k kernel recovers global row ids.  A replicated
+        layout is one partition: [[0]].  Built once per layout."""
+        lay = self.layout
+        if self._part_idx is None or self._part_idx[0] is not lay:
+            part = torch.full((1 if lay.replicated else lay.world, lay.parts_per_owner), -1,
+                              dtype=torch.int32)
+            for p in range(lay.P):
+                part[0 if lay.replicated else lay.owners[p], lay.slots[p]] = p
+            self._part_idx = (lay, part.to(self.device))
+        return self._part_idx[1]
+
+    def _check_eval_inputs(self, x, what):
+        tw, tb = self.tables
+        if not tw.use_shadow or tb.D != 1 or x.dim() != 2 or x.shape[1] != tw.D or \
+                x.dtype != torch.bfloat16:
+            raise ValueError("%s needs bf16 inputs [N, %d], a weight table with a bf16 shadow "
+                             "and a bias table of width 1" % (what, tw.D))
+        x = x.contiguous()
+        if x.data_ptr() % 16:                      # TMA needs a 16-byte aligned base
+            x = x.clone()
+        return x
+
     def full_softmax_nll(self, x, targets):
         """Per-row full-softmax NLL, fp32 [N], of bf16 inputs `x` [N, K] against this
         group's (weight, bias) tables: ``cross_entropy(x @ W.T + b, targets)`` with fp32
@@ -577,15 +602,10 @@ class NVSparseGroup(object):
         L = ops.lib()
         tw, tb = self.tables
         n, K = int(x.shape[0]), int(x.shape[1])
-        if not tw.use_shadow or tb.D != 1 or K != tw.D or x.dtype != torch.bfloat16:
-            raise ValueError("full_softmax_nll needs bf16 inputs [N, %d], a weight table with "
-                             "a bf16 shadow and a bias table of width 1" % tw.D)
+        x = self._check_eval_inputs(x, "full_softmax_nll")
         out = torch.empty(n, dtype=torch.float32, device=self.device)
         if n == 0:
             return out
-        x = x.contiguous()
-        if x.data_ptr() % 16:                      # TMA needs a 16-byte aligned base
-            x = x.clone()
         ids = targets.reshape(-1).to(self.device, torch.int64).contiguous()
         wait = self._wait
         stream = _sp(torch.cuda.current_stream(self.device))
@@ -613,6 +633,46 @@ class NVSparseGroup(object):
             consts.NUM_SMS, _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
             _vp(out.data_ptr()), stream), "full_softmax_nll")
         return out
+
+    def full_softmax_topk(self, x, k):
+        """The k largest full-softmax logits of each row of bf16 inputs `x` [N, K] against
+        this group's (weight, bias) tables: ``(log_probs fp32 [N, k], ids int64 [N, k])``, logit
+        descending and equal logits by ascending id, with fp32 logits computed from the rows
+        where their owners store them (`ops/csrc/kernels/softmax_eval.cu`).  1 <= k <= 32.
+        Scratch is per call and O(NUM_SMS · rows · k): rows are taken in chunks so that the
+        per-CTA lists fit in `consts.TOPK_WS_BYTES`.  One-sided: no other rank takes part."""
+        L = ops.lib()
+        tw, tb = self.tables
+        n, K = int(x.shape[0]), int(x.shape[1])
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, tw.V):
+            raise ValueError("full_softmax_topk: k must be an int in [1, %d], got %r"
+                             % (min(32, tw.V), k))
+        x = self._check_eval_inputs(x, "full_softmax_topk")
+        log_probs = torch.empty(n, k, dtype=torch.float32, device=self.device)
+        ids = torch.empty(n, k, dtype=torch.int64, device=self.device)
+        if n == 0:
+            return log_probs, ids
+        b_bf16 = tb.weight_dtype == torch.bfloat16
+        b_src, b_pitch = ("shadow", tb.Dps) if b_bf16 else ("table", tb.Dp)
+        cnt, part = self._row_counts(), self._part_index()
+        ctas = consts.NUM_SMS
+        chunk = max(128, consts.TOPK_WS_BYTES // (ctas * k * 8) // 128 * 128)
+        chunk = min(chunk, n)
+        ws = torch.empty(ctas * chunk * 2, dtype=torch.float32, device=self.device)
+        tk = torch.empty(ctas * chunk * k * 2, dtype=torch.int32, device=self.device)
+        stream = _sp(torch.cuda.current_stream(self.device))
+        for r0 in range(0, n, chunk):
+            m = min(chunk, n - r0)
+            _count(2)
+            ops.check(L.px_full_softmax_topk(
+                _vp(x[r0:].data_ptr()), m, K, _vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps,
+                _vp(tb.dev_ptrs(b_src).data_ptr()), b_pitch, int(b_bf16), _vp(cnt.data_ptr()),
+                _vp(part.data_ptr()), int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
+                _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), self._wait,
+                _vp(ws.data_ptr()), ctas, k, _vp(tk.data_ptr()),
+                _vp(log_probs[r0:].data_ptr()), _vp(ids[r0:].data_ptr()), stream),
+                "full_softmax_topk")
+        return log_probs, ids
 
     def add_pending(self, token, grads):
         gs = []
