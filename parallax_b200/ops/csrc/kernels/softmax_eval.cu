@@ -317,6 +317,24 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
   }
 }
 
+// one warp's merge of a row's (max, Σexp) pairs over the grid's ws entries: lane l merges
+// entries l, l + 32, ..., then the lanes merge by xor shuffles; every lane returns the result
+__device__ __forceinline__ float2 ev_grid_lse(const float2* __restrict__ ws, int grid, int N,
+                                             int row, int lane) {
+  float2 c = make_float2(-INFINITY, 0.f);
+  for (int g = lane; g < grid; g += 32) {
+    const float2 p = ws[(size_t)g * N + row];
+    lse_merge(c, p.x, p.y);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, c.x, o);
+    const float s2 = __shfl_xor_sync(0xffffffffu, c.y, o);
+    lse_merge(c, m2, s2);
+  }
+  return c;
+}
+
 template <typename BiasT>
 __global__ void __launch_bounds__(256)
 px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, int K,
@@ -327,17 +345,7 @@ px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, i
                                float* __restrict__ nll) {
   const int lane = threadIdx.x & 31;
   for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
-    float2 c = make_float2(-INFINITY, 0.f);
-    for (int g = lane; g < grid; g += 32) {
-      const float2 p = ws[(size_t)g * N + row];
-      lse_merge(c, p.x, p.y);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float m2 = __shfl_xor_sync(0xffffffffu, c.x, o);
-      const float s2 = __shfl_xor_sync(0xffffffffu, c.y, o);
-      lse_merge(c, m2, s2);
-    }
+    const float2 c = ev_grid_lse(ws, grid, N, row, lane);
     float d = 0.f;
     for (int ch = lane; ch < K / 8; ch += 32) {
       float xf[8], wf[8];
@@ -367,17 +375,7 @@ px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
                                     float* __restrict__ log_probs, long long* __restrict__ ids) {
   const int lane = threadIdx.x & 31;
   for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
-    float2 c = make_float2(-INFINITY, 0.f);
-    for (int g = lane; g < grid; g += 32) {
-      const float2 p = ws[(size_t)g * N + row];
-      lse_merge(c, p.x, p.y);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float m2 = __shfl_xor_sync(0xffffffffu, c.x, o);
-      const float s2 = __shfl_xor_sync(0xffffffffu, c.y, o);
-      lse_merge(c, m2, s2);
-    }
+    const float2 c = ev_grid_lse(ws, grid, N, row, lane);
     const float lse = c.x + logf(c.y);
     int pos[TK_LISTS_PER_LANE];
     TopkEntry head[TK_LISTS_PER_LANE];
@@ -418,14 +416,14 @@ px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
   }
 }
 
-constexpr int ev_smem_bytes(int kb) {
-  return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8;
-}
-// the top-k kernels add the block's global ids, and a candidate list and a copy of the row's list
-// per consumer quad (231 104 bytes at K = 512, KC = 32)
+// dynamic shared memory of px_full_softmax_lse_kernel<·, kc> at kb K-blocks: alignment slack,
+// table block, X ring, bias and barriers; the top-k kernels (kc > 0) add the block's global ids,
+// and a candidate list and a copy of the row's list per consumer quad
 constexpr int ev_smem_bytes(int kb, int kc) {
-  return ev_smem_bytes(kb) + EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry);
+  return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8 +
+         (kc > 0 ? EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0);
 }
+static_assert(ev_smem_bytes(EV_KMAX / BK, 0) == 198208, "log-sum-exp shared memory at K = 512");
 static_assert(ev_smem_bytes(EV_KMAX / BK, 32) <= 227 * 1024, "top-k shared memory");
 
 }  // namespace tc
@@ -464,7 +462,7 @@ int ev_combine_blocks(int N) {
 }
 
 template <typename BiasT, int KC>
-void ev_topk_launch(int grid, const CUtensorMap& tx, const tc::TopkArgs& a, cudaStream_t stream) {
+void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC>& a, cudaStream_t stream) {
   using namespace tc;
   static bool set = false;
   if (!set) {
@@ -474,6 +472,24 @@ void ev_topk_launch(int grid, const CUtensorMap& tx, const tc::TopkArgs& a, cuda
     set = true;
   }
   px_full_softmax_lse_kernel<BiasT, KC><<<grid, THREADS, ev_smem_bytes(a.kb, KC), stream>>>(tx, a);
+}
+
+template <typename BiasT>
+void ev_nll(int grid, const CUtensorMap& tx, const tc::EvalArgs& a, const void* X,
+            const long long* targets, const void* wt, const void* bt, int V, float* nll,
+            cudaStream_t stream) {
+  ev_launch<BiasT, 0>(grid, tx, a, stream);
+  tc::px_full_softmax_combine_kernel<<<ev_combine_blocks(a.N), 256, 0, stream>>>(
+      a.ws, grid, a.N, a.K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt, a.w_pitch,
+      (const BiasT*)bt, a.b_pitch, targets, V, nll);
+}
+
+// the list capacity is k rounded up to 8, 16 or 32
+template <typename BiasT>
+void ev_topk(int grid, const CUtensorMap& tx, const tc::TopkArgs& a, cudaStream_t stream) {
+  if (a.k <= 8) ev_launch<BiasT, 8>(grid, tx, a, stream);
+  else if (a.k <= 16) ev_launch<BiasT, 16>(grid, tx, a, stream);
+  else ev_launch<BiasT, 32>(grid, tx, a, stream);
 }
 
 }  // namespace
@@ -503,27 +519,8 @@ int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_p
   int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
                     slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
   if (rc) return rc;
-  constexpr int SMEM_MAX = ev_smem_bytes(EV_KMAX / BK);
-  static bool set = false;
-  if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<float, 0>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<__nv_bfloat16, 0>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
-    set = true;
-  }
-  const int blocks = ev_combine_blocks(N);
-  if (b_bf16) {
-    px_full_softmax_lse_kernel<__nv_bfloat16, 0><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
-    px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
-        (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
-        w_pitch, (const __nv_bfloat16*)bt, b_pitch, targets, g->V, nll);
-  } else {
-    px_full_softmax_lse_kernel<float, 0><<<grid, THREADS, ev_smem_bytes(a.kb), stream>>>(tx, a);
-    px_full_softmax_combine_kernel<<<blocks, 256, 0, stream>>>(
-        (const float2*)ws, grid, N, K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt,
-        w_pitch, (const float*)bt, b_pitch, targets, g->V, nll);
-  }
+  (b_bf16 ? ev_nll<__nv_bfloat16> : ev_nll<float>)(grid, tx, a, X, targets, wt, bt, g->V, nll,
+                                                   stream);
   return (int)cudaGetLastError();
 }
 
@@ -550,15 +547,7 @@ int px_full_softmax_topk(const void* X, int N, int K, const void* w_ptrs, int w_
                     slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
   if (rc) return rc;
   a.tk = (TopkEntry*)tk; a.part_idx = part_idx; a.g = *g; a.k = k;
-  if (b_bf16) {
-    if (k <= 8) ev_topk_launch<__nv_bfloat16, 8>(grid, tx, a, stream);
-    else if (k <= 16) ev_topk_launch<__nv_bfloat16, 16>(grid, tx, a, stream);
-    else ev_topk_launch<__nv_bfloat16, 32>(grid, tx, a, stream);
-  } else {
-    if (k <= 8) ev_topk_launch<float, 8>(grid, tx, a, stream);
-    else if (k <= 16) ev_topk_launch<float, 16>(grid, tx, a, stream);
-    else ev_topk_launch<float, 32>(grid, tx, a, stream);
-  }
+  (b_bf16 ? ev_topk<__nv_bfloat16> : ev_topk<float>)(grid, tx, a, stream);
   px_full_softmax_topk_combine_kernel<<<ev_combine_blocks(N), 256, 0, stream>>>(
       (const float2*)ws, (const TopkEntry*)tk, grid, N, k, log_probs, ids);
   return (int)cudaGetLastError();

@@ -166,12 +166,17 @@ def full_softmax_topk(inputs, weight, bias, k):
     return full_softmax_topk_composition(inputs, weight, bias, k)
 
 
-def full_softmax_composition(inputs, targets, weight, bias):
-    """The unfused full softmax: gather every row, materialise the [N, V] logits."""
+def _gathered_logits(inputs, weight, bias):
+    """fp32 [N, V] logits of the unfused compositions, from every row of the tables gathered."""
     ids = torch.arange(weight.num_embeddings, device=inputs.device)
     w, b = lookup_many([weight, bias], ids)
     w, b = w.to(inputs.dtype), b.squeeze(-1).float()
-    logits = (inputs @ w.t()).float() + b
+    return (inputs @ w.t()).float() + b
+
+
+def full_softmax_composition(inputs, targets, weight, bias):
+    """The unfused full softmax: gather every row, materialise the [N, V] logits."""
+    logits = _gathered_logits(inputs, weight, bias)
     return torch.nn.functional.cross_entropy(logits, targets, reduction="none")
 
 
@@ -181,10 +186,7 @@ def full_softmax_topk_composition(inputs, weight, bias, k):
     of equal values open, so it only finds each row's k-th value; the rows' candidates at or
     above it are then sorted stably (ascending id within equal values).  Gradients flow into
     `log_probs`."""
-    ids = torch.arange(weight.num_embeddings, device=inputs.device)
-    w, b = lookup_many([weight, bias], ids)
-    w, b = w.to(inputs.dtype), b.squeeze(-1).float()
-    lp = torch.log_softmax((inputs @ w.t()).float() + b, dim=-1)
+    lp = torch.log_softmax(_gathered_logits(inputs, weight, bias), dim=-1)
     n = lp.shape[0]
     with torch.no_grad():
         kth = torch.topk(lp, k, dim=1).values[:, -1:]

@@ -436,8 +436,7 @@ class NVSparseGroup(object):
         self._cur_step = 0
         self._done_step = -1
         self._last_n = 1
-        self._row_cnt = None
-        self._part_idx = None
+        self._slots = None
         # ClipByGlobalNorm(include_sparse=True): (dense group, clip state) of the rule this
         # group contributes to, and the group's private hyper-parameters for the clipped apply
         self.joint_clip = None
@@ -556,32 +555,30 @@ class NVSparseGroup(object):
         return outs, pend
 
     # ------------------------------------------------------------- evaluation
-    def _row_counts(self):
-        """int32 [owners, slots] on the device: real rows of the partition held in each
-        (owner, slot) of the layout (the rest of a slot is padding).  Built once per layout."""
+    def _slot_maps(self):
+        """(row counts, partition index), int32 [owners, slots] on the device, built once per
+        layout: the real rows of the partition held in each (owner, slot) of the layout (the
+        rest of a slot is padding), and that partition (-1: none), from which the top-k kernel
+        recovers global row ids.  A replicated layout is one partition: owners = 1, [[0]]."""
         lay = self.layout
-        if self._row_cnt is None or self._row_cnt[0] is not lay:
-            cnt = torch.zeros(1 if lay.replicated else lay.world, lay.parts_per_owner,
-                              dtype=torch.int32)
+        if self._slots is None or self._slots[0] is not lay:
+            shape = (1 if lay.replicated else lay.world, lay.parts_per_owner)
+            cnt = torch.zeros(shape, dtype=torch.int32)
+            part = torch.full(shape, -1, dtype=torch.int32)
             for p in range(lay.P):
-                cnt[0 if lay.replicated else lay.owners[p], lay.slots[p]] = lay.partition_rows(p)
-            self._row_cnt = (lay, cnt.to(self.device))
-        return self._row_cnt[1]
+                o = 0 if lay.replicated else lay.owners[p]
+                cnt[o, lay.slots[p]] = lay.partition_rows(p)
+                part[o, lay.slots[p]] = p
+            self._slots = (lay, cnt.to(self.device), part.to(self.device))
+        return self._slots[1:]
 
-    def _part_index(self):
-        """int32 [owners, slots] on the device: the partition held in each (owner, slot) of the
-        layout (-1: none), from which the top-k kernel recovers global row ids.  A replicated
-        layout is one partition: [[0]].  Built once per layout."""
-        lay = self.layout
-        if self._part_idx is None or self._part_idx[0] is not lay:
-            part = torch.full((1 if lay.replicated else lay.world, lay.parts_per_owner), -1,
-                              dtype=torch.int32)
-            for p in range(lay.P):
-                part[0 if lay.replicated else lay.owners[p], lay.slots[p]] = p
-            self._part_idx = (lay, part.to(self.device))
-        return self._part_idx[1]
-
-    def _check_eval_inputs(self, x, what):
+    def _eval_operands(self, x, what):
+        """Checks the inputs of the eval entry point `what` and returns what px_full_softmax_nll
+        and px_full_softmax_topk share: (x, K, (bias source, bias pitch), head, tail, stream).
+        head is their ctypes arguments from the weight shadow pointers through the row counts,
+        tail those from the slot count through `wait`; the top-k kernel takes its partition
+        index between the two.  The bias rows are the master rows: fp32, or bf16 rows of the
+        shadow's layout with bf16 masters (widened where they are added)."""
         tw, tb = self.tables
         if not tw.use_shadow or tb.D != 1 or x.dim() != 2 or x.shape[1] != tw.D or \
                 x.dtype != torch.bfloat16:
@@ -590,7 +587,15 @@ class NVSparseGroup(object):
         x = x.contiguous()
         if x.data_ptr() % 16:                      # TMA needs a 16-byte aligned base
             x = x.clone()
-        return x
+        b_bf16 = tb.weight_dtype == torch.bfloat16
+        b_src, b_pitch = ("shadow", tb.Dps) if b_bf16 else ("table", tb.Dp)
+        cnt, _ = self._slot_maps()
+        head = (_vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps, _vp(tb.dev_ptrs(b_src).data_ptr()),
+                b_pitch, int(b_bf16), _vp(cnt.data_ptr()))
+        tail = (int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
+                _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), self._wait)
+        return (x, int(x.shape[1]), (b_src, b_pitch), head, tail,
+                _sp(torch.cuda.current_stream(self.device)))
 
     def full_softmax_nll(self, x, targets):
         """Per-row full-softmax NLL, fp32 [N], of bf16 inputs `x` [N, K] against this
@@ -601,36 +606,27 @@ class NVSparseGroup(object):
         NaN in its row.  One-sided: no other rank takes part."""
         L = ops.lib()
         tw, tb = self.tables
-        n, K = int(x.shape[0]), int(x.shape[1])
-        x = self._check_eval_inputs(x, "full_softmax_nll")
+        x, K, (b_src, b_pitch), head, tail, stream = self._eval_operands(x, "full_softmax_nll")
+        n = int(x.shape[0])
         out = torch.empty(n, dtype=torch.float32, device=self.device)
         if n == 0:
             return out
         ids = targets.reshape(-1).to(self.device, torch.int64).contiguous()
-        wait = self._wait
-        stream = _sp(torch.cuda.current_stream(self.device))
+        # target bias from the master rows like every bias row the eval kernel reads
         w_t = torch.empty((n, tw.Dps), dtype=torch.bfloat16, device=self.device)
-        # target bias from the master rows like every bias row the eval kernel reads: fp32, or
-        # bf16 rows of the shadow's layout with bf16 masters (widened where they are added)
-        b_bf16 = tb.weight_dtype == torch.bfloat16
-        b_src, b_pitch = ("shadow", tb.Dps) if b_bf16 else ("table", tb.Dp)
         b_t = torch.empty((n, b_pitch), dtype=tb.weight_dtype, device=self.device)
         descs = (ops.LookupTable * 2)(_lookup_table(tw, "shadow", w_t),
                                       _lookup_table(tb, b_src, b_t))
         _count()
         ops.check(L.px_sparse_lookup(
             _vp(ids.data_ptr()), 1, n, descs, 2, _vp(0), ctypes.byref(self.geom),
-            _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), wait, stream),
+            _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), self._wait, stream),
             "sparse_lookup(full softmax targets)")
-        cnt = self._row_counts()
         ws = torch.empty(consts.NUM_SMS * n * 2, dtype=torch.float32, device=self.device)
         _count(2)
         ops.check(L.px_full_softmax_nll(
-            _vp(x.data_ptr()), n, K, _vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps,
-            _vp(tb.dev_ptrs(b_src).data_ptr()), b_pitch, int(b_bf16), _vp(cnt.data_ptr()),
-            int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
-            _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), wait, _vp(ws.data_ptr()),
-            consts.NUM_SMS, _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
+            _vp(x.data_ptr()), n, K, *head, *tail, _vp(ws.data_ptr()), consts.NUM_SMS,
+            _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
             _vp(out.data_ptr()), stream), "full_softmax_nll")
         return out
 
@@ -642,33 +638,27 @@ class NVSparseGroup(object):
         Scratch is per call and O(NUM_SMS · rows · k): rows are taken in chunks so that the
         per-CTA lists fit in `consts.TOPK_WS_BYTES`.  One-sided: no other rank takes part."""
         L = ops.lib()
-        tw, tb = self.tables
-        n, K = int(x.shape[0]), int(x.shape[1])
-        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, tw.V):
+        V = self.tables[0].V
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, V):
             raise ValueError("full_softmax_topk: k must be an int in [1, %d], got %r"
-                             % (min(32, tw.V), k))
-        x = self._check_eval_inputs(x, "full_softmax_topk")
+                             % (min(32, V), k))
+        x, K, _, head, tail, stream = self._eval_operands(x, "full_softmax_topk")
+        n = int(x.shape[0])
         log_probs = torch.empty(n, k, dtype=torch.float32, device=self.device)
         ids = torch.empty(n, k, dtype=torch.int64, device=self.device)
         if n == 0:
             return log_probs, ids
-        b_bf16 = tb.weight_dtype == torch.bfloat16
-        b_src, b_pitch = ("shadow", tb.Dps) if b_bf16 else ("table", tb.Dp)
-        cnt, part = self._row_counts(), self._part_index()
+        _, part = self._slot_maps()
         ctas = consts.NUM_SMS
         chunk = max(128, consts.TOPK_WS_BYTES // (ctas * k * 8) // 128 * 128)
         chunk = min(chunk, n)
         ws = torch.empty(ctas * chunk * 2, dtype=torch.float32, device=self.device)
         tk = torch.empty(ctas * chunk * k * 2, dtype=torch.int32, device=self.device)
-        stream = _sp(torch.cuda.current_stream(self.device))
         for r0 in range(0, n, chunk):
             m = min(chunk, n - r0)
             _count(2)
             ops.check(L.px_full_softmax_topk(
-                _vp(x[r0:].data_ptr()), m, K, _vp(tw.dev_ptrs("shadow").data_ptr()), tw.Dps,
-                _vp(tb.dev_ptrs(b_src).data_ptr()), b_pitch, int(b_bf16), _vp(cnt.data_ptr()),
-                _vp(part.data_ptr()), int(cnt.shape[1]), ctypes.byref(self.geom), self.rank,
-                _vp(self.hdr_buf.local_ptr), _vp(self.ctl.data_ptr()), self._wait,
+                _vp(x[r0:].data_ptr()), m, K, *head, _vp(part.data_ptr()), *tail,
                 _vp(ws.data_ptr()), ctas, k, _vp(tk.data_ptr()),
                 _vp(log_probs[r0:].data_ptr()), _vp(ids[r0:].data_ptr()), stream),
                 "full_softmax_topk")

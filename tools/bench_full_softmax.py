@@ -1,14 +1,22 @@
-"""Full-softmax evaluation of the LM1B output layer: the gather + matmul + cross_entropy
-composition against the fused kernel (`parallax.nn.full_softmax_nll`), in one process.
+"""Full-softmax evaluation of the LM1B output layer, in one process: the NLL's gather + matmul +
+cross_entropy composition against the fused kernel (`parallax.nn.full_softmax_nll`), and top-k
+next-word prediction's gather + matmul + log_softmax + top-k composition against the fused top-k
+kernel (`parallax.nn.full_softmax_topk`), next to the fused NLL at the same N.
 
-    python tools/bench_full_softmax.py [--n 640 2560] [--iters 10] [--out result.json]
+    python tools/bench_full_softmax.py [--n 640 2560] [--k 1 10 32] [--out result.json]
 
-Builds LM1B's (softmax_w, softmax_b) co-lookup group through the engine on the NVLink
-fabric, one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N the two
-arms alternate; per arm it reports ms per call (CUDA events, after warm-up), the growth of
-`torch.cuda.max_memory_allocated` during one call, the achieved TFLOP/s from 2·N·V·K, and
-the largest |Δ| between the arms' NLL (the composition rounds logits to bf16).  The card
-name, power limit and max SM clock are read in the same run.
+Builds LM1B's (softmax_w, softmax_b) co-lookup group through the engine on the NVLink fabric,
+one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N:
+- NLL: the composition and the fused kernel alternate over --rounds rounds of --iters calls
+  (median).  The records carry the largest |Δ| between the arms' NLL (the composition rounds
+  logits to bf16).
+- top-k, for each k of --k (an empty list times the NLL only): the fused top-k and the fused NLL
+  alternate over the rounds, and the composition is timed after them in each round over
+  --comp_iters calls.  The fused ids are compared with the composition's where its consecutive
+  log-probabilities, the (k+1)-th included, differ by > 2e-2.
+Per arm: ms per call (CUDA events, after warm-up), the growth of `torch.cuda.max_memory_allocated`
+during one call, and the achieved TFLOP/s from 2·N·V·K.  The card name, power limit and max SM
+clock are read in the same run.
 """
 import argparse
 import json
@@ -22,7 +30,8 @@ import torch  # noqa: E402
 
 import parallax_b200 as parallax  # noqa: E402
 from parallax_b200.models.lm1b import LM1B, lm1b_graph  # noqa: E402
-from parallax_b200.parallel.engine import full_softmax_composition  # noqa: E402
+from parallax_b200.parallel.engine import (full_softmax_composition,  # noqa: E402
+                                           full_softmax_topk_composition)
 
 
 def card():
@@ -53,10 +62,23 @@ def timed(fn, iters):
     return e0.elapsed_time(e1) / iters, growth
 
 
+def alternate(arms, rounds):
+    """{name: (ms per call of each round, allocation growth)} of arms [(name, fn, iters)],
+    timed in turn in every round."""
+    ms, mem = {name: [] for name, _, _ in arms}, {}
+    for _ in range(rounds):
+        for name, fn, iters in arms:
+            t_ms, mem[name] = timed(fn, iters)
+            ms[name].append(t_ms)
+    return {name: (ms[name], mem[name]) for name in ms}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, nargs="+", default=[640, 2560])
+    ap.add_argument("--k", type=int, nargs="*", default=[1, 10, 32])
     ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--comp_iters", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -74,37 +96,53 @@ def main():
     w, b = m.softmax_w, m.softmax_b
     assert w.table.group is b.table.group and w.table.use_shadow
     V, K = w.num_embeddings, w.embedding_dim
-    arms = {
-        "composition": lambda x, t: full_softmax_composition(x, t, w, b),
-        "fused": lambda x, t: parallax.nn.full_softmax_nll(x, t, w, b),
-    }
     results = []
+
+    def report(arm, n, timing, k=None, extra=None):
+        ms, grow = timing
+        med = statistics.median(ms)
+        r = {"arm": arm, "N": n, **({} if k is None else {"k": k}), "V": V, "K": K,
+             "ms": round(med, 3), "ms_all": [round(v, 3) for v in ms],
+             "mem_growth_MB": round(grow / 2 ** 20, 1),
+             "tflops": round(2.0 * n * V * K / (med * 1e-3) / 1e12, 1), **(extra or {}),
+             "card": info}
+        results.append(r)
+        print(json.dumps(r), flush=True)
+        return med
+
     with torch.no_grad():
         for n in a.n:
             g = torch.Generator(device="cuda").manual_seed(n)
             x = (torch.randn(n, K, device="cuda", generator=g) * 0.5).bfloat16()
             t = torch.randint(0, V, (n,), device="cuda", generator=g)
-            outs = {k: f(x, t) for k, f in arms.items()}             # warm-up + values
-            for k, f in arms.items():
-                f(x, t)
-            diff = float((outs["fused"] - outs["composition"]).abs().max())
-            del outs
-            ms = {k: [] for k in arms}
-            mem = {}
-            for _ in range(a.rounds):                                # arms alternate
-                for k, f in arms.items():
-                    t_ms, grow = timed(lambda: f(x, t), a.iters)
-                    ms[k].append(t_ms)
-                    mem[k] = grow
-            for k in arms:
-                med = statistics.median(ms[k])
-                r = {"arm": k, "N": n, "V": V, "K": K, "ms": round(med, 3),
-                     "ms_all": [round(v, 3) for v in ms[k]],
-                     "mem_growth_MB": round(mem[k] / 2 ** 20, 1),
-                     "tflops": round(2.0 * n * V * K / (med * 1e-3) / 1e12, 1),
-                     "max_abs_diff_nll": diff, "card": info}
-                results.append(r)
-                print(json.dumps(r), flush=True)
+            comp = lambda: full_softmax_composition(x, t, w, b)          # noqa: E731
+            nll = lambda: parallax.nn.full_softmax_nll(x, t, w, b)       # noqa: E731
+            ref, fused = comp(), nll()                                   # warm-up + values
+            comp(), nll()
+            diff = {"max_abs_diff_nll": float((fused - ref).abs().max())}
+            del ref, fused
+            res = alternate([("composition", comp, a.iters), ("fused", nll, a.iters)], a.rounds)
+            for arm in ("composition", "fused"):
+                report(arm, n, res[arm], extra=diff)
+            for k in a.k:
+                topk = lambda: parallax.nn.full_softmax_topk(x, w, b, k)    # noqa: E731
+                tcomp = lambda: full_softmax_topk_composition(x, w, b, k)   # noqa: E731
+                lp, ids = topk()
+                clp, cids = full_softmax_topk_composition(x, w, b, k + 1)
+                d = clp[:, :-1] - clp[:, 1:]                  # [N, k]: the (k+1)-th included
+                ok = d > 2e-2
+                ok[:, 1:] &= d[:, :-1] > 2e-2
+                agree = {"ids_checked": int(ok.sum()),
+                         "ids_equal": bool(torch.equal(ids[ok], cids[:, :k][ok])),
+                         "max_abs_diff_log_probs": float((lp - clp[:, :k]).abs().max())}
+                del lp, ids, clp, cids, d, ok
+                res = alternate([("fused_topk", topk, a.iters), ("fused_nll", nll, a.iters),
+                                 ("composition", tcomp, a.comp_iters)], a.rounds)
+                report("composition", n, res["composition"], k)
+                tk = report("fused_topk", n, res["fused_topk"], k, agree)
+                nl = report("fused_nll", n, res["fused_nll"], k)
+                print(json.dumps({"N": n, "k": k, "topk_over_nll": round(tk / nl, 3)}),
+                      flush=True)
     sess.close()
     if a.out:
         with open(a.out, "w") as f:
