@@ -88,11 +88,18 @@ class LM1B(nn.Module):
 
     def __init__(self, vocab_size=793470, emb_size=512, state_size=2048,
                  projected_size=512, num_sampled=8192, num_steps=20,
-                 num_shards=32, keep_prob=0.9, lazy=False, eval_top_k=0):
+                 num_shards=32, keep_prob=0.9, lazy=False, eval_top_k=0, eval_sample=0,
+                 sample_temperature=1.0):
         """`eval_top_k` = k > 0: in eval mode `forward` also returns ``"top_k_ids"``, the k
-        most likely next words of every position (`parallax.nn.full_softmax_topk`)."""
+        most likely next words of every position (`parallax.nn.full_softmax_topk`).
+        `eval_sample` = n > 0: in eval mode `forward` also returns ``"sample_ids"`` and
+        ``"sample_log_probs"`` [B, T, n], n next words of every position drawn without
+        replacement at temperature `sample_temperature` (`parallax.nn.full_softmax_sample`,
+        seeded by the `sample_seed` feed)."""
         super().__init__()
         self.eval_top_k = int(eval_top_k)
+        self.eval_sample = int(eval_sample)
+        self.sample_temperature = float(sample_temperature)
         self.vocab_size, self.emb_size = vocab_size, emb_size
         self.state_size, self.projected_size = state_size, projected_size
         self.num_sampled, self.num_steps = num_sampled, num_steps
@@ -121,10 +128,16 @@ class LM1B(nn.Module):
             out = F.dropout(out, 1.0 - self.keep_prob)
         return out.reshape(T * Bsz, -1), c, h
 
-    def forward(self, x, y, w=None, initial_state_c=None, initial_state_h=None):
+    def forward(self, x, y=None, w=None, initial_state_c=None, initial_state_h=None,
+                sample_seed=None):
+        """`y` may be None in eval mode: no loss (and no pass over the softmax table for it),
+        e.g. to generate text with `eval_sample`.  `sample_seed`: the int seed of the eval-mode
+        samples (None: drawn from torch's default generator)."""
         Bsz, T = x.shape
         dev = self.W.device
         dt = self.W.dtype
+        if y is None and self.training:
+            raise ValueError("LM1B needs targets y in training")
         # Everything below is time-major (rows ordered (t, b)): the LSTM node consumes and
         # produces [T, B, ·] and the loss is a mean over all rows, so transposing the
         # [B, T] *ids* once replaces transposed copies of the [B, T, 512] activations and
@@ -144,18 +157,25 @@ class LM1B(nn.Module):
         pre = self.prefetch_softmax(y) if sampled_mode else None
         inputs, c, h = self.lstm(e, c, h)
         row_w = None if w is None else w.t().reshape(-1)
+        out = {}
         if sampled_mode:
-            loss = self.sampled_softmax_loss(inputs, pre, row_w)
-        else:
+            out["loss"] = self.sampled_softmax_loss(inputs, pre, row_w)
+        elif y is not None:
             loss = self.full_softmax_loss(inputs, y.t().reshape(-1))
             if row_w is not None:
                 loss = loss * row_w.to(loss.dtype)
-            loss = loss.mean()
-        out = {"loss": loss, "final_state_c": c.detach(), "final_state_h": h.detach()}
+            out["loss"] = loss.mean()
+        out.update(final_state_c=c.detach(), final_state_h=h.detach())
         if self.eval_top_k > 0 and not self.training:
             _, ids = pnn.full_softmax_topk(inputs, self.softmax_w, self.softmax_b,
                                            self.eval_top_k)
             out["top_k_ids"] = ids.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
+        if self.eval_sample > 0 and not self.training:
+            seed = None if sample_seed is None else int(sample_seed)
+            lp, ids = pnn.full_softmax_sample(inputs, self.softmax_w, self.softmax_b,
+                                              self.eval_sample, self.sample_temperature, seed)
+            out["sample_ids"] = ids.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
+            out["sample_log_probs"] = lp.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
         return out
 
     def prefetch_softmax(self, y):

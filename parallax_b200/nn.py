@@ -174,6 +174,53 @@ def full_softmax_topk(inputs, weight, bias, k):
     return _ft(inputs, weight, bias, k)
 
 
+def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, seed=None):
+    """Next-word sampling from a partitioned output table: for every row of `inputs`,
+    `num_samples` = n distinct rows of the table drawn without replacement from ::
+
+        softmax((inputs @ weight.weight.T + bias.weight.T) / temperature)
+
+    in draw order.  Returns ``(log_probs, ids)``, both ``[N, n]``: `ids` int64 global row ids
+    (never a padding row), `log_probs` fp32 the tempered ``log_softmax(logits / temperature)``
+    at each id — each id's own log-probability, not the probability of the sequence of draws
+    without replacement.
+
+    The draws are the n largest Gumbel keys ``s − log E`` of the row (Gumbel-top-k), s the fp32
+    logit times fp32(1 / temperature) and E ~ Exp(1) a hash of (seed, row index in `inputs`,
+    global id) (`parallax_b200.parallel.engine.sample_uniform`).  So a given seed draws the same
+    ids whatever the world size, partitioning, layout or path, except where two keys are within
+    a few ulp.  `seed=None` draws a seed from torch's default CPU generator, so successive calls
+    differ, as `torch.multinomial`'s do.  `inputs`, `weight` and `bias` are those of
+    `full_softmax_nll`.  Under the conditions of its fused path and with n <= 32, one fused
+    kernel keeps each row's n best keys where the rows live (no gathered table, no [N, V]
+    logits); otherwise the table is gathered and the logits materialised, which also carries
+    gradients into `log_probs`.  `ValueError` for the shapes `full_softmax_nll` refuses, a
+    `num_samples` that is not an int in [1, V], a `temperature` that is not a finite real number
+    > 0, and a `seed` that is neither None nor an int in [0, 2^32)."""
+    import math
+    import numbers
+    if inputs.dim() != 2:
+        raise ValueError("inputs must be [N, K], got shape %s" % (tuple(inputs.shape),))
+    _check_full_softmax(inputs, weight, bias)
+    V = weight.num_embeddings
+    if isinstance(num_samples, bool) or not isinstance(num_samples, int) or \
+            not 1 <= num_samples <= V:
+        raise ValueError("num_samples must be an int in [1, %d], got %r" % (V, num_samples))
+    if isinstance(temperature, bool) or not isinstance(temperature, numbers.Real) or \
+            not math.isfinite(temperature) or not temperature > 0:
+        raise ValueError("temperature must be a finite real number > 0, got %r" % (temperature,))
+    inv_tau = float(torch.tensor(1.0 / float(temperature), dtype=torch.float32))
+    if not math.isfinite(inv_tau) or inv_tau <= 0.0:
+        raise ValueError("temperature %r has no finite fp32 reciprocal > 0" % (temperature,))
+    if seed is None:
+        seed = int(torch.randint(0, 1 << 32, (), dtype=torch.int64))
+    elif isinstance(seed, bool) or not isinstance(seed, numbers.Integral) or \
+            not 0 <= seed < 1 << 32:
+        raise ValueError("seed must be None or an int in [0, 2^32), got %r" % (seed,))
+    from .parallel.engine import full_softmax_sample as _fsm
+    return _fsm(inputs, weight, bias, num_samples, inv_tau, int(seed))
+
+
 def _check_full_softmax(inputs, weight, bias):
     if weight.embedding_dim != inputs.shape[1]:
         raise ValueError("weight rows have %d columns, inputs have %d"

@@ -22,6 +22,12 @@
 // px_full_softmax_topk_combine_kernel merges the grid's sorted lists and the (max, Σexp) pairs
 // into log-probabilities and int64 ids.
 //
+// Sampling (px_full_softmax_sample): the top-k instantiations with SAMPLE = true scale the
+// biased logits by 1/τ before the (max, Σexp) pairs, so those are of s = l/τ, then replace each s
+// by its Gumbel key s − log E (sparse_group.cuh) and keep the n best keys with the same topk_row:
+// the n largest keys of a row are n draws without replacement from softmax(s), in draw order.
+// The combine recovers s of each kept entry from its key and writes s − lse.
+//
 // One-sided like the lookup: peers' rows are read over NVLink with 16-byte loads; nothing is
 // exchanged, so a rank may evaluate alone.  In sync mode the kernel first waits applied[o] >=
 // completed steps on the group header (the lookup's freshness rule).
@@ -63,7 +69,16 @@ struct TopkArgs : EvalArgs {
   GroupGeom g;                      // for the global ids of the partitions' rows
   int k;
 };
-template <int KC> using EvalParams = typename std::conditional<KC == 0, EvalArgs, TopkArgs>::type;
+
+// the sampling kernels' arguments: the lists hold (key, global id) pairs
+struct SampleArgs : TopkArgs {
+  float inv_tau;                    // fp32(1/τ), finite and > 0
+  uint32_t seed;
+  int row0;                         // index of X's row 0 within the caller's batch (chunking)
+};
+template <int KC, bool SAMPLE = false>
+using EvalParams = typename std::conditional<
+    KC == 0, EvalArgs, typename std::conditional<SAMPLE, SampleArgs, TopkArgs>::type>::type;
 
 __device__ __forceinline__ bool tk_beats(float v, int id, float v2, int id2) {
   return v > v2 || (v == v2 && id < id2);
@@ -156,10 +171,11 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
 }
 
 // BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows).  KC: top-k list
-// capacity (0: log-sum-exp only; else k <= KC and the top-k epilogue runs)
-template <typename BiasT, int KC>
+// capacity (0: log-sum-exp only; else k <= KC and the top-k epilogue runs).  SAMPLE (KC > 0):
+// the lists rank Gumbel keys of the tempered logits instead of the logits
+template <typename BiasT, int KC, bool SAMPLE = false>
 __global__ void __launch_bounds__(THREADS, 1)
-px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParams<KC> a) {
+px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParams<KC, SAMPLE> a) {
   constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -282,6 +298,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
             for (int e = 0; e < 2; ++e) {
               float& v = acc[j * 4 + 2 * h + e];
               v += s_bias[j * 8 + cq + e];
+              if constexpr (SAMPLE) v *= a.inv_tau;
               mx = fmaxf(mx, v);
             }
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
@@ -303,6 +320,21 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
             float2 c = first ? make_float2(-INFINITY, 0.f) : *p;
             lse_merge(c, mx, sum);
             *p = c;
+          }
+          if constexpr (SAMPLE) {
+            // keys s − log E in place of s (padding stays −inf), and the quad's key maximum
+            const uint32_t rk = sample_row_key(a.seed, (uint32_t)(a.row0 + row));
+            mx = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                float& v = acc[j * 4 + 2 * h + e];
+                v -= sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
+                mx = fmaxf(mx, v);
+              }
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
           }
           if constexpr (KC > 0) {
             if (row < a.N)
@@ -366,13 +398,20 @@ px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, i
 
 // one warp per row: merge the grid's (max, Σexp) pairs, then the grid's sorted top-k lists in k
 // rounds of warp-wide arg-max over the lists' heads (lane l holds the heads of lists l, l + 32,
-// ...), and write log_probs = logit − lse and the ids of the row's k best entries
+// ...), and write log_probs = logit − lse and the ids of the row's k best entries.
+// SAMPLE: the entries are keys s − log E of the lists of the sampling kernels; the entry's s is
+// recovered as key + log E with the same noise (seed, row0 + row, id), which is within an ulp of
+// the key of the s the kernel scored.  Storing s with each entry instead would widen the entry,
+// the lists and topk_row that the top-k kernels share; recomputing costs one hash and two
+// logarithms per output.
 constexpr int TK_LISTS_PER_LANE = 8;       // grid <= 256
 
+template <bool SAMPLE>
 __global__ void __launch_bounds__(256)
 px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
                                     const TopkEntry* __restrict__ tk, int grid, int N, int k,
-                                    float* __restrict__ log_probs, long long* __restrict__ ids) {
+                                    float* __restrict__ log_probs, long long* __restrict__ ids,
+                                    uint32_t seed, int row0) {
   const int lane = threadIdx.x & 31;
   for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
     const float2 c = ev_grid_lse(ws, grid, N, row, lane);
@@ -410,6 +449,8 @@ px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
       }
     }
     if (lane < k) {
+      if constexpr (SAMPLE)
+        mine.v += sample_log_e(sample_row_key(seed, (uint32_t)(row0 + row)), (uint32_t)mine.id);
       log_probs[(size_t)row * k + lane] = mine.v - lse;
       ids[(size_t)row * k + lane] = mine.id;
     }
@@ -461,17 +502,19 @@ int ev_combine_blocks(int N) {
   return blocks > PX_NUM_SMS * 8 ? PX_NUM_SMS * 8 : blocks;
 }
 
-template <typename BiasT, int KC>
-void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC>& a, cudaStream_t stream) {
+template <typename BiasT, int KC, bool SAMPLE = false>
+void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC, SAMPLE>& a,
+               cudaStream_t stream) {
   using namespace tc;
   static bool set = false;
   if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC>,
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize,
                          ev_smem_bytes(EV_KMAX / BK, KC));
     set = true;
   }
-  px_full_softmax_lse_kernel<BiasT, KC><<<grid, THREADS, ev_smem_bytes(a.kb, KC), stream>>>(tx, a);
+  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE>
+      <<<grid, THREADS, ev_smem_bytes(a.kb, KC), stream>>>(tx, a);
 }
 
 template <typename BiasT>
@@ -485,11 +528,36 @@ void ev_nll(int grid, const CUtensorMap& tx, const tc::EvalArgs& a, const void* 
 }
 
 // the list capacity is k rounded up to 8, 16 or 32
-template <typename BiasT>
-void ev_topk(int grid, const CUtensorMap& tx, const tc::TopkArgs& a, cudaStream_t stream) {
-  if (a.k <= 8) ev_launch<BiasT, 8>(grid, tx, a, stream);
-  else if (a.k <= 16) ev_launch<BiasT, 16>(grid, tx, a, stream);
-  else ev_launch<BiasT, 32>(grid, tx, a, stream);
+template <typename BiasT, bool SAMPLE>
+void ev_topk(int grid, const CUtensorMap& tx, const tc::EvalParams<8, SAMPLE>& a,
+             cudaStream_t stream) {
+  if (a.k <= 8) ev_launch<BiasT, 8, SAMPLE>(grid, tx, a, stream);
+  else if (a.k <= 16) ev_launch<BiasT, 16, SAMPLE>(grid, tx, a, stream);
+  else ev_launch<BiasT, 32, SAMPLE>(grid, tx, a, stream);
+}
+
+// px_full_softmax_topk (SAMPLE = false: inv_tau, seed and row0 unused) and px_full_softmax_sample
+template <bool SAMPLE>
+int ev_lists(const void* X, int N, int K, const void* w_ptrs, int w_pitch, const void* b_ptrs,
+             int b_pitch, int b_bf16, const int* row_cnt, const int* part_idx, int slots,
+             const GroupGeom* g, int rank, const void* hdr_mine, const void* ctl, int wait,
+             void* ws, int ws_ctas, int k, void* tk, float* log_probs, long long* ids,
+             float inv_tau, uint32_t seed, int row0, cudaStream_t stream) {
+  using namespace tc;
+  if (N <= 0) return 0;
+  if (ws_ctas > 32 * TK_LISTS_PER_LANE) return -2;
+  SampleArgs a;
+  CUtensorMap tx;
+  int grid;
+  int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                    slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
+  if (rc) return rc;
+  a.tk = (TopkEntry*)tk; a.part_idx = part_idx; a.g = *g; a.k = k;
+  a.inv_tau = inv_tau; a.seed = seed; a.row0 = row0;
+  (b_bf16 ? ev_topk<__nv_bfloat16, SAMPLE> : ev_topk<float, SAMPLE>)(grid, tx, a, stream);
+  px_full_softmax_topk_combine_kernel<SAMPLE><<<ev_combine_blocks(N), 256, 0, stream>>>(
+      (const float2*)ws, (const TopkEntry*)tk, grid, N, k, log_probs, ids, seed, row0);
+  return (int)cudaGetLastError();
 }
 
 }  // namespace
@@ -536,21 +604,31 @@ int px_full_softmax_topk(const void* X, int N, int K, const void* w_ptrs, int w_
                          const int* part_idx, int slots, const GroupGeom* g, int rank,
                          const void* hdr_mine, const void* ctl, int wait, void* ws, int ws_ctas,
                          int k, void* tk, float* log_probs, long long* ids, cudaStream_t stream) {
-  using namespace tc;
   if (k < 1 || k > 32) return -3;
-  if (N <= 0) return 0;
-  if (ws_ctas > 32 * TK_LISTS_PER_LANE) return -2;
-  TopkArgs a;
-  CUtensorMap tx;
-  int grid;
-  int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
-                    slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
-  if (rc) return rc;
-  a.tk = (TopkEntry*)tk; a.part_idx = part_idx; a.g = *g; a.k = k;
-  (b_bf16 ? ev_topk<__nv_bfloat16> : ev_topk<float>)(grid, tx, a, stream);
-  px_full_softmax_topk_combine_kernel<<<ev_combine_blocks(N), 256, 0, stream>>>(
-      (const float2*)ws, (const TopkEntry*)tk, grid, N, k, log_probs, ids);
-  return (int)cudaGetLastError();
+  return ev_lists<false>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt, part_idx,
+                         slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, k, tk, log_probs, ids,
+                         1.f, 0u, 0, stream);
+}
+
+// n draws without replacement from softmax((X w^T + b) / τ) for each row of X [N, K], in draw
+// order (Gumbel-top-k): ids int64 [N, n] are the n largest keys s − log E of the row, s = fp32
+// logit · inv_tau and E the noise of (seed, row0 + row, id) (sparse_group.cuh), so a row's draws
+// depend on its index in the caller's batch, not on the chunk; log_probs fp32 [N, n] are s − lse
+// at those ids.  Arguments as px_full_softmax_topk with k = n (tk holds (key, id) entries), plus
+//   inv_tau: fp32(1/τ), finite and > 0;   seed: the call's seed;   row0: batch index of X's row 0.
+// Returns 0, a negative argument error (-3: n out of range, -4: inv_tau not finite and > 0), or a
+// CUDA error code.
+int px_full_softmax_sample(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                           const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                           const int* part_idx, int slots, const GroupGeom* g, int rank,
+                           const void* hdr_mine, const void* ctl, int wait, void* ws, int ws_ctas,
+                           int n, void* tk, float* log_probs, long long* ids, float inv_tau,
+                           unsigned int seed, int row0, cudaStream_t stream) {
+  if (n < 1 || n > 32) return -3;
+  if (!(inv_tau > 0.f) || !isfinite(inv_tau)) return -4;
+  return ev_lists<true>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt, part_idx,
+                        slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, n, tk, log_probs, ids,
+                        inv_tau, seed, row0, stream);
 }
 
 }  // extern "C"

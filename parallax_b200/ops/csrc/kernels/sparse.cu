@@ -87,10 +87,7 @@ __device__ __forceinline__ float4 unpack_bf16x4(const uint2& v) {
 // hash and rounding in torch arithmetic, and the two agree bit for bit.
 // The 16 random bits of element (row, col) are a hash of the table's seed, the global step, the
 // row's GLOBAL id and the column only: replicas, world sizes and partitionings round alike.
-__device__ __forceinline__ uint32_t sr_mix(uint32_t x) {
-  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu;
-  return x ^ (x >> 16);
-}
+// sr_mix is in sparse_group.cuh.
 __device__ __forceinline__ uint32_t sr_row_key(uint32_t seed, uint32_t step, uint32_t gid) {
   return sr_mix(sr_mix(seed ^ step) ^ gid);
 }

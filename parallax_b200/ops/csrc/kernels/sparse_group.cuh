@@ -23,6 +23,28 @@ __device__ __forceinline__ int geom_gid(const GroupGeom& g, int p, int idx) {
   return p < g.extras ? p * (g.base + 1) + idx : p * g.base + g.extras + idx;
 }
 
+// 32-bit integer hash (xor-shift, multiply, twice); `optim.sr_mix` is the same hash in torch.
+// It keys the stochastic rounding of bf16 masters (sparse.cu) and the sampling noise below.
+__device__ __forceinline__ uint32_t sr_mix(uint32_t x) {
+  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu;
+  return x ^ (x >> 16);
+}
+
+// Sampling noise (full-softmax sampling in softmax_eval.cu; `engine.sample_uniform` and
+// `engine.sample_log_e` are the same in torch).  Row `row` of a call draws with the keys
+// s − log E of its global ids, E = −log1p(−v) ~ Exp(1) (so −log E is Gumbel), where
+//   v = min(h · 2^-32 + 2^-33, 1 − 2^-24),  h = sr_mix(sample_row_key(seed, row) ^ gid).
+// h and v are bit-identical in torch; E keeps fp32 relative precision down to 1.2e-10, where
+// the winner is decided, and the clamp keeps every key finite.
+__device__ __forceinline__ uint32_t sample_row_key(uint32_t seed, uint32_t row) {
+  return sr_mix(sr_mix(seed) ^ row);
+}
+__device__ __forceinline__ float sample_log_e(uint32_t row_key, uint32_t gid) {
+  const float v = fminf(__fadd_rn(__fmul_rn(__uint2float_rn(sr_mix(row_key ^ gid)), 0x1p-32f),
+                                  0x1p-33f), 0x1.fffffep-1f);
+  return logf(-log1pf(-v));
+}
+
 // per-rank control block of a group (local memory)
 struct SparseCtl {
   uint32_t step;                // completed steps

@@ -182,23 +182,86 @@ def full_softmax_composition(inputs, targets, weight, bias):
 
 def full_softmax_topk_composition(inputs, weight, bias, k):
     """The unfused top-k: gather every row, materialise the [N, V] logits, `log_softmax`, then
-    the k best of each row by (logit descending, id ascending).  `torch.topk` leaves the order
-    of equal values open, so it only finds each row's k-th value; the rows' candidates at or
-    above it are then sorted stably (ascending id within equal values).  Gradients flow into
-    `log_probs`."""
+    the k best of each row by (logit descending, id ascending) (`_ordered_top`).  Gradients
+    flow into `log_probs`."""
     lp = torch.log_softmax(_gathered_logits(inputs, weight, bias), dim=-1)
-    n = lp.shape[0]
+    top = _ordered_top(lp.detach(), k)
+    return lp.gather(1, top), top
+
+
+def _ordered_top(keys, k):
+    """int64 [N, k]: the columns of each row's k largest `keys` [N, V], ordered by (key
+    descending, column ascending).  `torch.topk` leaves the order of equal values open, so it
+    only finds each row's k-th value; the rows' candidates at or above it are then sorted
+    stably (ascending column within equal values)."""
+    n = keys.shape[0]
     with torch.no_grad():
-        kth = torch.topk(lp, k, dim=1).values[:, -1:]
-        r, c = (lp >= kth).nonzero(as_tuple=True)   # row-major: ids ascend within a row
-        o = torch.sort(lp[r, c], descending=True, stable=True).indices
+        kth = torch.topk(keys, k, dim=1).values[:, -1:]
+        r, c = (keys >= kth).nonzero(as_tuple=True)   # row-major: ids ascend within a row
+        o = torch.sort(keys[r, c], descending=True, stable=True).indices
         o = o[torch.sort(r[o], stable=True).indices]
         r, c = r[o], c[o]
         cnt = torch.bincount(r, minlength=n)
         rank = torch.arange(r.numel(), device=r.device) - (torch.cumsum(cnt, 0) - cnt)[r]
         keep = rank < k
-        top = torch.empty(n, k, dtype=torch.int64, device=lp.device)
+        top = torch.empty(n, k, dtype=torch.int64, device=keys.device)
         top[r[keep], rank[keep]] = c[keep]
+    return top
+
+
+def full_softmax_sample(inputs, weight, bias, n, inv_tau, seed):
+    """``(log_probs [N, n], ids [N, n])``: n draws without replacement from the tempered full
+    softmax of each row, in draw order (the n largest Gumbel keys).  Fused where
+    `_fused_eval_group` finds a group and n <= 32; everything else (and training) runs
+    `full_softmax_sample_composition`.  Both take the same keys, so they draw the same ids
+    except where two keys are within a few ulp."""
+    grp = _fused_eval_group(inputs, weight, bias)
+    if grp is not None and n <= FUSED_TOPK_MAX:
+        return grp.full_softmax_sample(inputs, n, inv_tau, seed)
+    return full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed)
+
+
+def sample_uniform(seed, rows, gids):
+    """fp32 [len(rows), len(gids)]: the sampling noise's uniform v of (seed, row, global id),
+    bit for bit the kernels' (`sample_log_e` in `kernels/sparse_group.cuh`)::
+
+        h = sr_mix(sr_mix(sr_mix(seed) ^ row) ^ gid)
+        v = min(fp32(h) · 2^-32 + 2^-33, 1 − 2^-24)
+
+    `rows` and `gids` are int64 tensors of values in [0, 2^32)."""
+    sr_mix, m32 = _optim.sr_mix, _optim._M32
+    rk = sr_mix(sr_mix(int(seed) & m32) ^ (rows & m32))
+    h = sr_mix(rk[:, None] ^ (gids & m32)[None, :])
+    v = h.to(torch.float32) * 2.0 ** -32 + 2.0 ** -33
+    return v.clamp_(max=1.0 - 2.0 ** -24)
+
+
+def sample_log_e(seed, rows, gids):
+    """fp32 [len(rows), len(gids)]: log E with E = −log1p(−v) ~ Exp(1) (`sample_uniform`); the
+    Gumbel key of a scaled logit s is s − log E."""
+    return torch.log(-torch.log1p(-sample_uniform(seed, rows, gids)))
+
+
+# elements of the int64 temporaries of the composition's noise, per row chunk
+_NOISE_CHUNK = 1 << 24
+
+
+def full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed):
+    """The unfused sampler: gather every row, materialise the [N, V] logits, scale them by
+    `inv_tau` and take `log_softmax`; the keys s − log E come from the torch noise in row chunks,
+    and the ids are each row's n best keys by (key descending, id ascending) (`_ordered_top`).
+    Gradients flow into `log_probs`."""
+    s = _gathered_logits(inputs, weight, bias) * inv_tau
+    lp = torch.log_softmax(s, dim=-1)
+    N, V = s.shape
+    with torch.no_grad():
+        keys = s.detach().clone()
+        gids = torch.arange(V, device=s.device)
+        step = max(1, _NOISE_CHUNK // max(V, 1))
+        for r0 in range(0, N, step):
+            rows = torch.arange(r0, min(N, r0 + step), device=s.device)
+            keys[r0:r0 + step] -= sample_log_e(seed, rows, gids)
+        top = _ordered_top(keys, n)
     return lp.gather(1, top), top
 
 

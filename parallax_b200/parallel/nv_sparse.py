@@ -573,12 +573,13 @@ class NVSparseGroup(object):
         return self._slots[1:]
 
     def _eval_operands(self, x, what):
-        """Checks the inputs of the eval entry point `what` and returns what px_full_softmax_nll
-        and px_full_softmax_topk share: (x, K, (bias source, bias pitch), head, tail, stream).
-        head is their ctypes arguments from the weight shadow pointers through the row counts,
-        tail those from the slot count through `wait`; the top-k kernel takes its partition
-        index between the two.  The bias rows are the master rows: fp32, or bf16 rows of the
-        shadow's layout with bf16 masters (widened where they are added)."""
+        """Checks the inputs of the eval entry point `what` and returns what
+        px_full_softmax_nll, px_full_softmax_topk and px_full_softmax_sample share: (x, K,
+        (bias source, bias pitch), head, tail, stream).  head is their ctypes arguments from the
+        weight shadow pointers through the row counts, tail those from the slot count through
+        `wait`; the top-k and sampling kernels take their partition index between the two.  The
+        bias rows are the master rows: fp32, or bf16 rows of the shadow's layout with bf16
+        masters (widened where they are added)."""
         tw, tb = self.tables
         if not tw.use_shadow or tb.D != 1 or x.dim() != 2 or x.shape[1] != tw.D or \
                 x.dtype != torch.bfloat16:
@@ -637,12 +638,27 @@ class NVSparseGroup(object):
         where their owners store them (`ops/csrc/kernels/softmax_eval.cu`).  1 <= k <= 32.
         Scratch is per call and O(NUM_SMS · rows · k): rows are taken in chunks so that the
         per-CTA lists fit in `consts.TOPK_WS_BYTES`.  One-sided: no other rank takes part."""
+        return self._ranked(x, k, "full_softmax_topk", "k")
+
+    def full_softmax_sample(self, x, n, inv_tau, seed):
+        """n draws without replacement from ``softmax((x @ W.T + b) · inv_tau)`` for each row
+        of bf16 inputs `x` [N, K], in draw order: ``(log_probs fp32 [N, n], ids int64 [N, n])``,
+        where log_probs are the tempered log-probabilities of the ids.  The kernel keeps the n
+        largest Gumbel keys ``s − log E`` of each row (s the scaled fp32 logit, E the noise of
+        (seed, row, id), `engine.sample_log_e`), so the draws depend on the seed, the row's
+        index in `x` and the ids only.  1 <= n <= 32, inv_tau = fp32(1/τ) > 0, seed in
+        [0, 2^32).  Chunked, one-sided and fresh as `full_softmax_topk`."""
+        return self._ranked(x, n, "full_softmax_sample", "num_samples", (inv_tau, seed))
+
+    def _ranked(self, x, k, what, k_name, sample=None):
+        """The list-keeping eval kernels: top-k (`sample` None) or sampling (`sample` =
+        (inv_tau, seed)), in row chunks whose per-CTA lists fit in `consts.TOPK_WS_BYTES`."""
         L = ops.lib()
         V = self.tables[0].V
         if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, V):
-            raise ValueError("full_softmax_topk: k must be an int in [1, %d], got %r"
-                             % (min(32, V), k))
-        x, K, _, head, tail, stream = self._eval_operands(x, "full_softmax_topk")
+            raise ValueError("%s: %s must be an int in [1, %d], got %r"
+                             % (what, k_name, min(32, V), k))
+        x, K, _, head, tail, stream = self._eval_operands(x, what)
         n = int(x.shape[0])
         log_probs = torch.empty(n, k, dtype=torch.float32, device=self.device)
         ids = torch.empty(n, k, dtype=torch.int64, device=self.device)
@@ -656,12 +672,15 @@ class NVSparseGroup(object):
         tk = torch.empty(ctas * chunk * k * 2, dtype=torch.int32, device=self.device)
         for r0 in range(0, n, chunk):
             m = min(chunk, n - r0)
+            args = (_vp(x[r0:].data_ptr()), m, K, *head, _vp(part.data_ptr()), *tail,
+                    _vp(ws.data_ptr()), ctas, k, _vp(tk.data_ptr()),
+                    _vp(log_probs[r0:].data_ptr()), _vp(ids[r0:].data_ptr()))
             _count(2)
-            ops.check(L.px_full_softmax_topk(
-                _vp(x[r0:].data_ptr()), m, K, *head, _vp(part.data_ptr()), *tail,
-                _vp(ws.data_ptr()), ctas, k, _vp(tk.data_ptr()),
-                _vp(log_probs[r0:].data_ptr()), _vp(ids[r0:].data_ptr()), stream),
-                "full_softmax_topk")
+            if sample is None:
+                rc = L.px_full_softmax_topk(*args, stream)
+            else:
+                rc = L.px_full_softmax_sample(*args, sample[0], sample[1], r0, stream)
+            ops.check(rc, what)
         return log_probs, ids
 
     def add_pending(self, token, grads):

@@ -1,9 +1,12 @@
 """Full-softmax evaluation of the LM1B output layer, in one process: the NLL's gather + matmul +
 cross_entropy composition against the fused kernel (`parallax.nn.full_softmax_nll`), and top-k
 next-word prediction's gather + matmul + log_softmax + top-k composition against the fused top-k
-kernel (`parallax.nn.full_softmax_topk`), next to the fused NLL at the same N.
+kernel (`parallax.nn.full_softmax_topk`), next to the fused NLL at the same N, and sampling's
+gather + matmul + log_softmax + noise + top-n composition against the fused sampler
+(`parallax.nn.full_softmax_sample`), next to the fused top-k at the same n and the fused NLL.
 
-    python tools/bench_full_softmax.py [--n 640 2560] [--k 1 10 32] [--out result.json]
+    python tools/bench_full_softmax.py [--n 640 2560] [--k 1 10 32] [--sample 1 10 32]
+                                       [--temperature 1.0] [--out result.json]
 
 Builds LM1B's (softmax_w, softmax_b) co-lookup group through the engine on the NVLink fabric,
 one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N:
@@ -14,6 +17,10 @@ one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N:
   alternate over the rounds, and the composition is timed after them in each round over
   --comp_iters calls.  The fused ids are compared with the composition's where its consecutive
   log-probabilities, the (k+1)-th included, differ by > 2e-2.
+- sampling, for each n of --sample (default none) at --temperature: the fused sampler, the fused
+  top-k at k = n and the fused NLL alternate over the rounds, and the composition is timed after
+  them.  The records carry the share of first draws equal to the composition's (same seed; its
+  logits are rounded to bf16, so keys closer than that may swap).
 Per arm: ms per call (CUDA events, after warm-up), the growth of `torch.cuda.max_memory_allocated`
 during one call, and the achieved TFLOP/s from 2·N·V·K.  The card name, power limit and max SM
 clock are read in the same run.
@@ -31,6 +38,7 @@ import torch  # noqa: E402
 import parallax_b200 as parallax  # noqa: E402
 from parallax_b200.models.lm1b import LM1B, lm1b_graph  # noqa: E402
 from parallax_b200.parallel.engine import (full_softmax_composition,  # noqa: E402
+                                           full_softmax_sample_composition,
                                            full_softmax_topk_composition)
 
 
@@ -77,6 +85,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, nargs="+", default=[640, 2560])
     ap.add_argument("--k", type=int, nargs="*", default=[1, 10, 32])
+    ap.add_argument("--sample", type=int, nargs="*", default=[])
+    ap.add_argument("--temperature", type=float, default=1.0)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--comp_iters", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=3)
@@ -102,6 +112,8 @@ def main():
         ms, grow = timing
         med = statistics.median(ms)
         r = {"arm": arm, "N": n, **({} if k is None else {"k": k}), "V": V, "K": K,
+             **({} if k is None or not arm.endswith("sample") else
+                {"temperature": a.temperature}),
              "ms": round(med, 3), "ms_all": [round(v, 3) for v in ms],
              "mem_growth_MB": round(grow / 2 ** 20, 1),
              "tflops": round(2.0 * n * V * K / (med * 1e-3) / 1e12, 1), **(extra or {}),
@@ -143,6 +155,29 @@ def main():
                 nl = report("fused_nll", n, res["fused_nll"], k)
                 print(json.dumps({"N": n, "k": k, "topk_over_nll": round(tk / nl, 3)}),
                       flush=True)
+            inv_tau = float(torch.tensor(1.0 / a.temperature, dtype=torch.float32))
+            for k in a.sample:
+                smp = lambda: parallax.nn.full_softmax_sample(    # noqa: E731
+                    x, w, b, k, a.temperature, 12345)
+                scomp = lambda: full_softmax_sample_composition(  # noqa: E731
+                    x, w, b, k, inv_tau, 12345)
+                topk = lambda: parallax.nn.full_softmax_topk(x, w, b, k)    # noqa: E731
+                lp, ids = smp()
+                clp, cids = scomp()
+                agree = {"first_draw_equal": round(float((ids[:, 0] == cids[:, 0]).float()
+                                                         .mean()), 4),
+                         "max_abs_diff_log_probs_equal_ids": float(
+                             (lp - clp).abs()[ids == cids].max())}
+                del lp, ids, clp, cids
+                res = alternate([("fused_sample", smp, a.iters), ("fused_topk", topk, a.iters),
+                                 ("fused_nll", nll, a.iters),
+                                 ("composition_sample", scomp, a.comp_iters)], a.rounds)
+                report("composition_sample", n, res["composition_sample"], k)
+                sm = report("fused_sample", n, res["fused_sample"], k, agree)
+                tk = report("fused_topk", n, res["fused_topk"], k)
+                nl = report("fused_nll", n, res["fused_nll"], k)
+                print(json.dumps({"N": n, "n": k, "sample_over_topk": round(sm / tk, 3),
+                                  "sample_over_nll": round(sm / nl, 3)}), flush=True)
     sess.close()
     if a.out:
         with open(a.out, "w") as f:
