@@ -231,102 +231,6 @@ px_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
   }
 }
 
-__device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + __expf(-x)); }
-__device__ __forceinline__ float tanh_(float x) {
-  const float e = __expf(-2.f * fabsf(x));
-  return copysignf((1.f - e) / (1.f + e), x);
-}
-
-// ---------------------------------------------------------------------------
-// Recurrent LSTM step with the whole cell fused into the GEMM epilogue:
-//   gates = xw_t + h_{t-1} · Wh          (wgmma, accumulator in registers)
-//   c_t = σ(f+fb)·c_{t-1} + σ(i)·tanh(j);  m_t = σ(o)·tanh(c_t)
-// The 4S gate columns are stored GATE-INTERLEAVED: tile n (128 columns) holds
-// [i | j | f | o] × 32 hidden units (n·32 … n·32+31), so one CTA owns every
-// gate of its 32 units and the cell update never leaves the SM.  In the wgmma
-// accumulator layout a thread holds the same two columns of every 8-column
-// group, so it holds all four gates of 2 hidden units × 4 unit groups for each
-// of its 2 rows.  Replaces cuBLAS addmm + the stand-alone cell kernel (and the
-// [B,4S] pre-activation round trip).
-struct LstmArgs {
-  const __nv_bfloat16* xw;   // [M, 4S] permuted layout (input half + bias)
-  const float* c_prev;       // [M, S]
-  float* c_new;              // [M, S]
-  __nv_bfloat16* m_out;      // [M, S]
-  __nv_bfloat16* act;        // [M, 4S] permuted layout: σ(i) | tanh(j) | σ(f+fb) | σ(o)
-  int M, S, K;
-  float forget_bias;
-};
-
-template <int STAGES>
-__global__ void __launch_bounds__(THREADS, 1)
-px_lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                        const __grid_constant__ CUtensorMap tmap_b, LstmArgs g) {
-  constexpr int BN = 128;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  constexpr int STAGE_BYTES = BM * BK * 2 + BN * BK * 2;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  const int n_tile = blockIdx.x, m_tile = blockIdx.y;
-
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  float acc[BN / 2];
-  mainloop<BN, STAGES>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, 0, g.K / BK, m_tile * BM,
-                       n_tile * BN, acc);
-  if (threadIdx.x < 128) return;
-
-  const int t = threadIdx.x - 128, lane = t & 31;
-  const int lrow = (t >> 5) * 16 + (lane >> 2);
-  const int lu = (lane & 3) * 2;                     // first of this thread's 2 units in a group
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = m_tile * BM + lrow + 8 * h;
-    if (row >= g.M) continue;
-    const size_t gcol0 = (size_t)row * 4 * g.S + (size_t)n_tile * BN;   // permuted column base
-    const size_t ccol0 = (size_t)row * g.S + (size_t)n_tile * 32;       // hidden-unit base
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {                                       // 8 hidden units per group
-      const int u = q * 8 + lu;
-      float pre[4][2];                                                  // [gate][unit]
-#pragma unroll
-      for (int gi = 0; gi < 4; ++gi) {
-        // pre-activations stay fp32 (accumulator + bf16 addend)
-        const float2 x = bf16x2_to_float2(
-            *reinterpret_cast<const uint32_t*>(g.xw + gcol0 + gi * 32 + u));
-        pre[gi][0] = acc[(gi * 4 + q) * 4 + 2 * h] + x.x;
-        pre[gi][1] = acc[(gi * 4 + q) * 4 + 2 * h + 1] + x.y;
-      }
-      const float2 cp = *reinterpret_cast<const float2*>(g.c_prev + ccol0 + u);
-      float si[2], tj[2], sf[2], so[2], cn[2], mo[2];
-      const float cpv[2] = {cp.x, cp.y};
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        si[e] = sigm(pre[0][e]);
-        tj[e] = tanh_(pre[1][e]);
-        sf[e] = sigm(pre[2][e] + g.forget_bias);
-        so[e] = sigm(pre[3][e]);
-        cn[e] = sf[e] * cpv[e] + si[e] * tj[e];
-        mo[e] = so[e] * tanh_(cn[e]);
-      }
-      *reinterpret_cast<float2*>(g.c_new + ccol0 + u) = make_float2(cn[0], cn[1]);
-      *reinterpret_cast<uint32_t*>(g.m_out + ccol0 + u) = float2_to_bf16x2(mo[0], mo[1]);
-      *reinterpret_cast<uint32_t*>(g.act + gcol0 + 0 * 32 + u) = float2_to_bf16x2(si[0], si[1]);
-      *reinterpret_cast<uint32_t*>(g.act + gcol0 + 1 * 32 + u) = float2_to_bf16x2(tj[0], tj[1]);
-      *reinterpret_cast<uint32_t*>(g.act + gcol0 + 2 * 32 + u) = float2_to_bf16x2(sf[0], sf[1]);
-      *reinterpret_cast<uint32_t*>(g.act + gcol0 + 3 * 32 + u) = float2_to_bf16x2(so[0], so[1]);
-    }
-  }
-}
-
 // ------------------------------------------------------------------ host side
 
 template <int BN, int STAGES>
@@ -412,35 +316,6 @@ int px_gemm_tc(const void* A, const void* B, void* C, const void* addend, float*
     }
     px_gemm_tc_kernel<64, STAGES, false><<<grid, THREADS, SMEM, stream>>>(ta, tb, g);
   }
-  return (int)cudaGetLastError();
-}
-
-// Fused recurrent LSTM step (see px_lstm_gates_tc_kernel).  h: [M,K] bf16;
-// WhP: [4S, K] bf16 gate-interleaved rows; xw/act: [M,4S] gate-interleaved.
-int px_lstm_gates_tc(const void* h, const void* WhP, const void* xw, const float* c_prev,
-                     float* c_new, void* m_out, void* act, int M, int S, int K,
-                     float forget_bias, cudaStream_t stream) {
-  using namespace tc;
-  if (M % BM || K % BK || S % 32) return -1;
-  CUtensorMap ta, tb;
-  int rc = make_tmap(&ta, h, M, K, BM);
-  if (rc) return rc;
-  rc = make_tmap(&tb, WhP, 4 * (uint64_t)S, K, 128);
-  if (rc) return rc;
-  LstmArgs g;
-  g.xw = (const __nv_bfloat16*)xw; g.c_prev = c_prev; g.c_new = c_new;
-  g.m_out = (__nv_bfloat16*)m_out; g.act = (__nv_bfloat16*)act;
-  g.M = M; g.S = S; g.K = K; g.forget_bias = forget_bias;
-  constexpr int STAGES = 4;
-  constexpr int SMEM = smem_bytes<128, STAGES>();
-  static bool set = false;
-  if (!set) {
-    cudaFuncSetAttribute(px_lstm_gates_tc_kernel<STAGES>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    set = true;
-  }
-  dim3 grid(4 * S / 128, M / BM, 1);
-  px_lstm_gates_tc_kernel<STAGES><<<grid, THREADS, SMEM, stream>>>(ta, tb, g);
   return (int)cudaGetLastError();
 }
 

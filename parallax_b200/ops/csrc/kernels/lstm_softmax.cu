@@ -60,25 +60,22 @@ template <typename T>
 __global__ void __launch_bounds__(256)
 px_lstm_cell_bwd_kernel(const T* __restrict__ dm, float* __restrict__ dc,
                         const T* __restrict__ act, const float* __restrict__ c_prev,
-                        const float* __restrict__ c_new, T* __restrict__ dgates, int B, int S,
-                        int interleaved) {
+                        const float* __restrict__ c_new, T* __restrict__ dgates, int B, int S) {
   const int total = B * S;
-  // gate g of unit s lives at column g*S + s (plain) or, gate-interleaved in
-  // tiles of 32 units, at (s/32)*128 + g*32 + s%32 (layout of the wgmma path)
-  const int GS = interleaved ? 32 : S;
+  // gate g of unit s lives at column g*S + s
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += gridDim.x * blockDim.x) {
     const int b = idx / S, s = idx - b * S;
-    const size_t g0 = (size_t)b * 4 * S + (interleaved ? (s >> 5) * 128 + (s & 31) : s);
-    const float si = to_f(act[g0]), tj = to_f(act[g0 + GS]), sf = to_f(act[g0 + 2 * GS]),
-                so = to_f(act[g0 + 3 * GS]);
+    const size_t g0 = (size_t)b * 4 * S + s;
+    const float si = to_f(act[g0]), tj = to_f(act[g0 + S]), sf = to_f(act[g0 + 2 * S]),
+                so = to_f(act[g0 + 3 * S]);
     const float tc = tanhf_(c_new[idx]);
     const float dmv = to_f(dm[idx]);
     const float dcv = dc[idx] + dmv * so * (1.f - tc * tc);
     dgates[g0] = from_f<T>(dcv * tj * si * (1.f - si));
-    dgates[g0 + GS] = from_f<T>(dcv * si * (1.f - tj * tj));
-    dgates[g0 + 2 * GS] = from_f<T>(dcv * c_prev[idx] * sf * (1.f - sf));
-    dgates[g0 + 3 * GS] = from_f<T>(dmv * tc * so * (1.f - so));
+    dgates[g0 + S] = from_f<T>(dcv * si * (1.f - tj * tj));
+    dgates[g0 + 2 * S] = from_f<T>(dcv * c_prev[idx] * sf * (1.f - sf));
+    dgates[g0 + 3 * S] = from_f<T>(dmv * tc * so * (1.f - so));
     dc[idx] = dcv * sf;
   }
 }
@@ -262,18 +259,16 @@ int px_lstm_cell_fwd(const void* gates, const float* c_prev, void* act, float* c
 }
 
 int px_lstm_cell_bwd(const void* dm, float* dc, const void* act, const float* c_prev,
-                     const float* c_new, void* dgates, int B, int S, int dtype, int interleaved,
-                     cudaStream_t stream) {
+                     const float* c_new, void* dgates, int B, int S, int dtype, cudaStream_t stream) {
   int blocks = (B * S + 255) / 256;
   if (blocks > PX_NUM_SMS * 8) blocks = PX_NUM_SMS * 8;
   if (dtype == 0)
     px_lstm_cell_bwd_kernel<float><<<blocks, 256, 0, stream>>>(
-        (const float*)dm, dc, (const float*)act, c_prev, c_new, (float*)dgates, B, S,
-        interleaved);
+        (const float*)dm, dc, (const float*)act, c_prev, c_new, (float*)dgates, B, S);
   else
     px_lstm_cell_bwd_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(
         (const __nv_bfloat16*)dm, dc, (const __nv_bfloat16*)act, c_prev, c_new,
-        (__nv_bfloat16*)dgates, B, S, interleaved);
+        (__nv_bfloat16*)dgates, B, S);
   return (int)cudaGetLastError();
 }
 

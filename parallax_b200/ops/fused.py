@@ -22,8 +22,7 @@ from . import lib as _lib, check as _check, register_signatures
 _vp, _i, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
 register_signatures({
     "px_lstm_cell_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
-    "px_lstm_cell_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "px_lstm_gates_tc": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
+    "px_lstm_cell_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_sampled_softmax": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_sampled_softmax_dot": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
                                     _vp]),
@@ -71,69 +70,6 @@ def lstm_layer_reference(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
     return torch.stack(outs), c, h
 
 
-_perm_cache = {}
-
-
-def _tc_forward_enabled():
-    """The fused wgmma forward step is opt-in (`PARALLAX_LSTM_TC_FWD=1`): it is
-    numerically equivalent but needs a per-step weight re-layout, and on one H100 (400 W
-    power limit) the LM1B bench step takes 1.64 ms with it against 1.42 ms without; the
-    wgmma split-K product on the backward path is always on."""
-    import os
-    return os.environ.get("PARALLAX_LSTM_TC_FWD", "0") == "1"
-
-
-def gate_interleave_perm(S, device):
-    """perm[n'] = n : column n' = tile·128 + g·32 + j of the gate-interleaved
-    layout holds original column n = g·S + tile·32 + j (g: i, j, f, o)."""
-    key = (S, str(device))
-    if key not in _perm_cache:
-        tiles = S // 32
-        g = torch.arange(4, device=device).view(1, 4, 1)
-        t = torch.arange(tiles, device=device).view(tiles, 1, 1)
-        j = torch.arange(32, device=device).view(1, 1, 32)
-        perm = (g * S + t * 32 + j).reshape(-1)
-        inv = torch.empty_like(perm)
-        inv[perm] = torch.arange(4 * S, device=device)
-        _perm_cache[key] = (perm, inv)
-    return _perm_cache[key]
-
-
-def _bwd_fused_w():
-    """Backward chain with the combined weight `Wc = W_P @ Wh` ([S, 4S]):
-    ``dm_{t-1} = dH_{t-1} W_P^T + dgates_t Wc^T`` — ONE product per time step on the
-    critical path instead of two (``dh = dH + dgates Wh^T`` then ``dm = dh W_P^T``); the
-    per-step `dh` values (needed only for dW_P) are produced afterwards by one batched GEMM
-    off the critical path.  "tc": wgmma split-K kernel, "cublas": torch.addmm, "0": off
-    (the default).  The combined product (128 x 2048 x 8192) reads 32 MB of weights per step
-    where the two it replaces read 10 MB; tools/bench_lstm_gemms.py times both."""
-    import os
-    return os.environ.get("PARALLAX_LSTM_BWD_FUSEDW", "0")
-
-
-def _wpt_side():
-    """PARALLAX_LSTM_WPT_SIDE=0: transpose W_P at the head of the backward pass instead."""
-    import os
-    return os.environ.get("PARALLAX_LSTM_WPT_SIDE", "1") != "0"
-
-
-def _dbias_stream():
-    """PARALLAX_LSTM_DBIAS_STREAM=1: the bias gradient (a bandwidth-bound column sum over
-    dgates) runs on a second side stream, next to the compute-bound weight-gradient GEMMs."""
-    import os
-    return os.environ.get("PARALLAX_LSTM_DBIAS_STREAM", "1") != "0"
-
-
-def _wgrad_chunks(T):
-    """How many pieces the weight-gradient GEMMs are cut into along time so that the
-    earlier pieces run on the side stream underneath the (latency-bound) recurrent
-    backward chain.  Default 1 (all after the loop, still on the side stream): the big
-    GEMMs compete for SMs with the latency-bound chain they would overlap."""
-    import os
-    n = int(os.environ.get("PARALLAX_LSTM_WGRAD_CHUNKS", "1"))
-    return max(1, min(n, T // 2 if T >= 4 else 1))
-
-
 class _LSTMLayerFn(torch.autograd.Function):
     """`W` is either the stacked `[E+P, 4S]` kernel of the reference's LSTM cell
     (`Wh is None`; rows `[:E]` multiply x, rows `[E:]` multiply h — one parameter, one
@@ -154,23 +90,10 @@ class _LSTMLayerFn(torch.autograd.Function):
             Wx, Wh = W.detach()[:E], W.detach()[E:]
         else:
             Wx = W
-        # wgmma path: recurrent GEMM with the LSTM cell fused into its epilogue
-        # (gate-interleaved column layout, see gemm_tc.cu)
-        tc = (dt == torch.bfloat16 and Bsz % 128 == 0 and P % 64 == 0 and S % 32 == 0 and
-              _tc_forward_enabled())
-        if tc:
-            perm, inv = gate_interleave_perm(S, dev)
-            Wx_l = Wx.index_select(1, perm)
-            Wh_l = Wh.index_select(1, perm)                 # [P, 4S]  (K-contiguous for bwd)
-            WhT = Wh_l.t().contiguous()                     # [4S, P]  (K-contiguous for fwd)
-            bias_l = bias.index_select(0, perm)
-        else:
-            Wx_l, Wh_l, bias_l, WhT = Wx, Wh, bias, None
         # W_P^T for the backward chain (dm_t = dh_t W_P^T as a plain NN GEMM): a 2 MB true
         # transpose, 17 us of uncoalesced copy — done here on the side stream, underneath
         # the forward chain, instead of at the head of the backward pass
-        ctx.WPT = None
-        if dev.type == "cuda" and any(ctx.needs_input_grad) and _wpt_side():
+        if any(ctx.needs_input_grad):
             from . import sinks
             cur = torch.cuda.current_stream(dev)
             ws = sinks.side_stream(dev)
@@ -180,7 +103,7 @@ class _LSTMLayerFn(torch.autograd.Function):
                 ctx.WPT_ev = torch.cuda.Event()
                 ctx.WPT_ev.record(ws)
             ctx.WPT.record_stream(cur)
-        xw = torch.addmm(bias_l, x.view(T * Bsz, E), Wx_l).view(T, Bsz, 4 * S)
+        xw = torch.addmm(bias, x.view(T * Bsz, E), Wx).view(T, Bsz, 4 * S)
         act = torch.empty(T, Bsz, 4 * S, dtype=dt, device=dev)
         c_all = torch.empty(T + 1, Bsz, S, dtype=torch.float32, device=dev)
         m_all = torch.empty(T, Bsz, S, dtype=dt, device=dev)
@@ -188,48 +111,27 @@ class _LSTMLayerFn(torch.autograd.Function):
         c_all[0].copy_(c0)
         h_all[0].copy_(h0)
         st = _stream()
-        if tc:
-            for t in range(T):
-                _check(L.px_lstm_gates_tc(_p(h_all[t]), _p(WhT), _p(xw[t]), _p(c_all[t]),
-                                          _p(c_all[t + 1]), _p(m_all[t]), _p(act[t]), Bsz, S, P,
-                                          float(forget_bias), st), "lstm_gates_tc")
-                torch.mm(m_all[t], W_P, out=h_all[t + 1])
-        else:
-            for t in range(T):
-                # accumulate straight into xw[t] (an `out=` different from the addend makes
-                # torch copy the 2 MB addend first — one more launch per step on the
-                # critical path)
-                gpre = xw[t].addmm_(h_all[t], Wh_l)
-                _check(L.px_lstm_cell_fwd(_p(gpre), _p(c_all[t]), _p(act[t]),
-                                          _p(c_all[t + 1]), _p(m_all[t]), Bsz, S,
-                                          float(forget_bias), _DT[dt], st), "lstm_cell_fwd")
-                torch.mm(m_all[t], W_P, out=h_all[t + 1])
+        for t in range(T):
+            # accumulate straight into xw[t] (an `out=` different from the addend makes
+            # torch copy the 2 MB addend first — one more launch per step on the
+            # critical path)
+            gpre = xw[t].addmm_(h_all[t], Wh)
+            _check(L.px_lstm_cell_fwd(_p(gpre), _p(c_all[t]), _p(act[t]),
+                                      _p(c_all[t + 1]), _p(m_all[t]), Bsz, S,
+                                      float(forget_bias), _DT[dt], st), "lstm_cell_fwd")
+            torch.mm(m_all[t], W_P, out=h_all[t + 1])
         _count(T)
-        ctx.save_for_backward(x, Wx_l, Wh_l, W_P, act, c_all, m_all, h_all)
+        ctx.save_for_backward(x, Wx, Wh, W_P, act, c_all, m_all, h_all)
         ctx.dims = (T, Bsz, E, S, P)
-        ctx.tc = tc
-        ctx.Wc = None
-        if (_bwd_fused_w() != "0" and dt == torch.bfloat16 and T > 1 and
-                torch.is_grad_enabled() is False and any(ctx.needs_input_grad)):
-            # combined weight for the backward chain, computed underneath the forward chain
-            from . import sinks
-            cur = torch.cuda.current_stream(dev)
-            ws = sinks.side_stream(dev)
-            ws.wait_stream(cur)
-            with torch.cuda.stream(ws):
-                ctx.Wc = torch.mm(W_P.detach(), Wh_l.detach())          # [S, 4S]
-                ctx.Wc_ev = torch.cuda.Event()
-                ctx.Wc_ev.record(ws)
-            ctx.Wc.record_stream(cur)
         return h_all[1:], c_all[T].clone(), h_all[T].clone()
 
     @staticmethod
     def backward(ctx, dH, dcT, dhT):
         from . import sinks
         L = _lib()
-        x, Wx, Wh, W_P, act, c_all, m_all, h_all = ctx.saved_tensors   # Wx/Wh: layout of `act`
+        x, Wx, Wh, W_P, act, c_all, m_all, h_all = ctx.saved_tensors
         T, Bsz, E, S, P = ctx.dims
-        tc, stacked = ctx.tc, ctx.stacked
+        stacked = ctx.stacked
         W_ref, bias_ref, WP_ref = ctx.param_refs
         dt, dev = x.dtype, x.device
         dH = dH.contiguous()
@@ -239,28 +141,24 @@ class _LSTMLayerFn(torch.autograd.Function):
             else dcT.float().clone()
         dh_rec = None if dhT is None else dhT.to(dt)
         dm = torch.empty(Bsz, S, dtype=dt, device=dev)
-        # dm_t = dh_t @ W_P^T runs as a plain NN GEMM on a materialised W_P^T.
-        if ctx.WPT is not None:
-            torch.cuda.current_stream(dev).wait_event(ctx.WPT_ev)
-            WPT = ctx.WPT
-        else:
-            WPT = W_P.t().contiguous()
+        # dm_t = dh_t @ W_P^T runs as a plain NN GEMM on the W_P^T made in forward.
+        cur = torch.cuda.current_stream(dev)
+        cur.wait_event(ctx.WPT_ev)
+        WPT = ctx.WPT
         # dh_{t-1} = dH_{t-1} + dgates_t @ Wh^T : Wh [P, 4S] is already the
         # K-contiguous "B^T" operand, so this skinny product (M=B, N=P, K=4S)
-        # goes to our wgmma split-K kernel with the +dH addend fused in.
+        # goes to our wgmma split-K kernel with the +dH addend fused in, its 8 K-splits
+        # per tile reducing through DSMEM in a cluster.
         from . import gemm as _gemm
         use_tc = (dt == torch.bfloat16 and Bsz % 128 == 0 and P % 64 == 0 and
                   (4 * S) % 1024 == 0 and Wh.is_contiguous())
-        # K-splits of the dh product: 8 CTAs per tile reducing through DSMEM in a cluster
-        # or 16 through the L2 workspace (LM1B bench step on one H100: 1.42 vs 1.45 ms)
-        ksp = 8 if _gemm.cluster_default() else 16
         WhT = None if use_tc else Wh.t().contiguous()
         st = _stream()
 
         # ---- weight-gradient outputs: the parameters' bucket sinks when a dense group
         # registered them (no pack copy afterwards), else fresh tensors
         def sink_of(ref, shape):
-            s_ = None if tc else sinks.get(ref)
+            s_ = sinks.get(ref)
             if s_ is not None and s_.dtype == dt and tuple(s_.shape) == tuple(shape):
                 return s_, True
             return torch.empty(shape, dtype=dt, device=dev), False
@@ -272,133 +170,49 @@ class _LSTMLayerFn(torch.autograd.Function):
             dWh_o = torch.empty(P, 4 * S, dtype=dt, device=dev)
         dbias_o, b_sunk = sink_of(bias_ref, (4 * S,))
         dWP_o, p_sunk = sink_of(WP_ref, (S, P))
-        # ---- weight-gradient GEMMs on the side stream, cut in time chunks so the earlier
-        # ones run underneath the recurrent chain
-        cur = torch.cuda.current_stream(dev)
         ws = sinks.side_stream(dev)
-        nchunks = _wgrad_chunks(T)
-        bounds = [round(i * T / nchunks) for i in range(nchunks + 1)]   # over t, ascending
-        state = {"first": True}
-        ws2 = sinks.side_stream(dev, 1) if (nchunks == 1 and _dbias_stream()) else None
-        # over several chunks the bias gradient is summed in fp32 and rounded once at the end:
-        # adding chunk sums into the bf16 output rounds it once per chunk
-        dbias_acc = torch.zeros(4 * S, dtype=torch.float32, device=dev) if nchunks > 1 else None
-
-        def wgrad(lo, hi):
-            """accumulate the contribution of steps [lo, hi) (their dgates / dh_tot are final)"""
-            ws.wait_stream(cur)
-            with torch.cuda.stream(ws):
-                dg = dgates[lo:hi].view(-1, 4 * S)
-                hT = h_all[lo:hi].reshape(-1, P).t()
-                xT = x[lo:hi].reshape(-1, E).t()
-                mT = m_all[lo:hi].reshape(-1, S).t()
-                dh2 = dh_tot[lo:hi].view(-1, P)
-                if state["first"]:
-                    torch.mm(hT, dg, out=dWh_o)
-                    torch.mm(xT, dg, out=dWx_o)
-                    if ws2 is None and dbias_acc is None:
-                        torch.sum(dg, 0, out=dbias_o)
-                    torch.mm(mT, dh2, out=dWP_o)
-                    state["first"] = False
-                else:
-                    dWh_o.addmm_(hT, dg)
-                    dWx_o.addmm_(xT, dg)
-                    dWP_o.addmm_(mT, dh2)
-                if dbias_acc is not None:
-                    dbias_acc.add_(dg.sum(0, dtype=torch.float32))
-                    if lo == 0:                 # the last chunk
-                        dbias_o.copy_(dbias_acc)
-        pending_hi = T
-        Wc = ctx.Wc
-        mode = _bwd_fused_w()
+        ws2 = sinks.side_stream(dev, 1)
         if dh_rec is None:
             dh_tot[T - 1].copy_(dH[T - 1])
         else:
             torch.add(dH[T - 1], dh_rec, out=dh_tot[T - 1])
-        if Wc is not None:
-            cur.wait_event(ctx.Wc_ev)
-            fused_tc = (mode == "tc" and Bsz % 128 == 0 and S % 64 == 0 and (4 * S) % 512 == 0)
-            WcT = None if fused_tc else Wc.t()
-            WhT_v = Wh.t()
-            # DMH[t] = dH[t] W_P^T for every step at once (dh_tot[T-1] carries dhT)
-            DMH = torch.empty(T, Bsz, S, dtype=dt, device=dev)
-            torch.mm(dH[:T - 1].reshape(-1, P), WPT, out=DMH[:T - 1].view(-1, S))
-            torch.mm(dh_tot[T - 1], WPT, out=DMH[T - 1])
-
-            def dh_chunk(lo, hi):
-                """dh_tot[lo:hi] (off the critical path; steps whose dgates[t+1] is final)"""
-                top = min(hi, T - 1)
-                if top > lo:
-                    torch.addmm(dH[lo:top].reshape(-1, P),
-                                dgates[lo + 1:top + 1].view(-1, 4 * S), WhT_v,
-                                out=dh_tot[lo:top].view(-1, P))
-            dm_t = DMH[T - 1]
-            for t in range(T - 1, -1, -1):
-                _check(L.px_lstm_cell_bwd(_p(dm_t), _p(dc), _p(act[t]), _p(c_all[t]),
-                                          _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt],
-                                          1 if tc else 0, st), "lstm_cell_bwd")
-                if t > 0:
-                    if fused_tc:
-                        _gemm.gemm_tn(dgates[t], Wc, addend=DMH[t - 1], splits=4, bn=64,
-                                      out=dm)
-                    else:
-                        torch.addmm(DMH[t - 1], dgates[t], WcT, out=dm)
-                    dm_t = dm
-                if t in bounds[1:-1]:
-                    ws.wait_stream(cur)
-                    with torch.cuda.stream(ws):
-                        dh_chunk(t, pending_hi)
-                    wgrad(t, pending_hi)
-                    pending_hi = t
-            dh_rec = _gemm.gemm_tn(dgates[0], Wh, splits=ksp, bn=64) if use_tc \
-                else torch.mm(dgates[0], WhT_v)
-            ws.wait_stream(cur)
-            with torch.cuda.stream(ws):
-                dh_chunk(0, pending_hi)
-            for t_ in (DMH, dH):
-                t_.record_stream(ws)
-        else:
-            for t in range(T - 1, -1, -1):
-                torch.mm(dh_tot[t], WPT, out=dm)
-                _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
-                                          _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt],
-                                          1 if tc else 0, st), "lstm_cell_bwd")
-                if t > 0:
-                    if use_tc:
-                        _gemm.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=ksp, bn=64,
-                                      out=dh_tot[t - 1])
-                    else:
-                        torch.addmm(dH[t - 1], dgates[t], WhT, out=dh_tot[t - 1])
+        for t in range(T - 1, -1, -1):
+            torch.mm(dh_tot[t], WPT, out=dm)
+            _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
+                                      _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt], st),
+                   "lstm_cell_bwd")
+            if t > 0:
+                if use_tc:
+                    _gemm.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=8, bn=64,
+                                  out=dh_tot[t - 1])
                 else:
-                    dh_rec = _gemm.gemm_tn(dgates[0], Wh, splits=ksp, bn=64) if use_tc \
-                        else torch.mm(dgates[0], WhT)
-                if t in bounds[1:-1]:
-                    wgrad(t, pending_hi)
-                    pending_hi = t
+                    torch.addmm(dH[t - 1], dgates[t], WhT, out=dh_tot[t - 1])
+            else:
+                dh_rec = _gemm.gemm_tn(dgates[0], Wh, splits=8, bn=64) if use_tc \
+                    else torch.mm(dgates[0], WhT)
         _count(T)
         dg2 = dgates.view(T * Bsz, 4 * S)
+        # the bias gradient, a bandwidth-bound column sum, runs on a second side stream next
+        # to the compute-bound weight-gradient GEMMs
+        ws2.wait_stream(cur)
+        with torch.cuda.stream(ws2):
+            torch.sum(dg2, 0, out=dbias_o)
+        ev_b = torch.cuda.Event()
+        ev_b.record(ws2)
+        dgates.record_stream(ws2)
+        dbias_o.record_stream(ws2)
         # dx first: the embedding gradient is what the rest of backward (and the sparse
-        # push) is waiting for; the last weight-gradient chunk goes to the side stream
-        ev_b = None
-        if ws2 is not None:
-            # bandwidth-bound column sum: runs next to the compute-bound GEMMs below
-            ws2.wait_stream(cur)
-            with torch.cuda.stream(ws2):
-                torch.sum(dg2, 0, out=dbias_o)
-            ev_b = torch.cuda.Event()
-            ev_b.record(ws2)
-            dgates.record_stream(ws2)
-            dbias_o.record_stream(ws2)
+        # push) is waiting for; the weight-gradient GEMMs go to the side stream
         dx = (dg2 @ Wx.t()).view(T, Bsz, E)
-        wgrad(0, pending_hi)
+        ws.wait_stream(cur)
+        with torch.cuda.stream(ws):
+            torch.mm(h_all[:T].reshape(-1, P).t(), dg2, out=dWh_o)
+            torch.mm(x.reshape(-1, E).t(), dg2, out=dWx_o)
+            torch.mm(m_all.reshape(-1, S).t(), dh_tot.view(-1, P), out=dWP_o)
         ev = torch.cuda.Event()
         ev.record(ws)
-        if ev_b is None:
-            ev_b = ev
         for t_ in (dgates, dh_tot, x, h_all, m_all, dWh_o, dWx_o, dbias_o, dWP_o):
             t_.record_stream(ws)
-        if dbias_acc is not None:
-            dbias_acc.record_stream(ws)
         outs, plain = [], False
         for ref, o, sunk, e_ in ((W_ref, dW if stacked else dWx_o, w_sunk, ev),
                                  (bias_ref, dbias_o, b_sunk, ev_b), (WP_ref, dWP_o, p_sunk, ev)):
@@ -413,18 +227,9 @@ class _LSTMLayerFn(torch.autograd.Function):
                 plain = True
         if plain or not stacked:
             cur.wait_event(ev)        # plain tensors are consumed on the current stream
-            if ev_b is not ev:
-                cur.wait_event(ev_b)
+            cur.wait_event(ev_b)
         dW_out, dbias, dW_P = outs
-        dWh = None if stacked else dWh_o
-        if tc:          # back to the caller's (plain) gate-column order
-            _, inv = gate_interleave_perm(S, dev)
-            if stacked:
-                dW_out = dW_out.index_select(1, inv)      # (tc path never uses sinks)
-            else:
-                dW_out, dWh = dW_out.index_select(1, inv), dWh.index_select(1, inv)
-            dbias = dbias.index_select(0, inv)
-        return dx, dW_out, dWh, dbias, dW_P, dc, dh_rec, None
+        return dx, dW_out, None if stacked else dWh_o, dbias, dW_P, dc, dh_rec, None
 
 
 def lstm_layer(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
@@ -509,12 +314,6 @@ def sampled_softmax_loss(inputs, true_w, samp_w, true_b, samp_b, logq_true, logq
 # ---------------------------------------------------------------------------
 # the whole loss head as one node
 # ---------------------------------------------------------------------------
-def _head_enabled():
-    """PARALLAX_SSM_HEAD=0 falls back to `sampled_softmax_loss` + PyTorch glue."""
-    import os
-    return os.environ.get("PARALLAX_SSM_HEAD", "1") != "0"
-
-
 def _head_forward(inputs, w_all, adj, targets, sampled):
     """-> (probs [N,S] in inputs.dtype, loss [N] fp32, dtrue [N] fp32).  `w_all` holds the
     N true-class rows followed by the S sampled rows; `adj` = bias - log Q for the same
@@ -621,7 +420,7 @@ def sampled_softmax_head(inputs, w_all, b_all, logq, targets, sampled, row_w=Non
     S = w_all.shape[0] - N
     dt = inputs.dtype
     vec = 4 if dt == torch.float32 else 8
-    fused = (inputs.is_cuda and _head_enabled() and dt in _DT and w_all.dtype == dt and
+    fused = (inputs.is_cuda and dt in _DT and w_all.dtype == dt and
              0 < S <= 256 * 64 and P % vec == 0 and b_all.numel() == N + S)
     if fused:
         inputs = inputs.contiguous()

@@ -47,14 +47,7 @@ def supported(A, Bt):
             A.data_ptr() % 16 == 0 and Bt.data_ptr() % 16 == 0)
 
 
-def cluster_default():
-    """Split-K reduction through distributed shared memory (thread-block cluster of the K-splits)
-    instead of L2 atomics + ticket + read-back; `PARALLAX_GEMM_CLUSTER=0` selects the latter."""
-    import os
-    return os.environ.get("PARALLAX_GEMM_CLUSTER", "1") != "0"
-
-
-def gemm_tn(A, Bt, addend=None, splits=None, out=None, bn=None, cluster=None):
+def gemm_tn(A, Bt, addend=None, splits=None, out=None, bn=None, cluster=True):
     M, K = A.shape
     N = Bt.shape[0]
     assert Bt.shape[1] == K
@@ -64,8 +57,8 @@ def gemm_tn(A, Bt, addend=None, splits=None, out=None, bn=None, cluster=None):
         splits = pick_splits(M, N, K, bn)
     if out is None:
         out = torch.empty(M, N, dtype=torch.bfloat16, device=A.device)
-    if cluster is None:
-        cluster = cluster_default()
+    # cluster: split-K reduction through distributed shared memory (a thread-block cluster of
+    # the K-splits) where the split count allows it, else L2 atomics + ticket + read-back
     cluster = bool(cluster) and 2 <= splits <= 16 and 128 % splits == 0
     ws = tk = None
     if splits > 1 and not cluster:

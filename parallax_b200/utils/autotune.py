@@ -80,8 +80,8 @@ class EngineAutotuner(object):
     graph replays — so the numbers the tuner sees are the numbers the job will run at.
     Knobs: CTAs of the dense comm kernels, CTA cap of the sparse kernels (continuous,
     GP/EI), then the schedule switches one by one (categorical): sparse push from inside
-    backward vs after it, last dense bucket held back behind the sparse push or not,
-    time-chunking of the weight-gradient GEMMs on the side stream.  Rank 0 decides; values
+    backward vs after it, last dense bucket held back behind the sparse push or not.  Every
+    knob is an attribute of the engine, its fabric or its groups.  Rank 0 decides; values
     are broadcast so every rank applies the same setting at the same step."""
     MEASURE = 8
 
@@ -89,8 +89,7 @@ class EngineAutotuner(object):
         self.engine = engine
         self.tuner = BayesianTuner(
             {"comm_blocks": (4.0, 128.0), "sparse_blocks": (16.0, 296.0)},
-            categorical={"early_push": [True, False], "defer_last": [True, False],
-                         "wgrad_chunks": [1, 2, 4]},
+            categorical={"early_push": [True, False], "defer_last": [True, False]},
             samples_per_point=1, warmups=0, max_points=10) if engine.comm.rank == 0 else None
         self.log = os.environ.get(PARALLAX_AUTOTUNE_LOG)
         self.done = False
@@ -120,7 +119,6 @@ class EngineAutotuner(object):
             grp.early_push = bool(vals["early_push"])
         if eng.dense is not None:
             eng.dense.defer_last = bool(vals["defer_last"])
-        os.environ["PARALLAX_LSTM_WGRAD_CHUNKS"] = str(vals["wgrad_chunks"])
         self.current = {k: v for k, v in vals.items() if k != "done"}
         self.done = bool(vals["done"])
         # the captured graph (if any) bakes the old grids / schedule in: capture again

@@ -33,13 +33,9 @@ def test_lstm_layer_matches_reference(dtype, tol):
             (float((r - g).abs().max()), scale)
 
 
-@pytest.mark.parametrize("tc_fwd", ["0", "1"])
-def test_lstm_layer_bf16_wgmma_backward_path(tc_fwd, monkeypatch):
+def test_lstm_layer_bf16_wgmma_backward_path():
     """B=128, 4S multiple of 1024: the recurrent backward product runs on the
-    wgmma split-K kernel with the fused addend; with PARALLAX_LSTM_TC_FWD=1 the
-    forward step runs on the wgmma kernel with the LSTM cell fused in its
-    epilogue (gate-interleaved layout)."""
-    monkeypatch.setenv("PARALLAX_LSTM_TC_FWD", tc_fwd)
+    wgmma split-K kernel with the fused addend."""
     from parallax_b200.ops.fused import lstm_layer, lstm_layer_reference
     torch.manual_seed(0)
     T, B, E, S, P = 3, 128, 64, 256, 64

@@ -36,7 +36,8 @@ _EXACT = [
     # the products of ops/fused.py at the LM1B bench shape (B 128, P 512, S 2048):
     # dh_{t-1} = dH_{t-1} + dgates_t·Wh^T over 8 cluster splits or 16 L2 splits
     (128, 512, 8192, 8, 64, True), (128, 512, 8192, 16, 64, True),
-    # PARALLAX_LSTM_BWD_FUSEDW=tc: dm = DMH + dgates·Wc^T
+    # a wide output (N 2048) over 4 splits: the shape of dm = dH·W_P^T + dgates·(W_P·Wh)^T,
+    # one product per step with the combined weight (tools/bench_lstm_gemms.py times it)
     (128, 2048, 8192, 4, 64, True),
     # dh_rec of the first step: no addend
     (128, 512, 8192, 8, 64, False), (128, 512, 8192, 16, 64, False),

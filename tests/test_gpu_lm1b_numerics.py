@@ -156,13 +156,9 @@ def test_lstm_cell_fwd_kernel_vs_fp64(dt, B, S, fb):
 
 @pytest.mark.parametrize("dt", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("B,S", _CELL_SHAPES)
-@pytest.mark.parametrize("interleaved", [0, 1])
-def test_lstm_cell_bwd_kernel_vs_fp64(dt, B, S, interleaved):
-    if interleaved and S % 32:
-        pytest.skip("the gate-interleaved layout tiles 32 units")
-    from parallax_b200.ops.fused import gate_interleave_perm
+def test_lstm_cell_bwd_kernel_vs_fp64(dt, B, S):
     L = _lib()
-    gen = _gen(B + S + interleaved)
+    gen = _gen(B + S)
     act = torch.cat([torch.sigmoid(_pre_activations(B, S, torch.float32, seed=S)[:, :S]),
                      torch.tanh(torch.randn(B, S, device="cuda", generator=gen) * 2),
                      torch.sigmoid(torch.randn(B, S, device="cuda", generator=gen) * 3 + 1),
@@ -172,18 +168,11 @@ def test_lstm_cell_bwd_kernel_vs_fp64(dt, B, S, interleaved):
     cn.view(-1)[::9] = 30.0                                # tanh(c) = 1: 1 − tanh² cancels
     dm = (torch.randn(B, S, device="cuda", generator=gen) * 0.5).to(dt)
     dc_in = torch.randn(B, S, device="cuda", generator=gen) * 0.5
-    if interleaved:
-        perm, inv = gate_interleave_perm(S, "cuda")
-        act_k = act.index_select(1, perm).contiguous()
-    else:
-        act_k = act
     dc = dc_in.clone()
     dg = torch.empty(B, 4 * S, dtype=dt, device="cuda")
-    assert L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act_k), _p(cp), _p(cn), _p(dg), B, S,
-                              0 if dt == torch.float32 else 1, interleaved, _stream()) == 0
+    assert L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act), _p(cp), _p(cn), _p(dg), B, S,
+                              0 if dt == torch.float32 else 1, _stream()) == 0
     torch.cuda.synchronize()
-    if interleaved:
-        dg = dg.index_select(1, inv)
     si, tj, sf, so = act.double().split(S, dim=1)
     tc = torch.tanh(cn.double())
     dmv = dm.double()
@@ -196,68 +185,7 @@ def test_lstm_cell_bwd_kernel_vs_fp64(dt, B, S, interleaved):
 
 
 # ===========================================================================
-# fused wgmma gates kernel (PARALLAX_LSTM_TC_FWD=1), called directly
-# ===========================================================================
-def _run_gates_tc(h, Wh, xw, cp, fb):
-    """Plain-layout operands in; the kernel sees the gate-interleaved layout.  Returns its
-    (act in plain column order, c_new, m)."""
-    from parallax_b200.ops.fused import gate_interleave_perm
-    L = _lib()
-    M, K = h.shape
-    S = cp.shape[1]
-    perm, inv = gate_interleave_perm(S, "cuda")
-    WhP = Wh.index_select(1, perm).t().contiguous()        # [4S, K], K-contiguous
-    xw_l = xw.index_select(1, perm).contiguous()
-    c_new = torch.empty(M, S, device="cuda")
-    m = torch.empty(M, S, dtype=torch.bfloat16, device="cuda")
-    act = torch.empty(M, 4 * S, dtype=torch.bfloat16, device="cuda")
-    assert L.px_lstm_gates_tc(_p(h), _p(WhP), _p(xw_l), _p(cp), _p(c_new), _p(m), _p(act),
-                              M, S, K, fb, _stream()) == 0
-    torch.cuda.synchronize()
-    return act.index_select(1, inv), c_new, m
-
-
-@pytest.mark.parametrize("M", [128, 256])
-@pytest.mark.parametrize("S", [256, 2048])
-@pytest.mark.parametrize("K", [64, 512, 1024])
-@pytest.mark.parametrize("fb", [0.0, 1.0])
-def test_lstm_gates_tc_exact_product_vs_fp64(M, S, K, fb):
-    """h and Wh are small multiples of 2^-4: the product is exact in fp32, so every output
-    meets the cell kernel's elementwise bounds."""
-    gen = _gen(M + S + K)
-    h = (torch.randint(-2, 3, (M, K), device="cuda", generator=gen) / 16.0).bfloat16()
-    Wh = (torch.randint(-2, 3, (K, 4 * S), device="cuda", generator=gen) / 16.0).bfloat16()
-    xw = torch.randn(M, 4 * S, device="cuda", generator=gen).bfloat16()
-    cp = torch.randn(M, S, device="cuda", generator=gen) * 2.0
-    act, c_new, m = _run_gates_tc(h, Wh, xw, cp, fb)
-    act64, c64, m64 = _cell_fwd64(h.double() @ Wh.double() + xw.double(), cp, fb)
-    sc = 1.0 + cp.double().abs()
-    _assert_elementwise("act", act, act64, 1.0, torch.bfloat16)
-    _assert_elementwise("c_new", c_new, c64, sc, torch.float32)
-    _assert_elementwise("m", m, m64, sc, torch.bfloat16)
-
-
-def test_lstm_gates_tc_random_vs_fp64():
-    """Random operands: the bounds widen by the fp32 accumulation error of the product,
-    2^-16·(|h|·|Wh|), propagated through the cell (|σ'|, |tanh'| <= 1)."""
-    M, S, K, fb = 128, 2048, 512, 1.0
-    gen = _gen(5)
-    h = (torch.randn(M, K, device="cuda", generator=gen) * 0.5).bfloat16()
-    Wh = (torch.randn(K, 4 * S, device="cuda", generator=gen) * 0.05).bfloat16()
-    xw = torch.randn(M, 4 * S, device="cuda", generator=gen).bfloat16()
-    cp = torch.randn(M, S, device="cuda", generator=gen) * 2.0
-    act, c_new, m = _run_gates_tc(h, Wh, xw, cp, fb)
-    act64, c64, m64 = _cell_fwd64(h.double() @ Wh.double() + xw.double(), cp, fb)
-    perr = 2.0 ** -16 * (h.double().abs() @ Wh.double().abs())
-    pu = sum(perr.split(S, dim=1))
-    sc_c = (1.0 + cp.double().abs()) * (1.0 + 1e6 * pu)
-    _assert_elementwise("act", act, act64, 1.0 + 1e6 * perr, torch.bfloat16)
-    _assert_elementwise("c_new", c_new, c64, sc_c, torch.float32)
-    _assert_elementwise("m", m, m64, sc_c, torch.bfloat16)
-
-
-# ===========================================================================
-# whole layer at the bench shape, every scheduling / kernel variant
+# whole layer at the bench shape
 # ===========================================================================
 B_, E_, S_, P_ = 128, 512, 2048, 512
 _NAMES = ["H", "cT", "hT", "dx", "dW", "dbias", "dW_P", "dc0", "dh0"]
@@ -309,58 +237,41 @@ def _layer_refs(T):
     return _ref_cache[T]
 
 
-_VARIANTS = {
-    "default": {},
-    "l2_splitk": {"PARALLAX_GEMM_CLUSTER": "0"},
-    "tc_fwd": {"PARALLAX_LSTM_TC_FWD": "1"},
-    "fusedw_tc": {"PARALLAX_LSTM_BWD_FUSEDW": "tc"},
-    "fusedw_cublas": {"PARALLAX_LSTM_BWD_FUSEDW": "cublas"},
-    "wgrad_chunks2": {"PARALLAX_LSTM_WGRAD_CHUNKS": "2"},
-    "wgrad_chunks3": {"PARALLAX_LSTM_WGRAD_CHUNKS": "3"},
-    "dbias_same_stream": {"PARALLAX_LSTM_DBIAS_STREAM": "0"},
-    "wpt_in_backward": {"PARALLAX_LSTM_WPT_SIDE": "0"},
-}
-
-
 @pytest.mark.parametrize("kind", ["plain", "stacked"])
-@pytest.mark.parametrize("variant", list(_VARIANTS))
-def test_lstm_layer_variants_vs_fp64(kind, variant, monkeypatch):
-    """B 128, E 512, S 2048, P 512 (the bench layer), T 4 (T 6 for three weight-gradient
-    chunks): outputs and every input gradient against fp64."""
-    for k, v in _VARIANTS[variant].items():
-        monkeypatch.setenv(k, v)
-    T = 6 if variant == "wgrad_chunks3" else 4
-    inp, ref, low = _layer_refs(T)
+def test_lstm_layer_vs_fp64(kind):
+    """B 128, E 512, S 2048, P 512 (the bench layer), T 4: outputs and every input gradient
+    against fp64."""
+    inp, ref, low = _layer_refs(4)
     got = _run_layer(kind, inp, torch.bfloat16)
     for name, g, r, lo in zip(_NAMES, got, ref, low):
-        _assert_calibrated("%s/%s/%s" % (kind, variant, name), g, r, lo, torch.bfloat16,
+        _assert_calibrated("%s/%s" % (kind, name), g, r, lo, torch.bfloat16,
                            _FACTOR_OF.get(name, FACTOR))
 
 
 def test_lstm_layer_schedule_variants_bit_identical(monkeypatch):
-    """Moving the W_P transpose or the bias sum to another stream changes no arithmetic, and the
-    cluster split-K reduction has a fixed order: these runs agree bit for bit.  A missing stream
-    wait shows up here as a difference."""
+    """With every side stream replaced by the current stream (the W_P transpose, the bias sum
+    and the weight-gradient GEMMs run in program order) the layer computes the same bits: the
+    streams change no arithmetic and the cluster split-K reduction has a fixed order.  A
+    missing stream wait shows up here as a difference."""
+    from parallax_b200.ops import sinks
     inp, _, _ = _layer_refs(4)
     base = _run_layer("stacked", inp, torch.bfloat16)
-    for env in ({}, {"PARALLAX_LSTM_WPT_SIDE": "0"}, {"PARALLAX_LSTM_DBIAS_STREAM": "0"}):
+    for serial in (False, True):
         with monkeypatch.context() as mp:
-            for k, v in env.items():
-                mp.setenv(k, v)
+            if serial:
+                mp.setattr(sinks, "side_stream",
+                           lambda device, which=0: torch.cuda.current_stream(device))
             got = _run_layer("stacked", inp, torch.bfloat16)
         for name, a, b in zip(_NAMES, base, got):
             assert torch.equal(a.reshape(-1).view(torch.uint8), b.reshape(-1).view(torch.uint8)), \
-                (env, name)
+                (serial, name)
 
 
-@pytest.mark.parametrize("variant", ["default", "wgrad_chunks2", "dbias_same_stream"])
-def test_lstm_layer_stacked_writes_bucket_sinks(variant, monkeypatch):
+def test_lstm_layer_stacked_writes_bucket_sinks():
     """The model's path: the weight gradients go straight into views of one gradient bucket on
     the side streams, autograd gets None for those parameters, and the bucket bytes around
     the views keep their bits."""
     from parallax_b200.ops import fused, sinks
-    for k, v in _VARIANTS[variant].items():
-        monkeypatch.setenv(k, v)
     inp, ref, low = _layer_refs(4)
     x, W, b, WP, h0 = (_leaf(inp[k], torch.bfloat16) for k in ("x", "W", "b", "WP", "h0"))
     c0 = _leaf(inp["c0"], torch.float32)
@@ -392,7 +303,7 @@ def test_lstm_layer_stacked_writes_bucket_sinks(variant, monkeypatch):
     got = {"dx": x.grad, "dW": views[0], "dbias": views[1], "dW_P": views[2], "dc0": c0.grad,
            "dh0": h0.grad, "H": H.detach(), "cT": cT.detach(), "hT": hT.detach()}
     for i, name in enumerate(_NAMES):
-        _assert_calibrated("sinks/%s/%s" % (variant, name), got[name], ref[i], low[i],
+        _assert_calibrated("sinks/%s" % name, got[name], ref[i], low[i],
                            torch.bfloat16, _FACTOR_OF.get(name, FACTOR))
     bits = bucket.view(torch.int16)
     keep = torch.ones_like(bits, dtype=torch.bool)
@@ -402,7 +313,7 @@ def test_lstm_layer_stacked_writes_bucket_sinks(variant, monkeypatch):
 
 
 # ===========================================================================
-# sampled softmax: the fused head and the PARALLAX_SSM_HEAD=0 path
+# sampled softmax: the fused head and the `sampled_softmax_loss` composition
 # ===========================================================================
 _V = 100000
 _SSM_SHAPES = ([(2560, 8192, 512)] + [(256, 1024, p) for p in (8, 64, 520)] +
@@ -444,16 +355,16 @@ def _ssm_objective(entry, inputs, w_all, b_all, logq, targets, sampled, rw):
                                                logq[:N], logq[N:], targets, sampled)
         obj = (rows * rw if rw is not None else rows).mean()
         return obj, rows, None
+    if entry == "loss":
+        b = b_all.reshape(-1)
+        rows = fused.sampled_softmax_loss(inputs, w_all[:N], w_all[N:], b[:N], b[N:],
+                                          logq[:N], logq[N:], targets, sampled)
+        obj = (rows * rw if rw is not None else rows).mean()
+        return obj, rows, None
     obj = fused.sampled_softmax_head(inputs, w_all, b_all, logq, targets, sampled, row_w=rw)
-    if entry == "head":
-        assert obj.grad_fn.name().startswith("_SampledSoftmaxHeadFn") or \
-            w_all.shape[0] - N > 256 * 64
+    assert obj.grad_fn.name().startswith("_SampledSoftmaxHeadFn") or \
+        w_all.shape[0] - N > 256 * 64
     with torch.no_grad():
-        if entry == "loss":
-            b = b_all.reshape(-1)
-            rows = fused.sampled_softmax_loss(inputs, w_all[:N], w_all[N:], b[:N], b[N:],
-                                              logq[:N], logq[N:], targets, sampled)
-            return obj, rows, None
         if w_all.shape[0] - N > 256 * 64:
             return obj, None, None
         adj = b_all.reshape(-1).float() - logq
@@ -488,9 +399,7 @@ def _ssm_run(entry, data, dt, bdt, rw):
                                     (torch.bfloat16, torch.float32),
                                     (torch.bfloat16, torch.bfloat16)])
 @pytest.mark.parametrize("weighted", [False, True])
-def test_sampled_softmax_vs_fp64(N, S, P, entry, dt, bdt, weighted, monkeypatch):
-    if entry == "loss":
-        monkeypatch.setenv("PARALLAX_SSM_HEAD", "0")
+def test_sampled_softmax_vs_fp64(N, S, P, entry, dt, bdt, weighted):
     data = _ssm_rounded(_ssm_inputs(N, S, P, seed=N + S + P), dt, bdt)
     rw = torch.rand(N, device="cuda", generator=_gen(9)) if weighted else None
     ref = _ssm_run("reference", data, torch.float64, torch.float64, rw)
@@ -534,10 +443,7 @@ def test_sampled_softmax_all_sampled_hit_row_and_extreme_offsets(dt, S):
     ref = _ssm_run("reference", data, torch.float64, torch.float64, None)
     low = _ssm_run("reference", data, dt, dt, None)
     for entry in ("head", "loss"):
-        with pytest.MonkeyPatch.context() as mp:
-            if entry == "loss":
-                mp.setenv("PARALLAX_SSM_HEAD", "0")
-            got = _ssm_run(entry, data, dt, dt, None)
+        got = _ssm_run(entry, data, dt, dt, None)
         assert float(got["rows"][0]) == 0.0
         for k in got:
             _assert_calibrated("extreme/%s/%s" % (entry, k), got[k], ref[k], low[k], dt)
