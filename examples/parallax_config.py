@@ -37,6 +37,11 @@ def add_flags(ap):
     # scales the embedding gradients by it (ScaleGradients), and its 1/K weighting expects it.
     ap.add_argument("--micro_batches", type=int, default=1,
                     help="forward/backward passes per optimizer step (gradient accumulation)")
+    # how parallax.nn.full_softmax_nll trains (LM1B with num_sampled=0): "fused" needs the
+    # NVLink fabric and --compute_dtype bf16
+    ap.add_argument("--full_softmax_train", default="composition",
+                    choices=["composition", "fused"],
+                    help="full-softmax training: gather + matmul composition, or fused kernels")
     return ap
 
 
@@ -61,6 +66,8 @@ def build_config(FLAGS):
         sc["cuda_graph"] = True
     if getattr(FLAGS, "micro_batches", 1) != 1:
         sc["micro_batches"] = FLAGS.micro_batches
+    if getattr(FLAGS, "full_softmax_train", "composition") != "composition":
+        sc["full_softmax_train"] = FLAGS.full_softmax_train
     cfg = parallax.Config()
     cfg.run_option = FLAGS.run_option
     cfg.average_sparse = FLAGS.average_sparse

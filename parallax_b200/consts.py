@@ -108,6 +108,10 @@ NUM_SMS = 132
 # bound on the per-CTA top-k lists of one fused full-softmax top-k launch (NUM_SMS · rows · k
 # 8-byte entries); larger batches are evaluated in row chunks, each reading the table once
 TOPK_WS_BYTES = 48 << 20
+# bound on the chunk scratch of the fused full-softmax backward (sess_config
+# ["full_softmax_train"] = "fused"): the gathered rows and the bf16 [N, Vc] softmax gradient of
+# one vocabulary chunk of Vc rows
+FULL_SOFTMAX_TRAIN_WS_BYTES = 256 << 20
 
 RUN_OPTIONS = ("PS", "MPI", "HYBRID")
 # "AR" is accepted as a modern alias of the reference's "MPI" run option.

@@ -137,8 +137,13 @@ def full_softmax_nll(inputs, targets, weight, bias):
     they form a co-lookup group on the NVLink fabric with a bf16 weight shadow, inputs are bf16
     with K % 8 == 0 and K <= 512, and no gradient is wanted, one fused kernel evaluates the
     softmax where the rows live (no gathered table, no [N, V] logits, fp32 logits; a target
-    outside [0, V) gives NaN in its row).  Otherwise the table is gathered and the logits
-    materialised, which also carries gradients to the tables."""
+    outside [0, V) gives NaN in its row).  Under the same conditions in training, a session
+    with ``sess_config["full_softmax_train"] = "fused"`` also runs the forward fused and a
+    fused backward: the table is recomputed in vocabulary chunks of bounded scratch, the
+    softmax gradient is bf16, and `inputs` and the tables get their gradients (the tables'
+    as every row, through the same push and owner kernels as a lookup's).  Otherwise the
+    table is gathered and the logits materialised, which also carries gradients to the
+    tables."""
     if inputs.dim() != 2:
         raise ValueError("inputs must be [N, K], got shape %s" % (tuple(inputs.shape),))
     if targets.dim() != 1 or targets.shape[0] != inputs.shape[0]:

@@ -96,7 +96,10 @@ _SIGS = {
     "px_full_softmax_nll": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                     c_int, c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
                                     c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
-                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "px_full_softmax_grad": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                     c_int, c_int, ctypes.c_longlong, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "px_full_softmax_topk": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                      c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(GroupGeom),
                                      c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,

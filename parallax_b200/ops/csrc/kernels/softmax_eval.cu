@@ -28,6 +28,13 @@
 // the n largest keys of a row are n draws without replacement from softmax(s), in draw order.
 // The combine recovers s of each kept entry from its key and writes s − lse.
 //
+// Training (px_full_softmax_grad): the log-sum-exp instantiations with GRAD = true take one
+// gathered chunk of the table, global ids [v0, v0 + rows), as a one-owner, one-slot table and
+// recompute its biased logits s.  The epilogue writes G = g_i · (exp(s − lse_i) − [v == t_i]) in
+// bf16 into a [N, ·] chunk buffer and the column sums of G (the bias gradient, fp32) of the
+// CTA's block: a CTA streams every X tile over its block, so the sums are complete in the CTA.
+// The caller multiplies G into dX = G·W_c and dW_c = Gᵀ·X.
+//
 // One-sided like the lookup: peers' rows are read over NVLink with 16-byte loads; nothing is
 // exchanged, so a rank may evaluate alone.  In sync mode the kernel first waits applied[o] >=
 // completed steps on the group header (the lookup's freshness rule).
@@ -76,9 +83,25 @@ struct SampleArgs : TopkArgs {
   uint32_t seed;
   int row0;                         // index of X's row 0 within the caller's batch (chunking)
 };
-template <int KC, bool SAMPLE = false>
+// the gradient kernels' arguments (KC == 0): the chunk's rows replace w, b and row_cnt
+struct GradArgs : EvalArgs {
+  const __nv_bfloat16* wc;          // [rows] bf16 weight rows of the chunk, pitch w_pitch
+  const void* bc;                   // [rows] bias rows of the chunk, pitch b_pitch
+  int rows;                         // real rows of the chunk
+  long long v0;                     // global id of the chunk's row 0
+  const float* lse;                 // [N] each row's log-sum-exp from the forward
+  const float* g;                   // [N] gradient of each row's NLL
+  const long long* targets;         // [N]
+  __nv_bfloat16* G;                 // [N][g_pitch] out: g_i · (softmax − onehot) of the chunk
+  int g_pitch;                      // >= the chunk's blocks · BV, even
+  float* db;                        // [rows] out: column sums of G
+};
+template <int KC, bool SAMPLE = false, bool GRAD = false>
 using EvalParams = typename std::conditional<
-    KC == 0, EvalArgs, typename std::conditional<SAMPLE, SampleArgs, TopkArgs>::type>::type;
+    GRAD, GradArgs,
+    typename std::conditional<
+        KC == 0, EvalArgs,
+        typename std::conditional<SAMPLE, SampleArgs, TopkArgs>::type>::type>::type;
 
 __device__ __forceinline__ bool tk_beats(float v, int id, float v2, int id2) {
   return v > v2 || (v == v2 && id < id2);
@@ -97,6 +120,17 @@ __device__ __forceinline__ bool ev_row_real(const EvalArgs& a, const int* cnt, i
   return lr < a.slots * a.rows_per_part &&
          (lr % a.rows_per_part) < __ldg(cnt + lr / a.rows_per_part);
 }
+__device__ __forceinline__ bool ev_row_real(const GradArgs& a, const int*, int lr) {
+  return lr < a.rows;
+}
+
+// an owner's weight and bias rows; the gradient kernels' one owner is the gathered chunk
+__device__ __forceinline__ const __nv_bfloat16* ev_wsrc(const EvalArgs& a, int owner) {
+  return a.w[owner];
+}
+__device__ __forceinline__ const __nv_bfloat16* ev_wsrc(const GradArgs& a, int) { return a.wc; }
+__device__ __forceinline__ const void* ev_bsrc(const EvalArgs& a, int owner) { return a.b[owner]; }
+__device__ __forceinline__ const void* ev_bsrc(const GradArgs& a, int) { return a.bc; }
 
 // Roles as in gemm_tc.cu: warpgroup 0 produces (thread 0 issues the X TMA loads), warpgroups
 // 1 and 2 each own 64 rows of the 128-row X tile and run wgmma m64×BV×16 against the resident
@@ -172,10 +206,12 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
 
 // BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows).  KC: top-k list
 // capacity (0: log-sum-exp only; else k <= KC and the top-k epilogue runs).  SAMPLE (KC > 0):
-// the lists rank Gumbel keys of the tempered logits instead of the logits
-template <typename BiasT, int KC, bool SAMPLE = false>
+// the lists rank Gumbel keys of the tempered logits instead of the logits.  GRAD (KC == 0): the
+// gradient epilogue over one gathered chunk instead of the (max, Σexp) pairs
+template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false>
 __global__ void __launch_bounds__(THREADS, 1)
-px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParams<KC, SAMPLE> a) {
+px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
+                           EvalParams<KC, SAMPLE, GRAD> a) {
   constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -186,6 +222,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
   uint64_t* empty_bar = full_bar + EV_STAGES;
   int* s_gid = reinterpret_cast<int*>(empty_bar + EV_STAGES);      // [BV] (KC > 0)
   TopkEntry* s_cand = reinterpret_cast<TopkEntry*>(s_gid + BV);   // [256 / 4 quads][2][KC]
+  float* s_db = reinterpret_cast<float*>(s_gid);                  // [BV] (GRAD)
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
@@ -210,7 +247,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
     const int owner = a.replicated ? a.rank : (a.rank + oi) % a.W;
     const int* cnt = a.row_cnt + (a.replicated ? 0 : owner) * a.slots;
     const int r0 = (item % a.nblk) * BV;
-    const __nv_bfloat16* src = a.w[owner];
+    const __nv_bfloat16* src = ev_wsrc(a, owner);
     __syncthreads();                            // every wgmma on the previous block has retired
     // table block -> shared memory, 128B-swizzled K-major (chunk c of row r at c ^ (r % 8));
     // padding rows and columns beyond K are zero.  Eight loads in flight per thread.
@@ -238,8 +275,9 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
       const int lr = r0 + threadIdx.x;
       float bv = -INFINITY;
       if (ev_row_real(a, cnt, lr))
-        bv = ev_bias(reinterpret_cast<const BiasT*>(a.b[owner]) + (size_t)lr * a.b_pitch);
+        bv = ev_bias(reinterpret_cast<const BiasT*>(ev_bsrc(a, owner)) + (size_t)lr * a.b_pitch);
       s_bias[threadIdx.x] = bv;
+      if constexpr (GRAD) s_db[threadIdx.x] = 0.f;
       if constexpr (KC > 0) {
         int gid = INT_MAX;
         if (bv != -INFINITY) {
@@ -268,6 +306,11 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
       const bool leader = (threadIdx.x & 127) == 0;
       const int lane = threadIdx.x & 31;
       const int cq = (lane & 3) * 2;
+      float colsum[GRAD ? BV / 4 : 1];        // GRAD: the lane's columns of G summed over rows
+      if constexpr (GRAD) {
+#pragma unroll
+        for (int i = 0; i < BV / 4; ++i) colsum[i] = 0.f;
+      }
       for (int mt = 0; mt < m_tiles; ++mt) {
         float acc[BV / 2];
         for (int kb = 0; kb < a.kb; ++kb, ++it) {
@@ -289,61 +332,105 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x, EvalParam
         // epilogue: a quad of lanes holds all BV columns of 2 rows (acc[j·4 + 2h + e] is row
         // lane/4 + 8h, column j·8 + (lane%4)·2 + e of the warp's 16 rows)
         const int rbase = mt * BM + cw * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
+        if constexpr (GRAD) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float mx = -INFINITY;
+          for (int h = 0; h < 2; ++h) {
+            const int row = rbase + 8 * h;
+            const bool rv = row < a.N;
+            // rows past N (zero-filled X) contribute nothing: g = 0, no store
+            const float nl2 = rv ? -__ldg(a.lse + row) * EV_LOG2E : 0.f;
+            const float gr = rv ? __ldg(a.g + row) : 0.f;
+            const long long tc = rv ? __ldg(a.targets + row) - (a.v0 + r0) : -1;
+            __nv_bfloat16* grow = a.G + (size_t)row * a.g_pitch + r0 + cq;
 #pragma unroll
-          for (int j = 0; j < BV / 8; ++j)
+            for (int j = 0; j < BV / 8; ++j) {
+              float gv[2];
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              float& v = acc[j * 4 + 2 * h + e];
-              v += s_bias[j * 8 + cq + e];
-              if constexpr (SAMPLE) v *= a.inv_tau;
-              mx = fmaxf(mx, v);
+              for (int e = 0; e < 2; ++e) {
+                const int c = j * 8 + cq + e;
+                const float b = s_bias[c];                  // −inf: padding, p = 0
+                float p = exp2f(fmaf(acc[j * 4 + 2 * h + e] + b, EV_LOG2E, nl2));
+                if (c == tc && b != -INFINITY) p -= 1.f;
+                gv[e] = gr * p;
+                colsum[j * 2 + e] += gv[e];
+              }
+              if (rv)
+                *reinterpret_cast<__nv_bfloat162*>(grow + j * 8) =
+                    __floats2bfloat162_rn(gv[0], gv[1]);
             }
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-          float sum = 0.f;
-          if (mx != -INFINITY) {
-            const float ms = mx * EV_LOG2E;
-#pragma unroll
-            for (int j = 0; j < BV / 8; ++j)
-#pragma unroll
-              for (int e = 0; e < 2; ++e)
-                sum += exp2f(fmaf(acc[j * 4 + 2 * h + e], EV_LOG2E, -ms));
           }
-          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-          const int row = rbase + 8 * h;
-          if ((lane & 3) == 0 && row < a.N) {
-            float2* p = a.ws + (size_t)blockIdx.x * a.N + row;
-            float2 c = first ? make_float2(-INFINITY, 0.f) : *p;
-            lse_merge(c, mx, sum);
-            *p = c;
-          }
-          if constexpr (SAMPLE) {
-            // keys s − log E in place of s (padding stays −inf), and the quad's key maximum
-            const uint32_t rk = sample_row_key(a.seed, (uint32_t)(a.row0 + row));
-            mx = -INFINITY;
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float mx = -INFINITY;
 #pragma unroll
             for (int j = 0; j < BV / 8; ++j)
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 float& v = acc[j * 4 + 2 * h + e];
-                v -= sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
+                v += s_bias[j * 8 + cq + e];
+                if constexpr (SAMPLE) v *= a.inv_tau;
                 mx = fmaxf(mx, v);
               }
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-          }
-          if constexpr (KC > 0) {
-            if (row < a.N)
-              topk_row<KC>(a, acc, h, cq, mx, s_gid, s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC,
-                           s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC + KC,
-                           a.tk + ((size_t)blockIdx.x * a.N + row) * a.k, first);
+            float sum = 0.f;
+            if (mx != -INFINITY) {
+              const float ms = mx * EV_LOG2E;
+#pragma unroll
+              for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                  sum += exp2f(fmaf(acc[j * 4 + 2 * h + e], EV_LOG2E, -ms));
+            }
+            sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+            const int row = rbase + 8 * h;
+            if ((lane & 3) == 0 && row < a.N) {
+              float2* p = a.ws + (size_t)blockIdx.x * a.N + row;
+              float2 c = first ? make_float2(-INFINITY, 0.f) : *p;
+              lse_merge(c, mx, sum);
+              *p = c;
+            }
+            if constexpr (SAMPLE) {
+              // keys s − log E in place of s (padding stays −inf), and the quad's key maximum
+              const uint32_t rk = sample_row_key(a.seed, (uint32_t)(a.row0 + row));
+              mx = -INFINITY;
+#pragma unroll
+              for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  float& v = acc[j * 4 + 2 * h + e];
+                  v -= sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
+                  mx = fmaxf(mx, v);
+                }
+              mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+              mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            }
+            if constexpr (KC > 0) {
+              if (row < a.N)
+                topk_row<KC>(a, acc, h, cq, mx, s_gid, s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC,
+                             s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC + KC,
+                             a.tk + ((size_t)blockIdx.x * a.N + row) * a.k, first);
+            }
           }
         }
       }
+      if constexpr (GRAD) {
+        // the 8 lanes of a warp that hold the same columns, then the CTA's 8 consumer warps
+#pragma unroll
+        for (int i = 0; i < BV / 4; ++i) {
+          float v = colsum[i];
+          v += __shfl_xor_sync(0xffffffffu, v, 4);
+          v += __shfl_xor_sync(0xffffffffu, v, 8);
+          v += __shfl_xor_sync(0xffffffffu, v, 16);
+          if (lane < 4) atomicAdd(&s_db[(i >> 1) * 8 + cq + (i & 1)], v);
+        }
+      }
+    }
+    if constexpr (GRAD) {
+      __syncthreads();
+      if (threadIdx.x < BV && r0 + (int)threadIdx.x < a.rows) a.db[r0 + threadIdx.x] = s_db[threadIdx.x];
     }
     first = false;
   }
@@ -367,14 +454,15 @@ __device__ __forceinline__ float2 ev_grid_lse(const float2* __restrict__ ws, int
   return c;
 }
 
-template <typename BiasT>
+// LSE: also write each row's log-sum-exp to lse [N] (the training forward keeps it for backward)
+template <typename BiasT, bool LSE = false>
 __global__ void __launch_bounds__(256)
 px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, int K,
                                const __nv_bfloat16* __restrict__ X,
                                const __nv_bfloat16* __restrict__ wt, int wt_pitch,
                                const BiasT* __restrict__ bt, int bt_pitch,
                                const long long* __restrict__ targets, int V,
-                               float* __restrict__ nll) {
+                               float* __restrict__ nll, float* __restrict__ lse) {
   const int lane = threadIdx.x & 31;
   for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
     const float2 c = ev_grid_lse(ws, grid, N, row, lane);
@@ -392,6 +480,7 @@ px_full_softmax_combine_kernel(const float2* __restrict__ ws, int grid, int N, i
       const long long t = targets[row];
       nll[row] = (t >= 0 && t < V) ? c.x + logf(c.y) - (d + (float)bt[(size_t)row * bt_pitch])
                                    : __int_as_float(0x7fc00000);
+      if constexpr (LSE) lse[row] = c.x + logf(c.y);
     }
   }
 }
@@ -459,10 +548,12 @@ px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
 
 // dynamic shared memory of px_full_softmax_lse_kernel<·, kc> at kb K-blocks: alignment slack,
 // table block, X ring, bias and barriers; the top-k kernels (kc > 0) add the block's global ids,
-// and a candidate list and a copy of the row's list per consumer quad
-constexpr int ev_smem_bytes(int kb, int kc) {
+// and a candidate list and a copy of the row's list per consumer quad; the gradient kernels
+// (grad) the block's column sums
+constexpr int ev_smem_bytes(int kb, int kc, bool grad = false) {
   return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8 +
-         (kc > 0 ? EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0);
+         (kc > 0 ? EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0) +
+         (grad ? EV_BV * 4 : 0);
 }
 static_assert(ev_smem_bytes(EV_KMAX / BK, 0) == 198208, "log-sum-exp shared memory at K = 512");
 static_assert(ev_smem_bytes(EV_KMAX / BK, 32) <= 227 * 1024, "top-k shared memory");
@@ -502,29 +593,31 @@ int ev_combine_blocks(int N) {
   return blocks > PX_NUM_SMS * 8 ? PX_NUM_SMS * 8 : blocks;
 }
 
-template <typename BiasT, int KC, bool SAMPLE = false>
-void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC, SAMPLE>& a,
+template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false>
+void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC, SAMPLE, GRAD>& a,
                cudaStream_t stream) {
   using namespace tc;
   static bool set = false;
   if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE>,
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         ev_smem_bytes(EV_KMAX / BK, KC));
+                         ev_smem_bytes(EV_KMAX / BK, KC, GRAD));
     set = true;
   }
-  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE>
-      <<<grid, THREADS, ev_smem_bytes(a.kb, KC), stream>>>(tx, a);
+  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD>
+      <<<grid, THREADS, ev_smem_bytes(a.kb, KC, GRAD), stream>>>(tx, a);
 }
 
 template <typename BiasT>
 void ev_nll(int grid, const CUtensorMap& tx, const tc::EvalArgs& a, const void* X,
             const long long* targets, const void* wt, const void* bt, int V, float* nll,
-            cudaStream_t stream) {
+            float* lse, cudaStream_t stream) {
   ev_launch<BiasT, 0>(grid, tx, a, stream);
-  tc::px_full_softmax_combine_kernel<<<ev_combine_blocks(a.N), 256, 0, stream>>>(
+  (lse ? tc::px_full_softmax_combine_kernel<BiasT, true>
+       : tc::px_full_softmax_combine_kernel<BiasT, false>)<<<ev_combine_blocks(a.N), 256, 0,
+                                                             stream>>>(
       a.ws, grid, a.N, a.K, (const __nv_bfloat16*)X, (const __nv_bfloat16*)wt, a.w_pitch,
-      (const BiasT*)bt, a.b_pitch, targets, V, nll);
+      (const BiasT*)bt, a.b_pitch, targets, V, nll, lse);
 }
 
 // the list capacity is k rounded up to 8, 16 or 32
@@ -572,13 +665,15 @@ extern "C" {
 //                    for a replicated layout, else W);
 //   ws:              fp32 [ws_ctas][N][2] scratch, the grid is at most ws_ctas CTAs;
 //   targets:         int64 [N]; wt / bt: the targets' rows from the group lookup (same pitches
-//                    and types).
+//                    and types);
+//   lse:             null, or fp32 [N] out: each row's log-sum-exp (kept for the backward).
 // Returns 0, a negative argument error, or a CUDA error code.
 int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
                         const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
                         int slots, const GroupGeom* g, int rank, const void* hdr_mine,
                         const void* ctl, int wait, void* ws, int ws_ctas, const long long* targets,
-                        const void* wt, const void* bt, float* nll, cudaStream_t stream) {
+                        const void* wt, const void* bt, float* nll, float* lse,
+                        cudaStream_t stream) {
   using namespace tc;
   if (N <= 0) return 0;
   EvalArgs a;
@@ -588,7 +683,7 @@ int px_full_softmax_nll(const void* X, int N, int K, const void* w_ptrs, int w_p
                     slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
   if (rc) return rc;
   (b_bf16 ? ev_nll<__nv_bfloat16> : ev_nll<float>)(grid, tx, a, X, targets, wt, bt, g->V, nll,
-                                                   stream);
+                                                   lse, stream);
   return (int)cudaGetLastError();
 }
 
@@ -629,6 +724,41 @@ int px_full_softmax_sample(const void* X, int N, int K, const void* w_ptrs, int 
   return ev_lists<true>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt, part_idx,
                         slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, n, tk, log_probs, ids,
                         inv_tau, seed, row0, stream);
+}
+
+// The gradient of the full-softmax NLL over one chunk of the table, global ids [v0, v0 + rows):
+//   G  [N][g_pitch] bf16 = g_i · (exp(x_i · w_v + b_v − lse_i) − [v == t_i]),  v in the chunk
+//   db [rows] fp32       = Σ_i G[i][v]
+// X [N, K] bf16 as px_full_softmax_nll; wc / bc: the chunk's bf16 weight rows and bias rows (fp32,
+// or bf16 when b_bf16), row pitches w_pitch / b_pitch elements as px_full_softmax_nll; lse, g fp32
+// [N] and targets int64 [N].  Columns of G from rows to g_pitch are written as zero; g_pitch >=
+// rows rounded up to 128 and even.  The grid is at most ctas CTAs.
+// Returns 0, a negative argument error, or a CUDA error code.
+int px_full_softmax_grad(const void* X, int N, int K, const void* wc, int w_pitch, const void* bc,
+                         int b_pitch, int b_bf16, int rows, long long v0, const float* lse,
+                         const float* g, const long long* targets, void* G, int g_pitch,
+                         float* db, int ctas, cudaStream_t stream) {
+  using namespace tc;
+  if (N <= 0 || rows <= 0) return 0;
+  if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % (b_bf16 ? 8 : 4))
+    return -1;
+  const int nblk = (rows + EV_BV - 1) / EV_BV;
+  if (ctas < 1 || g_pitch % 2 || g_pitch < nblk * EV_BV) return -2;
+  GradArgs a{};
+  a.N = N; a.K = K; a.kb = (K + BK - 1) / BK;
+  a.w_pitch = w_pitch; a.b_pitch = b_pitch;
+  a.W = 1; a.rank = 0; a.replicated = 1; a.owners = 1; a.slots = 1; a.rows_per_part = rows;
+  a.nblk = nblk;
+  a.wc = (const __nv_bfloat16*)wc; a.bc = bc; a.rows = rows; a.v0 = v0;
+  a.lse = lse; a.g = g; a.targets = targets;
+  a.G = (__nv_bfloat16*)G; a.g_pitch = g_pitch; a.db = db;
+  CUtensorMap tx;
+  int rc = make_tmap(&tx, X, N, K, BM);
+  if (rc) return rc;
+  const int grid = nblk < ctas ? nblk : ctas;
+  (b_bf16 ? ev_launch<__nv_bfloat16, 0, false, true> : ev_launch<float, 0, false, true>)(
+      grid, tx, a, stream);
+  return (int)cudaGetLastError();
 }
 
 }  // extern "C"

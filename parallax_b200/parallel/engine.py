@@ -123,32 +123,72 @@ def lookup_many(modules, ids, defer=False):
     return PendingLookup(outs) if defer else outs
 
 
-def _fused_eval_group(inputs, weight, bias):
-    """The co-lookup group whose fused full-softmax kernels can evaluate `inputs` against the
+def _fused_group(inputs, weight, bias):
+    """The co-lookup group whose fused full-softmax kernels can take `inputs` against the
     (weight, bias) embedding modules, else None: the modules form a group on the NVLink fabric
-    (protocol nvlink) whose weight table keeps a bf16 shadow, `inputs` is bf16 on the group's
-    device with K % 8 == 0 and K <= 512, and no gradient is wanted."""
+    (protocol nvlink) whose weight table keeps a bf16 shadow, and `inputs` is bf16 on the group's
+    device with K % 8 == 0 and K <= 512."""
     tabs = [getattr(m, "table", None) for m in (weight, bias)]
     grp = getattr(tabs[0], "group", None) if tabs[0] is not None else None
     K = int(inputs.shape[-1])
     if grp is not None and list(grp.tables) == tabs and grp.protocol == "nvlink" and \
             tabs[0].use_shadow and inputs.dtype == torch.bfloat16 and \
-            inputs.device == grp.device and K % 8 == 0 and K <= 512 and \
-            (not torch.is_grad_enabled() or not (inputs.requires_grad or
-                                                 weight._anchor.requires_grad or
-                                                 bias._anchor.requires_grad)):
+            inputs.device == grp.device and K % 8 == 0 and K <= 512:
         return grp
     return None
 
 
+def _wants_grad(inputs, weight, bias):
+    return torch.is_grad_enabled() and (inputs.requires_grad or weight._anchor.requires_grad or
+                                        bias._anchor.requires_grad)
+
+
+def _fused_eval_group(inputs, weight, bias):
+    """`_fused_group` where no gradient is wanted, else None."""
+    grp = _fused_group(inputs, weight, bias)
+    return None if grp is None or _wants_grad(inputs, weight, bias) else grp
+
+
+class _FullSoftmaxNLLFn(torch.autograd.Function):
+    """Fused full-softmax NLL in training (sess_config["full_softmax_train"] = "fused"):
+    forward `NVSparseGroup.full_softmax_nll_lse`, backward `full_softmax_nll_grad`.  When the
+    tables want gradients the forward counts one pending call of every row of the group
+    (`record_all_rows`) and the backward hands the rows to `add_pending`, so the unchanged
+    push and owner kernels apply them like a lookup's."""
+
+    @staticmethod
+    def forward(ctx, anchor_w, anchor_b, inputs, targets, group):
+        nll, lse = group.full_softmax_nll_lse(inputs, targets)
+        ctx.group = group
+        ctx.tables = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        ctx.token = group.record_all_rows() if ctx.tables else None
+        ctx.save_for_backward(inputs, targets, lse)
+        return nll
+
+    @staticmethod
+    def backward(ctx, g):
+        inputs, targets, lse = ctx.saved_tensors
+        want_x = ctx.needs_input_grad[2]
+        dx, dW, db = ctx.group.full_softmax_nll_grad(inputs, targets, lse, g, want_x=want_x,
+                                                     want_tables=ctx.tables)
+        if ctx.tables:
+            ctx.group.add_pending(ctx.token, [dW, db])
+        return None, None, dx if want_x else None, None, None
+
+
 def full_softmax_nll(inputs, targets, weight, bias):
     """Per-row ``cross_entropy(inputs @ W.T + b, targets, reduction="none")`` over every row
-    of the (weight, bias) embedding modules.  Where `_fused_eval_group` finds a group, its
-    fused kernel computes it where the rows live; everything else runs the gather + matmul +
-    cross_entropy composition (which also gives the tables their gradients in training)."""
-    grp = _fused_eval_group(inputs, weight, bias)
+    of the (weight, bias) embedding modules.  Where `_fused_group` finds a group, its fused
+    kernel computes it where the rows live when no gradient is wanted, and also in training
+    when the session sets ``full_softmax_train="fused"`` (`_FullSoftmaxNLLFn`); everything else
+    runs the gather + matmul + cross_entropy composition (which also gives the tables their
+    gradients in training)."""
+    grp = _fused_group(inputs, weight, bias)
     if grp is not None:
-        return grp.full_softmax_nll(inputs, targets)
+        if not _wants_grad(inputs, weight, bias):
+            return grp.full_softmax_nll(inputs, targets)
+        if grp.full_softmax_train == "fused":
+            return _FullSoftmaxNLLFn.apply(weight._anchor, bias._anchor, inputs, targets, grp)
     return full_softmax_composition(inputs, targets, weight, bias)
 
 
@@ -351,6 +391,7 @@ class TrainEngine(object):
         self._check_layerwise(sync)
         self._check_sparse_weights(sync)
         self._check_micro_batches(sync)
+        self._check_full_softmax_train()
         self._build()
         self._consistency_check()
         self._start_aux()
@@ -493,6 +534,31 @@ class TrainEngine(object):
                     "place with an all-reduce per step.  Use the default sharded update, or "
                     "sess_config={'fabric': 'library'} to accumulate over library "
                     "collectives" % k)
+
+    def _check_full_softmax_train(self):
+        """``sess_config["full_softmax_train"]``: "composition" (default) or "fused", how
+        `parallax.nn.full_softmax_nll` trains.  Refuses at build, before anything is
+        allocated, where the fused kernels cannot run."""
+        value = self.config.sess_option("full_softmax_train", "composition")
+        if value not in ("composition", "fused"):
+            raise ValueError("sess_config['full_softmax_train'] must be 'composition' or "
+                             "'fused', got %r" % (value,))
+        if value == "composition":
+            return
+        if self.backend != "nvlink":
+            raise ValueError(
+                "full_softmax_train='fused' needs the NVLink fabric (got fabric %r): the fused "
+                "kernels read the table rows where their owners store them" % (self.backend,))
+        if self.config.communication_config.ps_config.protocol == "nccl":
+            raise ValueError(
+                "full_softmax_train='fused' is not implemented for PSConfig(protocol='nccl'): "
+                "the fused kernels read peers' rows over NVLink, not through library "
+                "collectives")
+        cdt = self.config.sess_option("compute_dtype")
+        if cdt not in ("bf16", "bfloat16", torch.bfloat16):
+            raise ValueError(
+                "full_softmax_train='fused' needs compute_dtype='bf16' (got %r): the fused "
+                "kernels take bf16 inputs and bf16 table rows" % (cdt,))
 
     def _split_feeds(self, feeds):
         """The `micro_batches` parts of a step's feeds: every tensor feed with a dim 0 as

@@ -398,6 +398,10 @@ class NVSparseGroup(object):
         # pushed together, after the last one's backward, and weighted 1/K on the owner
         self.micro_batches = int(opts.get("micro_batches", 1))
         self._last_mb = True
+        # sess_config["full_softmax_train"]: "fused" trains `parallax.nn.full_softmax_nll` over
+        # this (weight, bias) group with `full_softmax_nll_lse` / `full_softmax_nll_grad`
+        self.full_softmax_train = opts.get("full_softmax_train", "composition")
+        self._all_ids = None
         hints = [t.capacity_hint for t in tables if t.capacity_hint]
         self.capacity_hint = max(hints) if hints else None
         self.hp = hp_stage(self.fabric, t0.optimizer)
@@ -605,13 +609,22 @@ class NVSparseGroup(object):
         table and no [N, V] logits (`ops/csrc/kernels/softmax_eval.cu`).  The targets' rows
         come from one launch of the group's lookup kernel.  A target outside [0, V) gives
         NaN in its row.  One-sided: no other rank takes part."""
+        return self._nll(x, targets, False)[0]
+
+    def full_softmax_nll_lse(self, x, targets):
+        """``(nll, lse)``, fp32 [N] each: `full_softmax_nll` and each row's log-sum-exp, which
+        the backward (`full_softmax_nll_grad`) takes."""
+        return self._nll(x, targets, True)
+
+    def _nll(self, x, targets, want_lse):
         L = ops.lib()
         tw, tb = self.tables
         x, K, (b_src, b_pitch), head, tail, stream = self._eval_operands(x, "full_softmax_nll")
         n = int(x.shape[0])
         out = torch.empty(n, dtype=torch.float32, device=self.device)
+        lse = torch.empty(n, dtype=torch.float32, device=self.device) if want_lse else None
         if n == 0:
-            return out
+            return out, lse
         ids = targets.reshape(-1).to(self.device, torch.int64).contiguous()
         # target bias from the master rows like every bias row the eval kernel reads
         w_t = torch.empty((n, tw.Dps), dtype=torch.bfloat16, device=self.device)
@@ -628,8 +641,88 @@ class NVSparseGroup(object):
         ops.check(L.px_full_softmax_nll(
             _vp(x.data_ptr()), n, K, *head, *tail, _vp(ws.data_ptr()), consts.NUM_SMS,
             _vp(ids.data_ptr()), _vp(w_t.data_ptr()), _vp(b_t.data_ptr()),
-            _vp(out.data_ptr()), stream), "full_softmax_nll")
-        return out
+            _vp(out.data_ptr()), _vp(lse.data_ptr() if want_lse else 0), stream),
+            "full_softmax_nll")
+        return out, lse
+
+    def _all_rows(self):
+        """int32 [V]: every global id of the group, allocated once."""
+        if self._all_ids is None:
+            self._all_ids = torch.arange(self.tables[0].V, dtype=torch.int32, device=self.device)
+        return self._all_ids
+
+    def record_all_rows(self):
+        """Counts one forward call whose gradient rows are every row of the group, in global
+        id order, without a lookup, and returns its token (the fused full-softmax training
+        forward; its backward hands the rows to `add_pending` like a lookup's)."""
+        self._fwd_calls += 1
+        return self._all_rows()
+
+    def full_softmax_train_chunk(self, n):
+        """Rows of one vocabulary chunk of `full_softmax_nll_grad` for n input rows: the
+        chunk's gathered rows and its bf16 [n, Vc] softmax gradient fit in
+        `consts.FULL_SOFTMAX_TRAIN_WS_BYTES`; a multiple of 128 · NUM_SMS where that fits
+        (whole waves of the gradient kernel's 128-row blocks), else of 128."""
+        tw, tb = self.tables
+        b_bytes = tb.Dps * 2 if tb.weight_dtype == torch.bfloat16 else tb.Dp * 4
+        rows = consts.FULL_SOFTMAX_TRAIN_WS_BYTES // (2 * n + 2 * tw.Dps + b_bytes)
+        wave = 128 * consts.NUM_SMS
+        vc = rows // wave * wave if rows >= wave else max(128, rows // 128 * 128)
+        return min(vc, (tw.V + 127) // 128 * 128)
+
+    def full_softmax_nll_grad(self, x, targets, lse, g, want_x=True, want_tables=True,
+                              chunk=None):
+        """Backward of `full_softmax_nll_lse` for the gradient `g` [N] of the NLL: ``(dx,
+        dW, db)`` with dx [N, K] in `x`'s dtype and the table gradient as every row in
+        global id order, dW [V, K] and db [V, 1] in the tables' lookup dtypes (what
+        `add_pending` takes); None for what is not wanted.  Over vocabulary chunks of
+        `chunk` rows (default `full_softmax_train_chunk`): one lookup launch gathers the
+        chunk's rows, the gradient kernel recomputes its logits and writes G = g · (softmax −
+        onehot) in bf16 and db, then dx += G·W_c (fp32) and dW_c = Gᵀ·x.  One-sided: no other
+        rank takes part."""
+        L = ops.lib()
+        tw, tb = self.tables
+        x, K, (b_src, b_pitch), _, _, stream = self._eval_operands(x, "full_softmax_nll_grad")
+        n, V, dev = int(x.shape[0]), tw.V, self.device
+        dx = torch.zeros(n, K, dtype=torch.float32, device=dev) if want_x else None
+        dW = torch.empty(V, K, dtype=torch.bfloat16, device=dev) if want_tables else None
+        db = torch.zeros(V, dtype=torch.float32, device=dev)
+        if n > 0:
+            ids = targets.reshape(-1).to(dev, torch.int64).contiguous()
+            lse = lse.to(dev, torch.float32).contiguous()
+            g = g.reshape(-1).to(dev, torch.float32).contiguous()
+            vc = int(chunk) if chunk else self.full_softmax_train_chunk(n)
+            gp = (vc + 127) // 128 * 128
+            wc = torch.empty((vc, tw.Dps), dtype=torch.bfloat16, device=dev)
+            bc = torch.empty((vc, b_pitch), dtype=tb.weight_dtype, device=dev)
+            G = torch.empty((n, gp), dtype=torch.bfloat16, device=dev)
+            all_ids = self._all_rows()
+            descs = (ops.LookupTable * 2)(_lookup_table(tw, "shadow", wc),
+                                          _lookup_table(tb, b_src, bc))
+            for v0 in range(0, V, vc):
+                m = min(vc, V - v0)
+                _count(2)
+                ops.check(L.px_sparse_lookup(
+                    _vp(all_ids[v0:].data_ptr()), 0, m, descs, 2, _vp(0),
+                    ctypes.byref(self.geom), _vp(self.hdr_buf.local_ptr),
+                    _vp(self.ctl.data_ptr()), self._wait, stream),
+                    "sparse_lookup(full softmax chunk)")
+                ops.check(L.px_full_softmax_grad(
+                    _vp(x.data_ptr()), n, K, _vp(wc.data_ptr()), tw.Dps, _vp(bc.data_ptr()),
+                    b_pitch, int(tb.weight_dtype == torch.bfloat16), m, v0,
+                    _vp(lse.data_ptr()), _vp(g.data_ptr()), _vp(ids.data_ptr()),
+                    _vp(G.data_ptr()), gp, _vp(db[v0:].data_ptr()), consts.NUM_SMS, stream),
+                    "full_softmax_grad")
+                Gc = G[:, :m]
+                if want_x:
+                    dx.add_(torch.mm(Gc, wc[:m, :K], out_dtype=torch.float32))
+                if want_tables:
+                    torch.mm(Gc.t(), x, out=dW[v0:v0 + m])
+        if want_x:
+            dx = dx.to(x.dtype)
+        if not want_tables:
+            return dx, None, None
+        return dx, dW.to(tw.out_dtype), db.to(tb.out_dtype)[:, None]
 
     def full_softmax_topk(self, x, k):
         """The k largest full-softmax logits of each row of bf16 inputs `x` [N, K] against
