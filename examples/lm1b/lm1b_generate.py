@@ -2,11 +2,13 @@
 `lm1b_distributed_driver.py --ckpt_dir …` (as `lm1b_eval.py` does, `--use_ema` included), prime
 the LSTM with a prefix and draw one word at a time from the full softmax at a temperature
 (`parallax.nn.full_softmax_sample`, fused on the rows' owners for bf16 tables on the NVLink
-fabric).  Each step feeds the previous words [B, 1] and the previous LSTM state, with no target,
-so the softmax table is read once per word.  The same `--seed` gives the same text.
+fabric), optionally truncated to the `--top_k` most likely words and the `--top_p` nucleus.
+Each step feeds the previous words [B, 1] and the previous LSTM state, with no target, so the
+softmax table is read once per word (ten times when truncated).  The same `--seed` gives the same
+text.
 
     python examples/lm1b/lm1b_generate.py --ckpt_dir /tmp/lm1b_ckpt --datadir … \\
-        --prefix "The meeting" --num_words 30 --temperature 0.8 --num_sequences 4 \\
+        --prefix "The meeting" --num_words 30 --temperature 0.8 --top_p 0.9 --num_sequences 4 \\
         --compute_dtype bf16
     python examples/lm1b/lm1b_generate.py --ckpt_dir … --use_synthetic --tiny --prefix "5 17"
 """
@@ -37,6 +39,10 @@ ap.add_argument("--prefix", default="",
 ap.add_argument("--num_words", type=int, default=20, help="words to generate at most")
 ap.add_argument("--num_sequences", type=int, default=4, help="sequences generated together")
 ap.add_argument("--temperature", type=float, default=1.0)
+ap.add_argument("--top_k", type=int, default=None,
+                help="sample only among the K most likely words (and words tied with the K-th)")
+ap.add_argument("--top_p", type=float, default=None,
+                help="sample only from the smallest set of most likely words of mass >= P")
 ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--compute_dtype", default=None,
                 help="bf16: bf16 LSTM outputs, which the fused sampler takes on the NVLink fabric")
@@ -50,7 +56,8 @@ def step_seed(seed, step):
 
 def main():
     kw = dict(vocab_size=FLAGS.vocab_size, lazy=True, eval_sample=1,
-              sample_temperature=FLAGS.temperature)
+              sample_temperature=FLAGS.temperature, sample_top_k=FLAGS.top_k,
+              sample_top_p=FLAGS.top_p)
     if FLAGS.tiny:
         kw.update(vocab_size=min(FLAGS.vocab_size, 10000), emb_size=32, state_size=64,
                   projected_size=32, num_sampled=64, lazy=False)
@@ -102,8 +109,9 @@ def main():
         if done.all():
             break
         x = nxt[:, None].astype(np.int64)
-    parallax.log.info("checkpoint %s (global_step %d), temperature %g, seed %d",
-                      path, eng.global_step, FLAGS.temperature, FLAGS.seed)
+    parallax.log.info("checkpoint %s (global_step %d), temperature %g, top_k %s, top_p %s, "
+                      "seed %d", path, eng.global_step, FLAGS.temperature, FLAGS.top_k,
+                      FLAGS.top_p, FLAGS.seed)
     for b in range(B):
         print(" ".join(word(i) for i in prefix + out[b]))
     sess.close()

@@ -108,6 +108,10 @@ NUM_SMS = 132
 # bound on the per-CTA top-k lists of one fused full-softmax top-k launch (NUM_SMS · rows · k
 # 8-byte entries); larger batches are evaluated in row chunks, each reading the table once
 TOPK_WS_BYTES = 48 << 20
+# digit width of the threshold search of truncated full-softmax sampling (top_k / top_p): one
+# histogram pass over the table per digit of the 32-bit key, [NUM_SMS, rows, 2^d] 8-byte bins
+# (EV_RADIX_BITS in ops/csrc/kernels/softmax_eval.cu, which refuses other digit positions)
+SAMPLE_RADIX_BITS = 4
 # bound on the chunk scratch of the fused full-softmax backward (sess_config
 # ["full_softmax_train"] = "fused"): the gathered rows and the bf16 [N, Vc] softmax gradient of
 # one vocabulary chunk of Vc rows

@@ -89,17 +89,19 @@ class LM1B(nn.Module):
     def __init__(self, vocab_size=793470, emb_size=512, state_size=2048,
                  projected_size=512, num_sampled=8192, num_steps=20,
                  num_shards=32, keep_prob=0.9, lazy=False, eval_top_k=0, eval_sample=0,
-                 sample_temperature=1.0):
+                 sample_temperature=1.0, sample_top_k=None, sample_top_p=None):
         """`eval_top_k` = k > 0: in eval mode `forward` also returns ``"top_k_ids"``, the k
         most likely next words of every position (`parallax.nn.full_softmax_topk`).
         `eval_sample` = n > 0: in eval mode `forward` also returns ``"sample_ids"`` and
         ``"sample_log_probs"`` [B, T, n], n next words of every position drawn without
         replacement at temperature `sample_temperature` (`parallax.nn.full_softmax_sample`,
-        seeded by the `sample_seed` feed)."""
+        seeded by the `sample_seed` feed), truncated to the `sample_top_k` most likely words
+        and to the nucleus of mass `sample_top_p` when those are given (None: no truncation)."""
         super().__init__()
         self.eval_top_k = int(eval_top_k)
         self.eval_sample = int(eval_sample)
         self.sample_temperature = float(sample_temperature)
+        self.sample_top_k, self.sample_top_p = sample_top_k, sample_top_p
         self.vocab_size, self.emb_size = vocab_size, emb_size
         self.state_size, self.projected_size = state_size, projected_size
         self.num_sampled, self.num_steps = num_sampled, num_steps
@@ -172,8 +174,11 @@ class LM1B(nn.Module):
             out["top_k_ids"] = ids.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
         if self.eval_sample > 0 and not self.training:
             seed = None if sample_seed is None else int(sample_seed)
+            trunc = {k: v for k, v in (("top_k", self.sample_top_k),
+                                       ("top_p", self.sample_top_p)) if v is not None}
             lp, ids = pnn.full_softmax_sample(inputs, self.softmax_w, self.softmax_b,
-                                              self.eval_sample, self.sample_temperature, seed)
+                                              self.eval_sample, self.sample_temperature, seed,
+                                              **trunc)
             out["sample_ids"] = ids.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
             out["sample_log_probs"] = lp.reshape(T, Bsz, -1).transpose(0, 1).contiguous()
         return out

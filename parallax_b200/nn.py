@@ -179,7 +179,8 @@ def full_softmax_topk(inputs, weight, bias, k):
     return _ft(inputs, weight, bias, k)
 
 
-def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, seed=None):
+def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, seed=None,
+                        top_k=None, top_p=None):
     """Next-word sampling from a partitioned output table: for every row of `inputs`,
     `num_samples` = n distinct rows of the table drawn without replacement from ::
 
@@ -199,9 +200,28 @@ def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, se
     `full_softmax_nll`.  Under the conditions of its fused path and with n <= 32, one fused
     kernel keeps each row's n best keys where the rows live (no gathered table, no [N, V]
     logits); otherwise the table is gathered and the logits materialised, which also carries
-    gradients into `log_probs`.  `ValueError` for the shapes `full_softmax_nll` refuses, a
-    `num_samples` that is not an int in [1, V], a `temperature` that is not a finite real number
-    > 0, and a `seed` that is neither None nor an int in [0, 2^32)."""
+    gradients into `log_probs`.
+
+    Truncation: `top_k` (an int in [num_samples, V]) and `top_p` (a real number in (0, 1]; 1
+    means no nucleus) restrict each row's draws to T = {v : s_v >= θ*}, θ* the largest θ with ::
+
+        count(θ) >= top_k   or   (mass(θ) >= top_p  and  count(θ) >= num_samples)
+
+    where count(θ) and mass(θ) are the number and the softmax(s) mass of the row's s >= θ, and an
+    absent argument makes its clause false.  So `top_k` alone keeps the k most likely words and
+    every word tied with the k-th; `top_p` alone keeps the smallest nucleus of mass >= p, never
+    fewer than num_samples words; both keep the smaller of the two sets.  The draws are the n
+    best keys within T (the untruncated draw order filtered to T, same noise), and `log_probs`
+    stay the log-probabilities under the untruncated softmax: the log-probability under the
+    renormalised distribution is ``log_probs − log mass(T)``, with mass(T) = Σ_{v in T}
+    exp(log_probs of v).  The fused path finds θ* with a radix search over the fp32 key, one
+    histogram pass over the table per 4-bit digit, so a truncated call reads the table 10 times.
+    With both None the call is exactly the untruncated one.
+
+    `ValueError` for the shapes `full_softmax_nll` refuses, a `num_samples` that is not an int in
+    [1, V], a `temperature` that is not a finite real number > 0, a `seed` that is neither None
+    nor an int in [0, 2^32), a `top_k` that is not an int in [1, V] or is below `num_samples`,
+    and a `top_p` that is not a finite real number in (0, 1]."""
     import math
     import numbers
     if inputs.dim() != 2:
@@ -222,8 +242,21 @@ def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, se
     elif isinstance(seed, bool) or not isinstance(seed, numbers.Integral) or \
             not 0 <= seed < 1 << 32:
         raise ValueError("seed must be None or an int in [0, 2^32), got %r" % (seed,))
+    if top_k is not None:
+        if isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral) or \
+                not 1 <= top_k <= V:
+            raise ValueError("top_k must be None or an int in [1, %d], got %r" % (V, top_k))
+        if num_samples > top_k:
+            raise ValueError("num_samples (%d) must not exceed top_k (%d)" % (num_samples, top_k))
+        top_k = int(top_k)
+    if top_p is not None:
+        if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real) or \
+                not math.isfinite(top_p) or not 0 < top_p <= 1:
+            raise ValueError("top_p must be None or a finite real number in (0, 1], got %r"
+                             % (top_p,))
+        top_p = None if top_p == 1 else float(top_p)
     from .parallel.engine import full_softmax_sample as _fsm
-    return _fsm(inputs, weight, bias, num_samples, inv_tau, int(seed))
+    return _fsm(inputs, weight, bias, num_samples, inv_tau, int(seed), top_k, top_p)
 
 
 def _check_full_softmax(inputs, weight, bias):

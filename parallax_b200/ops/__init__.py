@@ -109,6 +109,20 @@ _SIGS = {
                                        ctypes.POINTER(GroupGeom), c_int, c_void_p, c_void_p,
                                        c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                        c_void_p, c_float, ctypes.c_uint32, c_int, c_void_p]),
+    "px_full_softmax_sample_lse": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
+                                           c_int, c_int, c_void_p, c_int,
+                                           ctypes.POINTER(GroupGeom), c_int, c_void_p, c_void_p,
+                                           c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
+    "px_full_softmax_radix": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                      c_int, c_void_p, c_int, ctypes.POINTER(GroupGeom), c_int,
+                                      c_void_p, c_void_p, c_int, c_void_p, c_int, c_float,
+                                      c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
+    "px_full_softmax_sample_masked": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
+                                              c_int, c_int, c_void_p, c_void_p, c_int,
+                                              ctypes.POINTER(GroupGeom), c_int, c_void_p,
+                                              c_void_p, c_int, c_void_p, c_int, c_int, c_void_p,
+                                              c_void_p, c_void_p, c_float, ctypes.c_uint32,
+                                              c_int, c_void_p, c_void_p]),
     "px_sparse_push": (c_int, [c_void_p, c_int, ctypes.POINTER(PushTable), c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_int,
                                ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int, c_int,

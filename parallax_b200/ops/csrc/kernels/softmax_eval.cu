@@ -28,6 +28,23 @@
 // the n largest keys of a row are n draws without replacement from softmax(s), in draw order.
 // The combine recovers s of each kept entry from its key and writes s − lse.
 //
+// Truncated sampling (top-k / nucleus): each row keeps T = {v : s_v >= θ*}, θ* the largest θ
+// with count(θ) >= k or (mass(θ) >= p and count(θ) >= n), where count and mass are the number
+// and the softmax mass of the row's s >= θ, compared in the order-preserving uint32 key of fp32
+// (−0 taken as +0).  Three kinds of pass of the same GEMM kernel find and apply θ*:
+//   px_full_softmax_sample_lse   KC = 0, SAMPLE: the (max, Σexp) pairs of s, merged into each
+//                                row's lse and a zeroed threshold state (TruncRow).
+//   px_full_softmax_radix        HIST = d: for every real s whose key matches the row's prefix,
+//                                count 1 and exp(s − lse) into the bin of its next d-bit digit,
+//                                per consumer lane in shared memory, then the quad's sums into the
+//                                CTA's slice of a [grid, N, 2^d] workspace (the quad owns its
+//                                rows' slices: no atomics); one warp per row then sums the slices
+//                                and takes the highest digit whose cumulative (count, mass) from
+//                                above satisfies the predicate.  32 / d passes give θ*.
+//   px_full_softmax_sample_masked  the sampling kernel with MASK: keys of s below θ* become −inf
+//                                after the (max, Σexp) pairs are merged, so log-probabilities
+//                                stay those of the untruncated softmax.
+//
 // Training (px_full_softmax_grad): the log-sum-exp instantiations with GRAD = true take one
 // gathered chunk of the table, global ids [v0, v0 + rows), as a one-owner, one-slot table and
 // recompute its biased logits s.  The epilogue writes G = g_i · (exp(s − lse_i) − [v == t_i]) in
@@ -96,12 +113,52 @@ struct GradArgs : EvalArgs {
   int g_pitch;                      // >= the chunk's blocks · BV, even
   float* db;                        // [rows] out: column sums of G
 };
-template <int KC, bool SAMPLE = false, bool GRAD = false>
+
+// truncated sampling: a row's threshold search state.  The keys >= prefix (its bits below the
+// current digit zero) that lie above the prefix's range number `above` with softmax mass
+// `above_mass`; after the last pass prefix is the key of θ*
+struct TruncRow {
+  uint32_t prefix, above;
+  float above_mass;
+  float lse;                        // log-sum-exp of the row's s
+};
+struct HistBin { uint32_t cnt; float mass; };
+constexpr int EV_RADIX_BITS = 4;    // digit width d of a histogram pass
+
+// the tempered log-sum-exp kernels' arguments (KC == 0, SAMPLE)
+struct TempArgs : EvalArgs {
+  float inv_tau;
+};
+// the histogram kernels' arguments (KC == 0, HIST = d)
+struct HistArgs : TempArgs {
+  const TruncRow* rows;             // [N]
+  HistBin* hist;                    // [grid][N][2^d] per-CTA bins
+  int lo;                           // bit position of the pass's digit
+  uint32_t himask;                  // the key bits the prefix has fixed
+};
+// the masked sampling kernels' arguments (KC > 0, SAMPLE, MASK): keys below rows[].prefix drop
+struct MaskArgs : SampleArgs {
+  const TruncRow* rows;             // [N]
+};
+
+template <int KC, bool SAMPLE = false, bool GRAD = false, int HIST = 0, bool MASK = false>
 using EvalParams = typename std::conditional<
     GRAD, GradArgs,
     typename std::conditional<
-        KC == 0, EvalArgs,
-        typename std::conditional<SAMPLE, SampleArgs, TopkArgs>::type>::type>::type;
+        KC == 0,
+        typename std::conditional<
+            HIST != 0, HistArgs,
+            typename std::conditional<SAMPLE, TempArgs, EvalArgs>::type>::type,
+        typename std::conditional<
+            MASK, MaskArgs,
+            typename std::conditional<SAMPLE, SampleArgs, TopkArgs>::type>::type>::type>::type;
+
+// order-preserving uint32 key of an fp32 value (not NaN), −0 taken as +0
+__device__ __forceinline__ uint32_t ev_key(float f) {
+  uint32_t u = __float_as_uint(f);
+  if (u == 0x80000000u) u = 0u;
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
 
 __device__ __forceinline__ bool tk_beats(float v, int id, float v2, int id2) {
   return v > v2 || (v == v2 && id < id2);
@@ -207,11 +264,14 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
 // BiasT: float (fp32 master bias rows) or __nv_bfloat16 (bf16 master bias rows).  KC: top-k list
 // capacity (0: log-sum-exp only; else k <= KC and the top-k epilogue runs).  SAMPLE (KC > 0):
 // the lists rank Gumbel keys of the tempered logits instead of the logits.  GRAD (KC == 0): the
-// gradient epilogue over one gathered chunk instead of the (max, Σexp) pairs
-template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false>
+// gradient epilogue over one gathered chunk instead of the (max, Σexp) pairs.  SAMPLE with KC == 0:
+// the pairs are of s = l/τ.  HIST = d (KC == 0, SAMPLE): the digit histogram of truncated sampling
+// instead of the pairs.  MASK (KC > 0, SAMPLE): keys below the row's threshold drop out
+template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false, int HIST = 0,
+          bool MASK = false>
 __global__ void __launch_bounds__(THREADS, 1)
 px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
-                           EvalParams<KC, SAMPLE, GRAD> a) {
+                           EvalParams<KC, SAMPLE, GRAD, HIST, MASK> a) {
   constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -223,6 +283,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
   int* s_gid = reinterpret_cast<int*>(empty_bar + EV_STAGES);      // [BV] (KC > 0)
   TopkEntry* s_cand = reinterpret_cast<TopkEntry*>(s_gid + BV);   // [256 / 4 quads][2][KC]
   float* s_db = reinterpret_cast<float*>(s_gid);                  // [BV] (GRAD)
+  HistBin* s_hist = reinterpret_cast<HistBin*>(s_gid);            // [2^d][256 lanes] (HIST)
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
@@ -359,6 +420,62 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
                     __floats2bfloat162_rn(gv[0], gv[1]);
             }
           }
+        } else if constexpr (HIST != 0) {
+          // each consumer lane counts its 32 columns of the row into its own bins (bin-major,
+          // s_hist[bin][lane]: no atomics, no bank conflicts), then the quad's lane q sums
+          // bins q, q + 4, ... over the quad's four lanes into the CTA's slice
+          constexpr int NB = 1 << HIST;
+          const unsigned qmask = 0xfu << (lane & 28);
+          const int tid = threadIdx.x - 128;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = rbase + 8 * h;
+            if (row >= a.N) continue;                       // the quad's rows: quad-uniform
+            const TruncRow st = a.rows[row];
+            HistBin* gb = a.hist + ((size_t)blockIdx.x * a.N + row) * NB;
+            bool hit = false;
+#pragma unroll
+            for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                // s as SAMPLE scales it; padding rows are never candidates
+                const float b = s_bias[j * 8 + cq + e];
+                const float s = (acc[j * 4 + 2 * h + e] + b) * a.inv_tau;
+                hit |= b != -INFINITY && !((ev_key(s) ^ st.prefix) & a.himask);
+              }
+            if (!__any_sync(qmask, hit)) {                  // no key of the block matches
+              if (first)
+                for (int i = lane & 3; i < NB; i += 4) gb[i] = HistBin{0u, 0.f};
+              continue;
+            }
+#pragma unroll
+            for (int i = 0; i < NB; ++i) s_hist[i * 256 + tid] = HistBin{0u, 0.f};
+            const float nl2 = -st.lse * EV_LOG2E;
+#pragma unroll
+            for (int j = 0; j < BV / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float b = s_bias[j * 8 + cq + e];
+                const float s = (acc[j * 4 + 2 * h + e] + b) * a.inv_tau;
+                const uint32_t u = ev_key(s);
+                if (b == -INFINITY || ((u ^ st.prefix) & a.himask)) continue;
+                HistBin& bin = s_hist[((u >> a.lo) & (NB - 1)) * 256 + tid];
+                bin.cnt += 1u;
+                bin.mass += exp2f(fmaf(s, EV_LOG2E, nl2));
+              }
+            __syncwarp(qmask);
+            for (int i = lane & 3; i < NB; i += 4) {
+              HistBin v = first ? HistBin{0u, 0.f} : gb[i];
+#pragma unroll
+              for (int l = 0; l < 4; ++l) {
+                const HistBin o = s_hist[i * 256 + (tid & ~3) + l];
+                v.cnt += o.cnt;
+                v.mass += o.mass;
+              }
+              gb[i] = v;
+            }
+            __syncwarp(qmask);                              // before the bins are reused
+          }
         } else {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -392,16 +509,22 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
               lse_merge(c, mx, sum);
               *p = c;
             }
-            if constexpr (SAMPLE) {
+            if constexpr (SAMPLE && KC > 0) {
               // keys s − log E in place of s (padding stays −inf), and the quad's key maximum
               const uint32_t rk = sample_row_key(a.seed, (uint32_t)(a.row0 + row));
+              [[maybe_unused]] uint32_t thr = 0u;   // MASK: keys of s below θ* become −inf
+              if constexpr (MASK) thr = row < a.N ? a.rows[row].prefix : 0u;
               mx = -INFINITY;
 #pragma unroll
               for (int j = 0; j < BV / 8; ++j)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   float& v = acc[j * 4 + 2 * h + e];
-                  v -= sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
+                  if constexpr (MASK)
+                    v = ev_key(v) < thr ? -INFINITY
+                                        : v - sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
+                  else
+                    v -= sample_log_e(rk, (uint32_t)s_gid[j * 8 + cq + e]);
                   mx = fmaxf(mx, v);
                 }
               mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
@@ -546,17 +669,80 @@ px_full_softmax_topk_combine_kernel(const float2* __restrict__ ws,
   }
 }
 
+// truncated sampling, one warp per row: merge the grid's (max, Σexp) pairs of s into the row's
+// lse and start its threshold search (prefix 0: every key)
+__global__ void __launch_bounds__(256)
+px_full_softmax_trunc_init_kernel(const float2* __restrict__ ws, int grid, int N,
+                                  TruncRow* __restrict__ rows) {
+  const int lane = threadIdx.x & 31;
+  for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
+    const float2 c = ev_grid_lse(ws, grid, N, row, lane);
+    if (lane == 0) rows[row] = TruncRow{0u, 0u, 0.f, c.x + logf(c.y)};
+  }
+}
+
+// one radix step of the threshold search, one warp per row: sum the grid's bins of the digit at
+// bit lo (lane b and b + NB hold bin b), take suffix sums from the highest digit down, and fix
+// the highest digit b at which count(θ) >= k or (mass(θ) >= p and count(θ) >= n) holds for θ =
+// prefix | b << lo (k = 0 / p = 0: no such clause).  No digit: b = 0, so a row whose predicate
+// never holds (fp32 mass short of p) keeps every word.
+template <int D>
+__global__ void __launch_bounds__(256)
+px_full_softmax_select_kernel(const HistBin* __restrict__ hist, int grid, int N,
+                              TruncRow* __restrict__ rows, int lo, int k, float p, int n) {
+  constexpr int NB = 1 << D;
+  static_assert(NB <= 32, "one bin per lane");
+  const int lane = threadIdx.x & 31, bin = lane % NB;
+  for (int row = blockIdx.x * 8 + (threadIdx.x >> 5); row < N; row += gridDim.x * 8) {
+    uint32_t c = 0u;
+    float m = 0.f;
+    for (int g = lane / NB; g < grid; g += 32 / NB) {
+      const HistBin h = hist[((size_t)g * N + row) * NB + bin];
+      c += h.cnt;
+      m += h.mass;
+    }
+#pragma unroll
+    for (int o = NB; o < 32; o <<= 1) {
+      c += __shfl_xor_sync(0xffffffffu, c, o);
+      m += __shfl_xor_sync(0xffffffffu, m, o);
+    }
+#pragma unroll
+    for (int o = 1; o < NB; o <<= 1) {           // suffix sums: bins >= bin
+      const uint32_t c2 = __shfl_down_sync(0xffffffffu, c, o, NB);
+      const float m2 = __shfl_down_sync(0xffffffffu, m, o, NB);
+      if (bin + o < NB) { c += c2; m += m2; }
+    }
+    const TruncRow r = rows[row];
+    const uint32_t C = r.above + c;
+    const float M = r.above_mass + m;
+    const bool ok = (k > 0 && C >= (uint32_t)k) || (p > 0.f && M >= p && C >= (uint32_t)n);
+    const uint32_t bal = __ballot_sync(0xffffffffu, ok && lane < NB);
+    const int b = bal ? 31 - __clz(bal) : 0;
+    const uint32_t ca = __shfl_sync(0xffffffffu, c, (b + 1) & (NB - 1));   // bins above b
+    const float ma = __shfl_sync(0xffffffffu, m, (b + 1) & (NB - 1));
+    if (lane == 0) {
+      TruncRow o = r;
+      o.prefix |= (uint32_t)b << lo;
+      if (b + 1 < NB) { o.above += ca; o.above_mass += ma; }
+      rows[row] = o;
+    }
+  }
+}
+
 // dynamic shared memory of px_full_softmax_lse_kernel<·, kc> at kb K-blocks: alignment slack,
 // table block, X ring, bias and barriers; the top-k kernels (kc > 0) add the block's global ids,
 // and a candidate list and a copy of the row's list per consumer quad; the gradient kernels
-// (grad) the block's column sums
-constexpr int ev_smem_bytes(int kb, int kc, bool grad = false) {
+// (grad) the block's column sums; the histogram kernels (bins = 2^d) the bins of one row per
+// consumer lane
+constexpr int ev_smem_bytes(int kb, int kc, bool grad = false, int bins = 0) {
   return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8 +
          (kc > 0 ? EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0) +
-         (grad ? EV_BV * 4 : 0);
+         (grad ? EV_BV * 4 : 0) + 2 * 128 * bins * (int)sizeof(HistBin);
 }
 static_assert(ev_smem_bytes(EV_KMAX / BK, 0) == 198208, "log-sum-exp shared memory at K = 512");
 static_assert(ev_smem_bytes(EV_KMAX / BK, 32) <= 227 * 1024, "top-k shared memory");
+static_assert(ev_smem_bytes(EV_KMAX / BK, 0, false, 1 << EV_RADIX_BITS) <= 227 * 1024,
+              "histogram shared memory");
 
 }  // namespace tc
 
@@ -593,19 +779,21 @@ int ev_combine_blocks(int N) {
   return blocks > PX_NUM_SMS * 8 ? PX_NUM_SMS * 8 : blocks;
 }
 
-template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false>
-void ev_launch(int grid, const CUtensorMap& tx, const tc::EvalParams<KC, SAMPLE, GRAD>& a,
-               cudaStream_t stream) {
+template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false, int HIST = 0,
+          bool MASK = false>
+void ev_launch(int grid, const CUtensorMap& tx,
+               const tc::EvalParams<KC, SAMPLE, GRAD, HIST, MASK>& a, cudaStream_t stream) {
   using namespace tc;
+  constexpr int bins = HIST ? 1 << HIST : 0;
   static bool set = false;
   if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD>,
+    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD, HIST, MASK>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         ev_smem_bytes(EV_KMAX / BK, KC, GRAD));
+                         ev_smem_bytes(EV_KMAX / BK, KC, GRAD, bins));
     set = true;
   }
-  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD>
-      <<<grid, THREADS, ev_smem_bytes(a.kb, KC, GRAD), stream>>>(tx, a);
+  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD, HIST, MASK>
+      <<<grid, THREADS, ev_smem_bytes(a.kb, KC, GRAD, bins), stream>>>(tx, a);
 }
 
 template <typename BiasT>
@@ -621,25 +809,26 @@ void ev_nll(int grid, const CUtensorMap& tx, const tc::EvalArgs& a, const void* 
 }
 
 // the list capacity is k rounded up to 8, 16 or 32
-template <typename BiasT, bool SAMPLE>
-void ev_topk(int grid, const CUtensorMap& tx, const tc::EvalParams<8, SAMPLE>& a,
+template <typename BiasT, bool SAMPLE, bool MASK = false>
+void ev_topk(int grid, const CUtensorMap& tx, const tc::EvalParams<8, SAMPLE, false, 0, MASK>& a,
              cudaStream_t stream) {
-  if (a.k <= 8) ev_launch<BiasT, 8, SAMPLE>(grid, tx, a, stream);
-  else if (a.k <= 16) ev_launch<BiasT, 16, SAMPLE>(grid, tx, a, stream);
-  else ev_launch<BiasT, 32, SAMPLE>(grid, tx, a, stream);
+  if (a.k <= 8) ev_launch<BiasT, 8, SAMPLE, false, 0, MASK>(grid, tx, a, stream);
+  else if (a.k <= 16) ev_launch<BiasT, 16, SAMPLE, false, 0, MASK>(grid, tx, a, stream);
+  else ev_launch<BiasT, 32, SAMPLE, false, 0, MASK>(grid, tx, a, stream);
 }
 
-// px_full_softmax_topk (SAMPLE = false: inv_tau, seed and row0 unused) and px_full_softmax_sample
-template <bool SAMPLE>
+// px_full_softmax_topk (SAMPLE = false: inv_tau, seed and row0 unused), px_full_softmax_sample
+// and px_full_softmax_sample_masked (MASK: rows holds each row's threshold)
+template <bool SAMPLE, bool MASK = false>
 int ev_lists(const void* X, int N, int K, const void* w_ptrs, int w_pitch, const void* b_ptrs,
              int b_pitch, int b_bf16, const int* row_cnt, const int* part_idx, int slots,
              const GroupGeom* g, int rank, const void* hdr_mine, const void* ctl, int wait,
              void* ws, int ws_ctas, int k, void* tk, float* log_probs, long long* ids,
-             float inv_tau, uint32_t seed, int row0, cudaStream_t stream) {
+             float inv_tau, uint32_t seed, int row0, const void* rows, cudaStream_t stream) {
   using namespace tc;
   if (N <= 0) return 0;
   if (ws_ctas > 32 * TK_LISTS_PER_LANE) return -2;
-  SampleArgs a;
+  MaskArgs a;
   CUtensorMap tx;
   int grid;
   int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
@@ -647,10 +836,25 @@ int ev_lists(const void* X, int N, int K, const void* w_ptrs, int w_pitch, const
   if (rc) return rc;
   a.tk = (TopkEntry*)tk; a.part_idx = part_idx; a.g = *g; a.k = k;
   a.inv_tau = inv_tau; a.seed = seed; a.row0 = row0;
-  (b_bf16 ? ev_topk<__nv_bfloat16, SAMPLE> : ev_topk<float, SAMPLE>)(grid, tx, a, stream);
+  a.rows = (const TruncRow*)rows;
+  (b_bf16 ? ev_topk<__nv_bfloat16, SAMPLE, MASK> : ev_topk<float, SAMPLE, MASK>)(grid, tx, a,
+                                                                                 stream);
   px_full_softmax_topk_combine_kernel<SAMPLE><<<ev_combine_blocks(N), 256, 0, stream>>>(
       (const float2*)ws, (const TopkEntry*)tk, grid, N, k, log_probs, ids, seed, row0);
   return (int)cudaGetLastError();
+}
+
+// the setup of px_full_softmax_sample_lse and px_full_softmax_radix: ev_setup and inv_tau
+int ev_temp_setup(tc::TempArgs& a, CUtensorMap& tx, int& grid, const void* X, int N, int K,
+                  const void* w_ptrs, int w_pitch, const void* b_ptrs, int b_pitch, int b_bf16,
+                  const int* row_cnt, int slots, const GroupGeom* g, int rank,
+                  const void* hdr_mine, const void* ctl, int wait, void* ws, int ws_ctas,
+                  float inv_tau) {
+  if (!(inv_tau > 0.f) || !isfinite(inv_tau)) return -4;
+  const int rc = ev_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                          slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas);
+  a.inv_tau = inv_tau;
+  return rc;
 }
 
 }  // namespace
@@ -702,7 +906,7 @@ int px_full_softmax_topk(const void* X, int N, int K, const void* w_ptrs, int w_
   if (k < 1 || k > 32) return -3;
   return ev_lists<false>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt, part_idx,
                          slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, k, tk, log_probs, ids,
-                         1.f, 0u, 0, stream);
+                         1.f, 0u, 0, nullptr, stream);
 }
 
 // n draws without replacement from softmax((X w^T + b) / τ) for each row of X [N, K], in draw
@@ -723,7 +927,84 @@ int px_full_softmax_sample(const void* X, int N, int K, const void* w_ptrs, int 
   if (!(inv_tau > 0.f) || !isfinite(inv_tau)) return -4;
   return ev_lists<true>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt, part_idx,
                         slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, n, tk, log_probs, ids,
-                        inv_tau, seed, row0, stream);
+                        inv_tau, seed, row0, nullptr, stream);
+}
+
+// Truncated sampling, pass 1: the log-sum-exp of s = fp32 logit · inv_tau of each row of X [N, K]
+// into rows [N] (16-byte TruncRow: prefix, above, above_mass, lse), whose threshold search it
+// starts.  Arguments as px_full_softmax_nll up to ws_ctas, plus inv_tau (fp32(1/τ)).
+// Returns 0, a negative argument error (-4: inv_tau not finite and > 0), or a CUDA error code.
+int px_full_softmax_sample_lse(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                               const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                               int slots, const GroupGeom* g, int rank, const void* hdr_mine,
+                               const void* ctl, int wait, void* ws, int ws_ctas, float inv_tau,
+                               void* rows, cudaStream_t stream) {
+  using namespace tc;
+  if (N <= 0) return 0;
+  TempArgs a;
+  CUtensorMap tx;
+  int grid;
+  int rc = ev_temp_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                         slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, inv_tau);
+  if (rc) return rc;
+  (b_bf16 ? ev_launch<__nv_bfloat16, 0, true> : ev_launch<float, 0, true>)(grid, tx, a, stream);
+  px_full_softmax_trunc_init_kernel<<<ev_combine_blocks(N), 256, 0, stream>>>(
+      (const float2*)ws, grid, N, (TruncRow*)rows);
+  return (int)cudaGetLastError();
+}
+
+// Truncated sampling, one radix pass: the histogram of the d-bit digit at bit lo (d =
+// EV_RADIX_BITS; lo = 32 − d, 32 − 2d, ..., 0 in turn) of the keys that match each row's prefix,
+// into hist [ws_ctas][N][2^d] 8-byte (count, mass) bins, then the digit of θ* into rows.  After the
+// pass at lo = 0, rows[].prefix is the key of θ*.  Arguments as px_full_softmax_sample_lse, hist
+// in place of ws, plus
+//   k: top_k, 0 for none, else in [n, V];   p: top_p, 0 for none, else in (0, 1];
+//   n: the number of samples, in [1, 32].
+// Returns 0, a negative argument error (-2: lo not a digit position, -3: n out of range, -4:
+// inv_tau not finite and > 0, -5: k out of range, -6: p out of range), or a CUDA error code.
+int px_full_softmax_radix(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                          const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                          int slots, const GroupGeom* g, int rank, const void* hdr_mine,
+                          const void* ctl, int wait, void* hist, int ws_ctas, float inv_tau,
+                          void* rows, int lo, int k, float p, int n, cudaStream_t stream) {
+  using namespace tc;
+  constexpr int D = EV_RADIX_BITS;
+  if (lo < 0 || lo > 32 - D || lo % D) return -2;
+  if (n < 1 || n > 32) return -3;
+  if (k != 0 && (k < n || k > g->V)) return -5;
+  if (!(p >= 0.f && p <= 1.f)) return -6;
+  if (N <= 0) return 0;
+  HistArgs a;
+  CUtensorMap tx;
+  int grid;
+  int rc = ev_temp_setup(a, tx, grid, X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                         slots, g, rank, hdr_mine, ctl, wait, nullptr, ws_ctas, inv_tau);
+  if (rc) return rc;
+  a.rows = (const TruncRow*)rows; a.hist = (HistBin*)hist; a.lo = lo;
+  a.himask = lo + D >= 32 ? 0u : ~0u << (lo + D);
+  (b_bf16 ? ev_launch<__nv_bfloat16, 0, true, false, D> : ev_launch<float, 0, true, false, D>)(
+      grid, tx, a, stream);
+  px_full_softmax_select_kernel<D><<<ev_combine_blocks(N), 256, 0, stream>>>(
+      (const HistBin*)hist, grid, N, (TruncRow*)rows, lo, k, p, n);
+  return (int)cudaGetLastError();
+}
+
+// Truncated sampling, last pass: px_full_softmax_sample restricted to each row's T, the words
+// whose key of s is >= rows[].prefix after the last radix pass (the −inf keys of the rest are
+// set after the (max, Σexp) pairs, so log_probs are those of the untruncated softmax).  Arguments
+// and return codes as px_full_softmax_sample, plus rows.  T must hold at least n words.
+int px_full_softmax_sample_masked(const void* X, int N, int K, const void* w_ptrs, int w_pitch,
+                                  const void* b_ptrs, int b_pitch, int b_bf16, const int* row_cnt,
+                                  const int* part_idx, int slots, const GroupGeom* g, int rank,
+                                  const void* hdr_mine, const void* ctl, int wait, void* ws,
+                                  int ws_ctas, int n, void* tk, float* log_probs, long long* ids,
+                                  float inv_tau, unsigned int seed, int row0, const void* rows,
+                                  cudaStream_t stream) {
+  if (n < 1 || n > 32) return -3;
+  if (!(inv_tau > 0.f) || !isfinite(inv_tau)) return -4;
+  return ev_lists<true, true>(X, N, K, w_ptrs, w_pitch, b_ptrs, b_pitch, b_bf16, row_cnt,
+                              part_idx, slots, g, rank, hdr_mine, ctl, wait, ws, ws_ctas, n, tk,
+                              log_probs, ids, inv_tau, seed, row0, rows, stream);
 }
 
 // The gradient of the full-softmax NLL over one chunk of the table, global ids [v0, v0 + rows):

@@ -249,16 +249,19 @@ def _ordered_top(keys, k):
     return top
 
 
-def full_softmax_sample(inputs, weight, bias, n, inv_tau, seed):
+def full_softmax_sample(inputs, weight, bias, n, inv_tau, seed, top_k=None, top_p=None):
     """``(log_probs [N, n], ids [N, n])``: n draws without replacement from the tempered full
-    softmax of each row, in draw order (the n largest Gumbel keys).  Fused where
+    softmax of each row, in draw order (the n largest Gumbel keys), truncated to each row's top
+    `top_k` / nucleus `top_p` when given (`truncation_threshold`).  Fused where
     `_fused_eval_group` finds a group and n <= 32; everything else (and training) runs
     `full_softmax_sample_composition`.  Both take the same keys, so they draw the same ids
     except where two keys are within a few ulp."""
     grp = _fused_eval_group(inputs, weight, bias)
     if grp is not None and n <= FUSED_TOPK_MAX:
-        return grp.full_softmax_sample(inputs, n, inv_tau, seed)
-    return full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed)
+        if top_k is None and top_p is None:
+            return grp.full_softmax_sample(inputs, n, inv_tau, seed)
+        return grp.full_softmax_sample(inputs, n, inv_tau, seed, top_k=top_k, top_p=top_p)
+    return full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed, top_k, top_p)
 
 
 def sample_uniform(seed, rows, gids):
@@ -286,11 +289,42 @@ def sample_log_e(seed, rows, gids):
 _NOISE_CHUNK = 1 << 24
 
 
-def full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed):
+def truncation_threshold(s, n, top_k=None, top_p=None):
+    """fp32 [N]: each row's θ* of truncated sampling over the scaled logits `s` [N, V] (fp32):
+    the largest θ with ``count(θ) >= top_k`` or ``(mass(θ) >= top_p and count(θ) >= n)``, where
+    count(θ) and mass(θ) are the number and the softmax(s) mass of the row's s >= θ (an absent
+    argument makes its clause false; −0 equals +0, as in fp32 comparison).  A row keeps T = {v :
+    s_v >= θ*}.  Sort-based in row chunks: s is sorted per row, the masses are fp64, and every
+    position of a run of equal values takes the run's count and mass, so ties are kept together.
+    −inf where the predicate never holds (every word kept)."""
+    N, V = s.shape
+    out = torch.empty(N, dtype=torch.float32, device=s.device)
+    step = max(1, _NOISE_CHUNK // max(V, 1))
+    with torch.no_grad():
+        for r0 in range(0, N, step):
+            vals = torch.sort(s[r0:r0 + step].detach().float(), dim=1, descending=True).values
+            q = torch.softmax(vals.double(), dim=1)
+            mass = torch.cumsum(q, dim=1)
+            neg = (-vals).contiguous()                       # ascending
+            end = torch.searchsorted(neg, neg, right=True) - 1   # last position of each run
+            cnt, m = end + 1, mass.gather(1, end)
+            ok = torch.zeros_like(cnt, dtype=torch.bool)
+            if top_k is not None:
+                ok |= cnt >= top_k
+            if top_p is not None:
+                ok |= (m >= top_p) & (cnt >= n)
+            th = vals.gather(1, ok.int().argmax(1, keepdim=True))[:, 0]   # the first that holds
+            out[r0:r0 + step] = torch.where(ok.any(1), th, -float("inf"))
+    return out
+
+
+def full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed, top_k=None,
+                                    top_p=None):
     """The unfused sampler: gather every row, materialise the [N, V] logits, scale them by
     `inv_tau` and take `log_softmax`; the keys s − log E come from the torch noise in row chunks,
     and the ids are each row's n best keys by (key descending, id ascending) (`_ordered_top`).
-    Gradients flow into `log_probs`."""
+    With `top_k` / `top_p` the keys of s below the row's `truncation_threshold` are −inf first;
+    `log_probs` stay those of the untruncated softmax.  Gradients flow into `log_probs`."""
     s = _gathered_logits(inputs, weight, bias) * inv_tau
     lp = torch.log_softmax(s, dim=-1)
     N, V = s.shape
@@ -301,6 +335,9 @@ def full_softmax_sample_composition(inputs, weight, bias, n, inv_tau, seed):
         for r0 in range(0, N, step):
             rows = torch.arange(r0, min(N, r0 + step), device=s.device)
             keys[r0:r0 + step] -= sample_log_e(seed, rows, gids)
+        if top_k is not None or top_p is not None:
+            th = truncation_threshold(s, n, top_k, top_p)
+            keys.masked_fill_(s.detach() < th[:, None], -float("inf"))
         top = _ordered_top(keys, n)
     return lp.gather(1, top), top
 

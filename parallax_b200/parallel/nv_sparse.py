@@ -26,6 +26,7 @@ Reference semantics kept (file:line in /root/reference/parallax/parallax):
   replay shapes are static.
 """
 import ctypes
+import numbers
 
 import torch
 
@@ -733,19 +734,41 @@ class NVSparseGroup(object):
         per-CTA lists fit in `consts.TOPK_WS_BYTES`.  One-sided: no other rank takes part."""
         return self._ranked(x, k, "full_softmax_topk", "k")
 
-    def full_softmax_sample(self, x, n, inv_tau, seed):
+    def full_softmax_sample(self, x, n, inv_tau, seed, top_k=None, top_p=None):
         """n draws without replacement from ``softmax((x @ W.T + b) · inv_tau)`` for each row
         of bf16 inputs `x` [N, K], in draw order: ``(log_probs fp32 [N, n], ids int64 [N, n])``,
         where log_probs are the tempered log-probabilities of the ids.  The kernel keeps the n
         largest Gumbel keys ``s − log E`` of each row (s the scaled fp32 logit, E the noise of
         (seed, row, id), `engine.sample_log_e`), so the draws depend on the seed, the row's
         index in `x` and the ids only.  1 <= n <= 32, inv_tau = fp32(1/τ) > 0, seed in
-        [0, 2^32).  Chunked, one-sided and fresh as `full_softmax_topk`."""
-        return self._ranked(x, n, "full_softmax_sample", "num_samples", (inv_tau, seed))
+        [0, 2^32).  Chunked, one-sided and fresh as `full_softmax_topk`.
 
-    def _ranked(self, x, k, what, k_name, sample=None):
+        `top_k` (an int in [n, V]) and `top_p` (a real in (0, 1]) truncate each row to T = {v :
+        s_v >= θ*}, θ* the largest θ with count(θ) >= top_k or (mass(θ) >= top_p and count(θ)
+        >= n) (`parallax.nn.full_softmax_sample`); the draws are the n best keys within T and
+        log_probs stay those of the untruncated softmax.  Per row chunk: one log-sum-exp pass,
+        32 / `consts.SAMPLE_RADIX_BITS` histogram passes that find θ*, and the sampling pass
+        with keys below θ* dropped, each reading the table once."""
+        trunc = None
+        if top_k is not None or top_p is not None:
+            V = self.tables[0].V
+            if top_k is not None and (isinstance(top_k, bool) or not isinstance(top_k, int) or
+                                      not n <= top_k <= V):
+                raise ValueError("full_softmax_sample: top_k must be an int in [num_samples, "
+                                 "%d], got %r" % (V, top_k))
+            if top_p is not None and (isinstance(top_p, bool) or
+                                      not isinstance(top_p, numbers.Real) or
+                                      not 0.0 < top_p <= 1.0):
+                raise ValueError("full_softmax_sample: top_p must be a real number in (0, 1], "
+                                 "got %r" % (top_p,))
+            trunc = (top_k or 0, 0.0 if top_p is None else float(top_p))
+        return self._ranked(x, n, "full_softmax_sample", "num_samples", (inv_tau, seed), trunc)
+
+    def _ranked(self, x, k, what, k_name, sample=None, trunc=None):
         """The list-keeping eval kernels: top-k (`sample` None) or sampling (`sample` =
-        (inv_tau, seed)), in row chunks whose per-CTA lists fit in `consts.TOPK_WS_BYTES`."""
+        (inv_tau, seed)), truncated when `trunc` = (top_k or 0, top_p or 0), in row chunks
+        whose per-CTA lists (and digit bins, which reuse their memory) fit in
+        `consts.TOPK_WS_BYTES`."""
         L = ops.lib()
         V = self.tables[0].V
         if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, V):
@@ -759,10 +782,13 @@ class NVSparseGroup(object):
             return log_probs, ids
         _, part = self._slot_maps()
         ctas = consts.NUM_SMS
-        chunk = max(128, consts.TOPK_WS_BYTES // (ctas * k * 8) // 128 * 128)
+        d = consts.SAMPLE_RADIX_BITS
+        per_row = max(k, 1 << d) if trunc else k          # 8-byte entries per (CTA, row)
+        chunk = max(128, consts.TOPK_WS_BYTES // (ctas * per_row * 8) // 128 * 128)
         chunk = min(chunk, n)
         ws = torch.empty(ctas * chunk * 2, dtype=torch.float32, device=self.device)
-        tk = torch.empty(ctas * chunk * k * 2, dtype=torch.int32, device=self.device)
+        tk = torch.empty(ctas * chunk * per_row * 2, dtype=torch.int32, device=self.device)
+        rows = torch.empty(chunk * 4, dtype=torch.int32, device=self.device) if trunc else None
         for r0 in range(0, n, chunk):
             m = min(chunk, n - r0)
             args = (_vp(x[r0:].data_ptr()), m, K, *head, _vp(part.data_ptr()), *tail,
@@ -771,8 +797,22 @@ class NVSparseGroup(object):
             _count(2)
             if sample is None:
                 rc = L.px_full_softmax_topk(*args, stream)
-            else:
+            elif trunc is None:
                 rc = L.px_full_softmax_sample(*args, sample[0], sample[1], r0, stream)
+            else:
+                # θ* of every row of the chunk (into `rows`), then the masked sampling pass
+                common = (_vp(x[r0:].data_ptr()), m, K, *head, *tail)
+                ops.check(L.px_full_softmax_sample_lse(
+                    *common, _vp(ws.data_ptr()), ctas, sample[0], _vp(rows.data_ptr()), stream),
+                    what)
+                for lo in range(32 - d, -1, -d):
+                    _count(2)
+                    ops.check(L.px_full_softmax_radix(
+                        *common, _vp(tk.data_ptr()), ctas, sample[0], _vp(rows.data_ptr()), lo,
+                        trunc[0], trunc[1], k, stream), what)
+                _count(2)
+                rc = L.px_full_softmax_sample_masked(*args, sample[0], sample[1], r0,
+                                                     _vp(rows.data_ptr()), stream)
             ops.check(rc, what)
         return log_probs, ids
 

@@ -6,6 +6,7 @@ gather + matmul + log_softmax + noise + top-n composition against the fused samp
 (`parallax.nn.full_softmax_sample`), next to the fused top-k at the same n and the fused NLL.
 
     python tools/bench_full_softmax.py [--n 640 2560] [--k 1 10 32] [--sample 1 10 32]
+                                       [--trunc 1 10] [--top_k 40] [--top_p 0.9 0.95]
                                        [--temperature 1.0] [--out result.json]
 
 Builds LM1B's (softmax_w, softmax_b) co-lookup group through the engine on the NVLink fabric,
@@ -21,6 +22,10 @@ one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N:
   top-k at k = n and the fused NLL alternate over the rounds, and the composition is timed after
   them.  The records carry the share of first draws equal to the composition's (same seed; its
   logits are rounded to bf16, so keys closer than that may swap).
+- truncated sampling, for each n of --trunc (default none) and each truncation of --top_k
+  (alone) and --top_p (each alone): the fused truncated sampler, the fused untruncated sampler
+  at the same n and the fused NLL alternate over the rounds, and the truncated composition is
+  timed after them.  The records carry the share of rows whose draws equal the composition's.
 Per arm: ms per call (CUDA events, after warm-up), the growth of `torch.cuda.max_memory_allocated`
 during one call, and the achieved TFLOP/s from 2·N·V·K.  The card name, power limit and max SM
 clock are read in the same run.
@@ -86,6 +91,9 @@ def main():
     ap.add_argument("--n", type=int, nargs="+", default=[640, 2560])
     ap.add_argument("--k", type=int, nargs="*", default=[1, 10, 32])
     ap.add_argument("--sample", type=int, nargs="*", default=[])
+    ap.add_argument("--trunc", type=int, nargs="*", default=[])
+    ap.add_argument("--top_k", type=int, default=40)
+    ap.add_argument("--top_p", type=float, nargs="*", default=[0.9, 0.95])
     ap.add_argument("--temperature", type=float, default=1.0)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--comp_iters", type=int, default=2)
@@ -112,8 +120,7 @@ def main():
         ms, grow = timing
         med = statistics.median(ms)
         r = {"arm": arm, "N": n, **({} if k is None else {"k": k}), "V": V, "K": K,
-             **({} if k is None or not arm.endswith("sample") else
-                {"temperature": a.temperature}),
+             **({} if k is None or "sample" not in arm else {"temperature": a.temperature}),
              "ms": round(med, 3), "ms_all": [round(v, 3) for v in ms],
              "mem_growth_MB": round(grow / 2 ** 20, 1),
              "tflops": round(2.0 * n * V * K / (med * 1e-3) / 1e12, 1), **(extra or {}),
@@ -178,6 +185,33 @@ def main():
                 nl = report("fused_nll", n, res["fused_nll"], k)
                 print(json.dumps({"N": n, "n": k, "sample_over_topk": round(sm / tk, 3),
                                   "sample_over_nll": round(sm / nl, 3)}), flush=True)
+            truncs = ([{"top_k": a.top_k}] if a.top_k else []) + [{"top_p": p} for p in a.top_p]
+            for k in a.trunc:
+                for tr in truncs:
+                    trs = lambda: parallax.nn.full_softmax_sample(    # noqa: E731
+                        x, w, b, k, a.temperature, 12345, **tr)
+                    smp = lambda: parallax.nn.full_softmax_sample(    # noqa: E731
+                        x, w, b, k, a.temperature, 12345)
+                    tcomp = lambda: full_softmax_sample_composition(  # noqa: E731
+                        x, w, b, k, inv_tau, 12345, tr.get("top_k"), tr.get("top_p"))
+                    ids, cids = trs()[1], tcomp()[1]
+                    agree = {**tr, "rows_equal": round(float((ids == cids).all(1).float()
+                                                             .mean()), 4)}
+                    del ids, cids
+                    res = alternate([("fused_trunc_sample", trs, a.iters),
+                                     ("fused_sample", smp, a.iters),
+                                     ("fused_nll", nll, a.iters),
+                                     ("composition_trunc_sample", tcomp, a.comp_iters)],
+                                    a.rounds)
+                    report("composition_trunc_sample", n, res["composition_trunc_sample"], k,
+                           tr)
+                    tt = report("fused_trunc_sample", n, res["fused_trunc_sample"], k, agree)
+                    sm = report("fused_sample", n, res["fused_sample"], k)
+                    nl = report("fused_nll", n, res["fused_nll"], k)
+                    cm = statistics.median(res["composition_trunc_sample"][0])
+                    print(json.dumps({"N": n, "n": k, **tr, "trunc_over_sample": round(tt / sm, 3),
+                                      "trunc_over_nll": round(tt / nl, 3),
+                                      "composition_over_trunc": round(cm / tt, 2)}), flush=True)
     sess.close()
     if a.out:
         with open(a.out, "w") as f:
