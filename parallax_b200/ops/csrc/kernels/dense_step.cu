@@ -615,8 +615,10 @@ int px_dense_async(const void* my_grads, void* my_params, const void* const* mas
   return (int)cudaGetLastError();
 }
 
+// n must be a multiple of 16/sizeof(T): the kernel reads whole 16-byte vectors only
 int px_sumsq(const void* x, size_t n, int dtype, float mul, float* out, cudaStream_t stream) {
   const int vn = dtype == 0 ? 4 : 8;
+  if (n % vn != 0) return -1;
   const int blocks = px_clamp_blocks(n / vn, 512 * 4, PX_NUM_SMS * 2);
   if (dtype == 0) px_sumsq_kernel<float><<<blocks, 512, 0, stream>>>((const float*)x, n, mul, out);
   else px_sumsq_kernel<__nv_bfloat16><<<blocks, 512, 0, stream>>>((const __nv_bfloat16*)x, n, mul, out);

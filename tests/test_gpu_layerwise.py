@@ -46,7 +46,7 @@ def _layout(items, world, vn):
     return out, (off + q - 1) // q * q
 
 
-@pytest.mark.parametrize("world", [1, 2, 4, 8])
+@pytest.mark.parametrize("world", [1, 2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("variant", ["lars", "lars_nesterov", "lamb"])
 def test_passes_match_oracle(world, dtype, variant):

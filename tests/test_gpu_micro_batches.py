@@ -52,7 +52,7 @@ def _slot_args(s):
             s[2] if len(s) > 2 else None)
 
 
-@pytest.mark.parametrize("world", [1, 2, 4, 8])
+@pytest.mark.parametrize("world", [1, 2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("opt_name", ["sgd", "adagrad", "adam", "ftrl"])
 def test_accumulate_then_fused_step(world, dtype, opt_name):

@@ -55,8 +55,8 @@ def _full(tabs, V, D):
     return out
 
 
-@pytest.mark.parametrize("world,P,strategy", [(1, 1, "mod"), (2, 5, "mod"),
-                                              (4, 8, "div"), (8, 32, "mod")])
+@pytest.mark.parametrize("world,P,strategy", [(1, 1, "mod"), (2, 5, "mod"), (3, 8, "mod"),
+                                              (4, 8, "div"), (5, 8, "div"), (8, 32, "mod")])
 @pytest.mark.parametrize("D", [1, 4, 64, 130])
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
 def test_lookup_matches_index_select(world, P, strategy, D, out_dtype):
@@ -83,8 +83,9 @@ def test_lookup_matches_index_select(world, P, strategy, D, out_dtype):
         f.close()
 
 
-@pytest.mark.parametrize("world,run_option", [(1, "HYBRID"), (2, "HYBRID"),
-                                              (4, "PS"), (4, "MPI"), (8, "HYBRID")])
+@pytest.mark.parametrize("world,run_option", [(1, "HYBRID"), (2, "HYBRID"), (3, "HYBRID"),
+                                              (4, "PS"), (4, "MPI"), (6, "HYBRID"),
+                                              (8, "HYBRID")])
 @pytest.mark.parametrize("kind", ["sgd", "adagrad", "adam"])
 @pytest.mark.parametrize("local_agg", [True, False])
 def test_push_claim_apply(world, run_option, kind, local_agg):

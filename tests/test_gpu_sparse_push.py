@@ -132,15 +132,16 @@ def _push_check_apply(groups, inputs, step, V, scale, overflow=False):
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize("world,run_option", [(2, "HYBRID"), (4, "HYBRID"),
-                                              (2, "MPI"), (4, "MPI")])
+@pytest.mark.parametrize("world,run_option", [(2, "HYBRID"), (3, "HYBRID"), (4, "HYBRID"),
+                                              (6, "HYBRID"), (2, "MPI"), (4, "MPI")])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("boundary", [True, False])
 @pytest.mark.parametrize("local_agg", [True, False])
 @pytest.mark.parametrize("D,scale", [(36, 0.5), (64, 1.0), (64, 0.5)])
 def test_push_rings_exact(world, run_option, dtype, boundary, local_agg, D, scale):
     """D = 36 ships through the generic float4 path, D = 64 (bf16 wire, partitioned) through
-    16-byte copies; fp32 wire unless bf16 gradients cross with the boundary optimisation."""
+    16-byte copies; fp32 wire unless bf16 gradients cross with the boundary optimisation.
+    W = 3 and 6 place the P = 8 partitions unevenly over the owners."""
     V, n = 503, 300
     fabs, groups, _ = _groups(world, [D], optim.Adagrad(0.2, 1.0), run_option=run_option,
                               scale=scale, boundary=boundary, local_agg=local_agg, V=V)
