@@ -1012,8 +1012,8 @@ int px_full_softmax_sample_masked(const void* X, int N, int K, const void* w_ptr
 //   db [rows] fp32       = Σ_i G[i][v]
 // X [N, K] bf16 as px_full_softmax_nll; wc / bc: the chunk's bf16 weight rows and bias rows (fp32,
 // or bf16 when b_bf16), row pitches w_pitch / b_pitch elements as px_full_softmax_nll; lse, g fp32
-// [N] and targets int64 [N].  Columns of G from rows to g_pitch are written as zero; g_pitch >=
-// rows rounded up to 128 and even.  The grid is at most ctas CTAs.
+// [N] and targets int64 [N].  Columns of G from rows to rows rounded up to 128 are written as zero,
+// later ones are not written; g_pitch >= rows rounded up to 128, even.  Grid <= ctas CTAs.
 // Returns 0, a negative argument error, or a CUDA error code.
 int px_full_softmax_grad(const void* X, int N, int K, const void* wc, int w_pitch, const void* bc,
                          int b_pitch, int b_bf16, int rows, long long v0, const float* lse,

@@ -175,7 +175,7 @@ def test_no_logits_buffer():
 
 
 # ------------------------------------------------------------------ top-k
-@pytest.mark.parametrize("k", [1, 5, 32])
+@pytest.mark.parametrize("k", [1, 5, 9, 16, 17, 32])
 @pytest.mark.parametrize("world,V,P,strategy,K,N,replicated", CASES)
 def test_topk_kernel_matches_fp64_reference(world, V, P, strategy, K, N, replicated, k):
     Wt, Bt = _table(V, K, world * 10 + P)

@@ -50,7 +50,7 @@ def _check(lp, ids, ref, n, V, margin=2e-3):
 
 
 @pytest.mark.parametrize("tau", [0.7, 1.0, 1.5])
-@pytest.mark.parametrize("n", [1, 5, 32])
+@pytest.mark.parametrize("n", [1, 5, 12, 32])
 @pytest.mark.parametrize("world,V,P,strategy,K,N,replicated", CASES)
 def test_sample_kernel_matches_fp64_reference(world, V, P, strategy, K, N, replicated, n, tau):
     Wt, Bt = _table(V, K, world * 10 + P)

@@ -99,7 +99,7 @@ def _check_threshold(th, lse, s, n, top_k, top_p, min_checked=0.6):
     return int((~clear).sum())
 
 
-MODES = [(1, 40, None), (1, None, 0.9), (3, None, 0.5), (2, 40, 0.9)]
+MODES = [(1, 40, None), (1, None, 0.9), (3, None, 0.5), (2, 40, 0.9), (12, 40, 0.9)]
 
 
 @pytest.mark.parametrize("n,top_k,top_p", MODES)
@@ -184,7 +184,7 @@ def test_top_k_v_is_the_untruncated_sample_bit_for_bit():
     fabs, groups = _groups(4, Wt, Bt, 7, "div")
     x = torch.randn(N, K, generator=torch.Generator().manual_seed(9)).bfloat16().cuda()
     for grp in (groups[0], groups[3]):
-        for n in (1, 32):
+        for n in (1, 12, 32):                # list capacities 8, 16 and 32
             lp, ids = grp.full_softmax_sample(x, n, _inv(0.7), 11, top_k=V)
             lp0, ids0 = grp.full_softmax_sample(x, n, _inv(0.7), 11)
             assert torch.equal(ids, ids0) and torch.equal(lp, lp0)
