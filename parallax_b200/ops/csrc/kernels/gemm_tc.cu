@@ -18,6 +18,7 @@
 // second launch.  The reference reaches these products through cuBLAS
 // (tensorflow/core/kernels/matmul_op.cc:252-369 → cuda_blas.cc:2229).
 #include "wgmma.cuh"
+#include "lstm_cell.cuh"
 
 namespace tc {
 
@@ -94,6 +95,23 @@ __device__ __forceinline__ void cluster_sync_all() {
                "barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// Parks this consumer thread's accumulator fragment (see `mainloop`) as rows of a 128×BN fp32
+// tile at `park` (row stride BN+4 floats); ROUND: each value rounded to bf16 first.
+template <int BN, bool ROUND>
+__device__ __forceinline__ void park_acc(float* park, const float* acc) {
+  const int t = threadIdx.x - 128, lane = t & 31;
+  const int lrow = (t >> 5) * 16 + (lane >> 2);     // tile row of acc[j·4 + 0/1]; +8 for 2/3
+  const int lcol = (lane & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float2 v = make_float2(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1]);
+      if (ROUND) v = __bfloat1622float2(__floats2bfloat162_rn(v.x, v.y));
+      *reinterpret_cast<float2*>(park + (size_t)(lrow + 8 * h) * (BN + 4) + j * 8 + lcol) = v;
+    }
+}
+
 template <int BN, int STAGES, bool CLUSTER>
 __global__ void __launch_bounds__(THREADS, 1)
 px_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
@@ -127,16 +145,10 @@ px_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const int lcol = (lane & 3) * 2;
     const bool splitk = gridDim.z > 1;
     if (CLUSTER) {
-      // park the fp32 partial in shared memory (row stride BN+4 floats); every wgmma of both
-      // consumer warpgroups has retired before the stages are overwritten
+      // park the fp32 partial in shared memory; every wgmma of both consumer warpgroups has
+      // retired before the stages are overwritten
       consumer_sync();
-      float* park = reinterpret_cast<float*>(smem);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<float2*>(park + (size_t)(lrow + 8 * h) * (BN + 4) + j * 8 + lcol) =
-              make_float2(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1]);
+      park_acc<BN, false>(reinterpret_cast<float*>(smem), acc);
     } else {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -231,10 +243,128 @@ px_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
   }
 }
 
+// ------------------------------------------- LSTM recurrence: cell backward fused into dm
+//
+// One backward time step of the LSTMP recurrence in place of (dm = dh·W_P^T GEMM, cell kernel):
+// dm = dh · W_P^T (A = dh [M, P], Bt = W_P [S, P], both K-contiguous, K = P) with the cell
+// backward in the epilogue, so dm never makes a round trip through global memory.  While thread 0
+// streams the GEMM operands, warps 1-3 of the producer warpgroup copy the epilogue's operands for
+// the CTA's 128×BN tile (act, c_prev, c_new, dc) into shared memory with cp.async, so their load
+// latency hides under the GEMM.  The tile of dm is rounded to bf16 (what a bf16 GEMM would
+// store), parked in shared memory, and all 384 threads then run the cell backward over it in
+// 4-unit vectors, writing the four dgates columns and dc in place.
+struct CellBwdArgs {
+  float* dc;                    // [M, S] fp32: in dL/dc_new, out dL/dc_prev
+  const __nv_bfloat16* act;     // [M, 4S] σ(i) | tanh(j) | σ(f) | σ(o)
+  const float* c_prev;          // [M, S]
+  const float* c_new;           // [M, S]
+  __nv_bfloat16* dgates;        // [M, 4S]
+  int S, K;                     // K = P
+};
+
+__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(src)
+               : "memory");
+}
+
+template <int BN>
+__host__ __device__ constexpr int dm_cell_stages() { return BN >= 64 ? 2 : 4; }
+// epilogue operands in shared memory: act [4][128][BN] bf16, then c_prev, c_new, dc [128][BN] fp32
+template <int BN>
+__host__ __device__ constexpr int dm_cell_epi_bytes() { return 4 * BM * BN * 2 + 3 * BM * BN * 4; }
+
+template <int BN>
+__global__ void __launch_bounds__(THREADS, 1)
+px_lstm_dm_cell_bwd_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                           const __grid_constant__ CUtensorMap tmap_b, CellBwdArgs g) {
+  constexpr int STAGES = dm_cell_stages<BN>();
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  constexpr int STAGE_BYTES = BM * BK * 2 + BN * BK * 2;
+  static_assert(BM * (BN + 4) * 4 <= STAGES * STAGE_BYTES, "dm tile must fit the drained stages");
+  __nv_bfloat16* s_act = reinterpret_cast<__nv_bfloat16*>(smem + STAGES * STAGE_BYTES);
+  float* s_f32 = reinterpret_cast<float*>(s_act + 4 * BM * BN);   // c_prev | c_new | dc
+  uint64_t* full_bar =
+      reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + dm_cell_epi_bytes<BN>());
+  uint64_t* empty_bar = full_bar + STAGES;
+  const int n_tile = blockIdx.x, m_tile = blockIdx.y;
+  const int S = g.S, row0 = m_tile * BM, n0 = n_tile * BN;
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x >= 32 && threadIdx.x < 128) {
+    const int t = threadIdx.x - 32;
+    constexpr int ACH = BN * 2 / 16, FCH = BN * 4 / 16;   // 16-byte chunks per row segment
+    for (int i = t; i < 4 * BM * ACH; i += 96) {
+      const int q = i / (BM * ACH), r = (i / ACH) % BM, c = i % ACH;
+      cp_async_16(s_act + (size_t)(q * BM + r) * BN + c * 8,
+                  g.act + (size_t)(row0 + r) * 4 * S + (size_t)q * S + n0 + c * 8);
+    }
+    for (int i = t; i < 3 * BM * FCH; i += 96) {
+      const int a = i / (BM * FCH), r = (i / FCH) % BM, c = i % FCH;
+      const float* src = a == 0 ? g.c_prev : (a == 1 ? g.c_new : g.dc);
+      cp_async_16(s_f32 + (size_t)(a * BM + r) * BN + c * 4, src + (size_t)(row0 + r) * S + n0 + c * 4);
+    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+  }
+  float acc[BN / 2];
+  mainloop<BN, STAGES>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, 0, g.K / BK, row0, n0, acc);
+  float* park = reinterpret_cast<float*>(smem);
+  if (threadIdx.x >= 128) {
+    consumer_sync();                                // both warpgroups' wgmma have retired
+    park_acc<BN, true>(park, acc);
+  }
+  __syncthreads();
+  for (int v = threadIdx.x; v < BM * BN / 4; v += THREADS) {
+    const int r = v / (BN / 4), c4 = (v % (BN / 4)) * 4;
+    const size_t ci = (size_t)(row0 + r) * S + n0 + c4, gi = (size_t)(row0 + r) * 4 * S + n0 + c4;
+    const float4 dm4 = *reinterpret_cast<const float4*>(park + (size_t)r * (BN + 4) + c4);
+    const float4 cp4 = *reinterpret_cast<const float4*>(s_f32 + (size_t)r * BN + c4);
+    const float4 cn4 = *reinterpret_cast<const float4*>(s_f32 + (size_t)(BM + r) * BN + c4);
+    const float4 dc4 = *reinterpret_cast<const float4*>(s_f32 + (size_t)(2 * BM + r) * BN + c4);
+    float a[4][4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint2 w = *reinterpret_cast<const uint2*>(s_act + (size_t)(q * BM + r) * BN + c4);
+      const float2 lo = bf16x2_to_float2(w.x), hi = bf16x2_to_float2(w.y);
+      a[q][0] = lo.x; a[q][1] = lo.y; a[q][2] = hi.x; a[q][3] = hi.y;
+    }
+    const float dmv[4] = {dm4.x, dm4.y, dm4.z, dm4.w}, cp[4] = {cp4.x, cp4.y, cp4.z, cp4.w},
+                cn[4] = {cn4.x, cn4.y, cn4.z, cn4.w}, dci[4] = {dc4.x, dc4.y, dc4.z, dc4.w};
+    float dg[4][4], dco[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float ae[4] = {a[0][e], a[1][e], a[2][e], a[3][e]};
+      float dge[4];
+      dco[e] = lstm_cell_bwd_elem(ae, cp[e], cn[e], dmv[e], dci[e], dge);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) dg[q][e] = dge[q];
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      *reinterpret_cast<uint2*>(g.dgates + gi + (size_t)q * S) =
+          make_uint2(float2_to_bf16x2(dg[q][0], dg[q][1]), float2_to_bf16x2(dg[q][2], dg[q][3]));
+    *reinterpret_cast<float4*>(g.dc + ci) = make_float4(dco[0], dco[1], dco[2], dco[3]);
+  }
+}
+
 // ------------------------------------------------------------------ host side
 
 template <int BN, int STAGES>
 constexpr int smem_bytes() { return STAGES * (BM * BK * 2 + BN * BK * 2) + 1024 + 256; }
+
+// opt a kernel in to `bytes` of dynamic shared memory once
+template <auto Kernel>
+static void set_smem_once(int bytes) {
+  static bool done = false;
+  if (done) return;
+  cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  done = true;
+}
 
 }  // namespace tc
 
@@ -316,6 +446,38 @@ int px_gemm_tc(const void* A, const void* B, void* C, const void* addend, float*
     }
     px_gemm_tc_kernel<64, STAGES, false><<<grid, THREADS, SMEM, stream>>>(ta, tb, g);
   }
+  return (int)cudaGetLastError();
+}
+
+
+// One backward time step: dm = dh · W_P^T (dh [M, P], W_P [S, P]) with the cell backward in the
+// epilogue (see `px_lstm_dm_cell_bwd_kernel`).  bn: 16, 32 or 64 columns of dm per CTA.  Every
+// pointer 16-byte aligned.
+int px_lstm_dm_cell_bwd(const void* dh, const void* WP, float* dc, const void* act,
+                        const float* c_prev, const float* c_new, void* dgates, int M, int S, int P,
+                        int bn, cudaStream_t stream) {
+  using namespace tc;
+  if (M % BM || P % BK || (bn != 16 && bn != 32 && bn != 64) || S % bn) return -1;
+  for (const void* q : {dh, WP, (const void*)dc, act, (const void*)c_prev, (const void*)c_new,
+                        (const void*)dgates})
+    if ((uintptr_t)q % 16) return -1;
+  CUtensorMap ta, tb;
+  int rc = make_tmap(&ta, dh, M, P, BM);
+  if (rc) return rc;
+  rc = make_tmap(&tb, WP, S, P, bn);
+  if (rc) return rc;
+  CellBwdArgs g;
+  g.dc = dc; g.act = (const __nv_bfloat16*)act; g.c_prev = c_prev; g.c_new = c_new;
+  g.dgates = (__nv_bfloat16*)dgates; g.S = S; g.K = P;
+  dim3 grid(S / bn, M / BM);
+#define PX_DMB(BN_)                                                                            \
+  {                                                                                            \
+    constexpr int SMEM = smem_bytes<BN_, dm_cell_stages<BN_>()>() + dm_cell_epi_bytes<BN_>();  \
+    set_smem_once<px_lstm_dm_cell_bwd_kernel<BN_>>(SMEM);                                      \
+    px_lstm_dm_cell_bwd_kernel<BN_><<<grid, THREADS, SMEM, stream>>>(ta, tb, g);               \
+  }
+  if (bn == 16) PX_DMB(16) else if (bn == 32) PX_DMB(32) else PX_DMB(64)
+#undef PX_DMB
   return (int)cudaGetLastError();
 }
 

@@ -11,6 +11,7 @@
 //    sparse_xent_op_gpu.cu.cc, ≈15 elementwise passes over a [B·T, 8193] fp32
 //    tensor).
 #include "common.cuh"
+#include "lstm_cell.cuh"
 
 template <typename T> __device__ __forceinline__ float to_f(T v);
 template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
@@ -18,14 +19,6 @@ template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v
 template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
-__device__ __forceinline__ float tanhf_(float x) {
-  // accurate enough for bf16 activations, exact limits for |x| large
-  const float e = __expf(-2.f * fabsf(x));
-  const float t = (1.f - e) / (1.f + e);
-  return copysignf(t, x);
-}
 
 // gates: [B, 4S] pre-activation (i | j | f | o);  c_prev/c_new: [B, S] fp32
 // act:   [B, 4S] activated gates (σ(i) | tanh(j) | σ(f+1) | σ(o)) for backward
@@ -40,17 +33,12 @@ px_lstm_cell_fwd_kernel(const T* __restrict__ gates, const float* __restrict__ c
        idx += gridDim.x * blockDim.x) {
     const int b = idx / S, s = idx - b * S;
     const size_t g0 = (size_t)b * 4 * S + s;
-    const float si = sigmoidf_(to_f(gates[g0]));
-    const float tj = tanhf_(to_f(gates[g0 + S]));
-    const float sf = sigmoidf_(to_f(gates[g0 + 2 * S]) + forget_bias);
-    const float so = sigmoidf_(to_f(gates[g0 + 3 * S]));
-    const float c = sf * c_prev[idx] + si * tj;
-    c_new[idx] = c;
-    m[idx] = from_f<T>(so * tanhf_(c));
-    act[g0] = from_f<T>(si);
-    act[g0 + S] = from_f<T>(tj);
-    act[g0 + 2 * S] = from_f<T>(sf);
-    act[g0 + 3 * S] = from_f<T>(so);
+    float a[4], mv;
+    c_new[idx] = lstm_cell_fwd_elem(to_f(gates[g0]), to_f(gates[g0 + S]), to_f(gates[g0 + 2 * S]),
+                                    to_f(gates[g0 + 3 * S]), c_prev[idx], forget_bias, a, &mv);
+    m[idx] = from_f<T>(mv);
+#pragma unroll
+    for (int g = 0; g < 4; ++g) act[g0 + g * S] = from_f<T>(a[g]);
   }
 }
 
@@ -67,16 +55,12 @@ px_lstm_cell_bwd_kernel(const T* __restrict__ dm, float* __restrict__ dc,
        idx += gridDim.x * blockDim.x) {
     const int b = idx / S, s = idx - b * S;
     const size_t g0 = (size_t)b * 4 * S + s;
-    const float si = to_f(act[g0]), tj = to_f(act[g0 + S]), sf = to_f(act[g0 + 2 * S]),
-                so = to_f(act[g0 + 3 * S]);
-    const float tc = tanhf_(c_new[idx]);
-    const float dmv = to_f(dm[idx]);
-    const float dcv = dc[idx] + dmv * so * (1.f - tc * tc);
-    dgates[g0] = from_f<T>(dcv * tj * si * (1.f - si));
-    dgates[g0 + S] = from_f<T>(dcv * si * (1.f - tj * tj));
-    dgates[g0 + 2 * S] = from_f<T>(dcv * c_prev[idx] * sf * (1.f - sf));
-    dgates[g0 + 3 * S] = from_f<T>(dmv * tc * so * (1.f - so));
-    dc[idx] = dcv * sf;
+    float a[4], dg[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) a[g] = to_f(act[g0 + g * S]);
+    dc[idx] = lstm_cell_bwd_elem(a, c_prev[idx], c_new[idx], to_f(dm[idx]), dc[idx], dg);
+#pragma unroll
+    for (int g = 0; g < 4; ++g) dgates[g0 + g * S] = from_f<T>(dg[g]);
   }
 }
 

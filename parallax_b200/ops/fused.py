@@ -2,7 +2,8 @@
 
 `lstm_layer`  — a whole unrolled LSTMP layer as ONE autograd node: the
   sequential part per time step is 2 small GEMMs + 1 fused cell kernel
-  (forward) and 2 GEMMs + 1 fused kernel (backward); every weight gradient is
+  (forward) and 2 GEMMs, the first with the cell backward in its epilogue
+  (backward, bf16; elsewhere 2 GEMMs + 1 fused kernel); every weight gradient is
   a single GEMM batched over all time steps (the reference's TF graph issues
   one small GEMM + ~25 elementwise kernels per step and direction:
   `examples/lm1b/language_model.py:76-87`).
@@ -23,6 +24,7 @@ _vp, _i, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
 register_signatures({
     "px_lstm_cell_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
     "px_lstm_cell_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "px_lstm_dm_cell_bwd": (_i, [_vp] * 7 + [_i, _i, _i, _i, _vp]),
     "px_sampled_softmax": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_sampled_softmax_dot": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
                                     _vp]),
@@ -52,6 +54,19 @@ def _acc(t):
     """The references' accumulation type: fp32 for bf16/fp32 inputs, fp64 kept as fp64 (the
     tests' oracle)."""
     return t if t.dtype == torch.float64 else t.float()
+
+
+# Columns of dm per CTA of `px_lstm_dm_cell_bwd` (dm_t = dh_t·W_P^T with the cell backward in
+# its epilogue), measured with tools/bench_lstm_step.py at B 128, S 2048, P 512.
+BWD_BN = 16
+
+
+def _fused_bwd_ok(dt, Bsz, S, P, W_P):
+    """dm_t = dh_t·W_P^T with the cell backward fits one `px_lstm_dm_cell_bwd` launch: bf16,
+    whole 128-row tiles, S in BN-column tiles, P in 64-deep K-blocks, W_P as the K-contiguous
+    operand (the other operands are the layer's own 16-byte-aligned buffers)."""
+    return (dt == torch.bfloat16 and Bsz % 128 == 0 and S % BWD_BN == 0 and P % 64 == 0 and
+            W_P.is_contiguous() and W_P.data_ptr() % 16 == 0)
 
 
 def lstm_layer_reference(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
@@ -90,10 +105,10 @@ class _LSTMLayerFn(torch.autograd.Function):
             Wx, Wh = W.detach()[:E], W.detach()[E:]
         else:
             Wx = W
-        # W_P^T for the backward chain (dm_t = dh_t W_P^T as a plain NN GEMM): a 2 MB true
-        # transpose, 17 us of uncoalesced copy — done here on the side stream, underneath
+        # W_P^T for the unfused backward chain (dm_t = dh_t W_P^T as a plain NN GEMM): a 2 MB
+        # true transpose, 17 us of uncoalesced copy — done here on the side stream, underneath
         # the forward chain, instead of at the head of the backward pass
-        if any(ctx.needs_input_grad):
+        if any(ctx.needs_input_grad) and not _fused_bwd_ok(dt, Bsz, S, P, W_P):
             from . import sinks
             cur = torch.cuda.current_stream(dev)
             ws = sinks.side_stream(dev)
@@ -140,11 +155,15 @@ class _LSTMLayerFn(torch.autograd.Function):
         dc = torch.zeros(Bsz, S, dtype=torch.float32, device=dev) if dcT is None \
             else dcT.float().clone()
         dh_rec = None if dhT is None else dhT.to(dt)
-        dm = torch.empty(Bsz, S, dtype=dt, device=dev)
-        # dm_t = dh_t @ W_P^T runs as a plain NN GEMM on the W_P^T made in forward.
+        # dm_t = dh_t @ W_P^T: on the fused path one kernel with the cell backward in its
+        # epilogue (W_P [S, P] is already the K-contiguous operand), else a plain NN GEMM on the
+        # W_P^T made in forward followed by the cell kernel
+        fused = _fused_bwd_ok(dt, Bsz, S, P, W_P)
+        dm = None if fused else torch.empty(Bsz, S, dtype=dt, device=dev)
         cur = torch.cuda.current_stream(dev)
-        cur.wait_event(ctx.WPT_ev)
-        WPT = ctx.WPT
+        if not fused:
+            cur.wait_event(ctx.WPT_ev)
+            WPT = ctx.WPT
         # dh_{t-1} = dH_{t-1} + dgates_t @ Wh^T : Wh [P, 4S] is already the
         # K-contiguous "B^T" operand, so this skinny product (M=B, N=P, K=4S)
         # goes to our wgmma split-K kernel with the +dH addend fused in, its 8 K-splits
@@ -177,10 +196,15 @@ class _LSTMLayerFn(torch.autograd.Function):
         else:
             torch.add(dH[T - 1], dh_rec, out=dh_tot[T - 1])
         for t in range(T - 1, -1, -1):
-            torch.mm(dh_tot[t], WPT, out=dm)
-            _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
-                                      _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt], st),
-                   "lstm_cell_bwd")
+            if fused:
+                _check(L.px_lstm_dm_cell_bwd(_p(dh_tot[t]), _p(W_P), _p(dc), _p(act[t]),
+                                             _p(c_all[t]), _p(c_all[t + 1]), _p(dgates[t]), Bsz,
+                                             S, P, BWD_BN, st), "lstm_dm_cell_bwd")
+            else:
+                torch.mm(dh_tot[t], WPT, out=dm)
+                _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
+                                          _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt], st),
+                       "lstm_cell_bwd")
             if t > 0:
                 if use_tc:
                     _gemm.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=8, bn=64,
