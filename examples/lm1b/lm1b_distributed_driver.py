@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 import parallax_b200 as parallax
-from parallax_b200.models.lm1b import LM1B, lm1b_graph
+from parallax_b200.models.lm1b import LM1B, lm1b_graph, parse_hpconfig
 import parallax_config
 from parallax_b200.models.lm1b_data import Vocabulary, Dataset
 
@@ -43,33 +43,15 @@ FLAGS = ap.parse_args()
 
 NUM_TRAIN_WORDS = 798945280          # words in the 1B-word training shards
 
-MODEL_HP = {"keep_prob": float, "num_sampled": int, "emb_size": int, "state_size": int,
-            "projected_size": int}
-
-
-def apply_hpconfig():
-    """`--hpconfig a=1,b=2` (reference `language_model_graph.py` hps.parse)"""
-    model_kw = {}
-    for item in filter(None, (x.strip() for x in FLAGS.hpconfig.split(","))):
-        k, _, v = item.partition("=")
-        if k in MODEL_HP:
-            model_kw[k] = MODEL_HP[k](v)
-        elif hasattr(FLAGS, k):
-            cur = getattr(FLAGS, k)
-            setattr(FLAGS, k, type(cur)(v) if cur is not None else v)
-        else:
-            raise ValueError("unknown hyper-parameter %r in --hpconfig" % k)
-    return model_kw
-
 
 def main():
-    model_kw = apply_hpconfig()
+    model_kw = parse_hpconfig(FLAGS.hpconfig, FLAGS)
     kw = dict(vocab_size=FLAGS.vocab_size, num_steps=FLAGS.num_steps,
               num_shards=FLAGS.num_variable_shards, lazy=True)
-    kw.update(model_kw)
     if FLAGS.tiny:
         kw.update(vocab_size=min(FLAGS.vocab_size, 10000), emb_size=32, state_size=64,
                   projected_size=32, num_sampled=64, lazy=False)
+    kw.update(model_kw)
     model = LM1B(**kw)
     single_gpu_graph = lm1b_graph(model, FLAGS.batch_size, FLAGS.learning_rate,
                                   FLAGS.max_grad_norm)

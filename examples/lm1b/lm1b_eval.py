@@ -20,7 +20,7 @@ import torch
 
 import parallax_b200 as parallax
 from parallax_b200.checkpoint import latest_checkpoint
-from parallax_b200.models.lm1b import LM1B, lm1b_graph
+from parallax_b200.models.lm1b import LM1B, lm1b_graph, parse_hpconfig
 from parallax_b200.models.lm1b_data import Vocabulary, Dataset
 
 ap = argparse.ArgumentParser()
@@ -33,6 +33,13 @@ ap.add_argument("--num_steps", type=int, default=20)
 ap.add_argument("--vocab_size", type=int, default=793470)
 ap.add_argument("--max_batches", type=int, default=100)
 ap.add_argument("--tiny", action="store_true")
+ap.add_argument("--hpconfig", default="",
+                help="model hyper-parameters as lm1b_distributed_driver.py takes them: "
+                     "name=value,... (emb_size, state_size, projected_size, num_sampled, "
+                     "keep_prob); give the values the checkpoint was trained with")
+ap.add_argument("--compute_dtype", default=None,
+                help="bf16: bf16 LSTM outputs, which the fused full-softmax kernels take on the "
+                     "NVLink fabric")
 ap.add_argument("--top_k", type=int, default=0,
                 help="also report accuracy@1 and accuracy@K of the K most likely next words "
                      "(parallax.nn.full_softmax_topk); this reads the softmax table a second "
@@ -51,14 +58,18 @@ def topk_hits(top, y, w):
 
 
 def main():
+    model_kw = parse_hpconfig(FLAGS.hpconfig, FLAGS)
     kw = dict(vocab_size=FLAGS.vocab_size, num_steps=FLAGS.num_steps, lazy=True,
               eval_top_k=FLAGS.top_k)
     if FLAGS.tiny:
         kw.update(vocab_size=min(FLAGS.vocab_size, 10000), emb_size=32, state_size=64,
                   projected_size=32, num_sampled=64, lazy=False)
+    kw.update(model_kw)
     model = LM1B(**kw)
     graph = lm1b_graph(model, FLAGS.batch_size)
-    cfg = parallax.Config(ckpt_config=parallax.CheckPointConfig(ckpt_dir=FLAGS.ckpt_dir))
+    cfg = parallax.Config(ckpt_config=parallax.CheckPointConfig(ckpt_dir=FLAGS.ckpt_dir),
+                          sess_config={"compute_dtype": FLAGS.compute_dtype}
+                          if FLAGS.compute_dtype else None)
     path = latest_checkpoint(FLAGS.ckpt_dir)
     assert path is not None, "no checkpoint under %s" % FLAGS.ckpt_dir
     sess, *_ = parallax.parallel_run(graph, "localhost", parallax_config=cfg)   # restores on start

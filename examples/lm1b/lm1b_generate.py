@@ -22,7 +22,7 @@ import numpy as np
 import parallax_b200 as parallax
 from parallax_b200 import optim
 from parallax_b200.checkpoint import latest_checkpoint
-from parallax_b200.models.lm1b import LM1B, lm1b_graph
+from parallax_b200.models.lm1b import LM1B, lm1b_graph, parse_hpconfig
 from parallax_b200.models.lm1b_data import Vocabulary
 
 ap = argparse.ArgumentParser()
@@ -33,6 +33,10 @@ ap.add_argument("--use_synthetic", action="store_true",
 ap.add_argument("--use_ema", action="store_true")
 ap.add_argument("--vocab_size", type=int, default=793470)
 ap.add_argument("--tiny", action="store_true")
+ap.add_argument("--hpconfig", default="",
+                help="model hyper-parameters as lm1b_distributed_driver.py takes them: "
+                     "name=value,... (emb_size, state_size, projected_size, num_sampled, "
+                     "keep_prob); give the values the checkpoint was trained with")
 ap.add_argument("--prefix", default="",
                 help="words the sequences start with (ids with --use_synthetic or --tiny); "
                      "the sentence start <S> (id 0 without a vocabulary) is put in front")
@@ -55,12 +59,14 @@ def step_seed(seed, step):
 
 
 def main():
+    model_kw = parse_hpconfig(FLAGS.hpconfig, FLAGS)
     kw = dict(vocab_size=FLAGS.vocab_size, lazy=True, eval_sample=1,
               sample_temperature=FLAGS.temperature, sample_top_k=FLAGS.top_k,
               sample_top_p=FLAGS.top_p)
     if FLAGS.tiny:
         kw.update(vocab_size=min(FLAGS.vocab_size, 10000), emb_size=32, state_size=64,
                   projected_size=32, num_sampled=64, lazy=False)
+    kw.update(model_kw)
     model = LM1B(**kw)
     B = FLAGS.num_sequences
     cfg = parallax.Config(ckpt_config=parallax.CheckPointConfig(ckpt_dir=FLAGS.ckpt_dir),

@@ -241,3 +241,28 @@ def lm1b_graph(model, batch_size=128, learning_rate=0.2, max_grad_norm=10.0):
                     ClipByGlobalNorm(max_grad_norm, params=lstm_vars)],
         ema=ExponentialMovingAverage(0.999, params=lstm_vars),
         name="lm1b")
+
+
+# the LM1B keyword arguments `--hpconfig` sets in the example scripts, and their types
+HPCONFIG_MODEL_KEYS = {"keep_prob": float, "num_sampled": int, "emb_size": int,
+                       "state_size": int, "projected_size": int}
+
+
+def parse_hpconfig(spec, flags):
+    """`--hpconfig name=value,...` of the LM1B example scripts (the reference's `hps.parse`):
+    returns the model's keys (`HPCONFIG_MODEL_KEYS`) as `LM1B` keyword arguments, and sets any
+    other name that is an attribute of `flags` (an argparse namespace) to the value, converted
+    to the attribute's current type.  The training, evaluation and generation scripts share it,
+    so the same flags build the same model and a checkpoint restores into it.  `ValueError` for
+    any other name."""
+    model_kw = {}
+    for item in filter(None, (x.strip() for x in spec.split(","))):
+        k, _, v = item.partition("=")
+        if k in HPCONFIG_MODEL_KEYS:
+            model_kw[k] = HPCONFIG_MODEL_KEYS[k](v)
+        elif hasattr(flags, k):
+            cur = getattr(flags, k)
+            setattr(flags, k, type(cur)(v) if cur is not None else v)
+        else:
+            raise ValueError("unknown hyper-parameter %r in --hpconfig" % k)
+    return model_kw

@@ -135,7 +135,7 @@ def full_softmax_nll(inputs, targets, weight, bias):
     `inputs` is ``[N, K]``, `targets` ``[N]`` integer ids, `weight` / `bias` are the two
     embedding modules (``[V, K]`` and ``[V, 1]``) — the arguments `lookup_many` takes.  When
     they form a co-lookup group on the NVLink fabric with a bf16 weight shadow, inputs are bf16
-    with K % 8 == 0 and K <= 512, and no gradient is wanted, one fused kernel evaluates the
+    with K % 8 == 0 and K <= 1024, and no gradient is wanted, one fused kernel evaluates the
     softmax where the rows live (no gathered table, no [N, V] logits, fp32 logits; a target
     outside [0, V) gives NaN in its row).  Under the same conditions in training, a session
     with ``sess_config["full_softmax_train"] = "fused"`` also runs the forward fused and a

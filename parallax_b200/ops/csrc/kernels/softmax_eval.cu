@@ -11,7 +11,8 @@
 //                                   table byte is read once per call.  The epilogue adds the fp32
 //                                   bias, masks padding rows with −inf and merges the block's
 //                                   per-row (max, Σexp) into the CTA's slice of a [grid, N]
-//                                   workspace (only that CTA touches it: no atomics).
+//                                   workspace (only that CTA touches it: no atomics).  BV is
+//                                   128 for K <= 512 and 64 for 512 < K <= 1024 (ev_bv).
 //   px_full_softmax_combine_kernel  one row per warp: merge the grid's (max, Σexp) pairs and
 //                                   subtract the target logit, whose rows come from the group's
 //                                   lookup kernel.
@@ -63,9 +64,13 @@
 
 namespace tc {
 
-constexpr int EV_BV = 128;          // table rows per work item = wgmma N
 constexpr int EV_STAGES = 4;        // X ring depth (16 KB per stage)
-constexpr int EV_KMAX = 512;
+constexpr int EV_KMAX = 1024;
+// table rows per work item (= wgmma N) at width K: the resident block of BV rows × K bf16 is at
+// most 128 KB, so 128 rows up to K = 512 and 64 rows up to K = 1024.  Fewer rows per block
+// halve the FLOP per byte of X each CTA streams, so the wide height is only taken where needed.
+constexpr int ev_bv(int K) { return K <= 512 ? 128 : 64; }
+constexpr int ev_kmax(int bv) { return 128 * 512 / bv; }   // the widest K a block height takes
 constexpr float EV_LOG2E = 1.4426950408889634f;
 
 // one top-k list entry; the order key is (v descending, id ascending).  An empty entry is
@@ -199,13 +204,13 @@ __device__ __forceinline__ float ev_bias(const __nv_bfloat16* row) {
 }
 
 // Top-k epilogue of one row h of the quad's two (all four lanes call it; the row is < N).  A lane
-// holds 32 of the block's BV logits at acc[j·4 + 2h + e], column j·8 + cq + e; s_gid has their
+// holds BV/4 of the block's BV logits at acc[j·4 + 2h + e], column j·8 + cq + e; s_gid has their
 // global ids.  The list of the CTA is skipped unless the block's row maximum mx can enter it.
 // Otherwise up to k rounds of quad-wide arg-max extract, best first, the block's entries that
 // beat the list's (k − r)-th entry in round r.  The list is copied to shared memory (lbuf) by the
 // four lanes at once, the candidates are staged in cand, and both are merged into the list from
 // its tail, so entries ahead of the first insertion are not rewritten.
-template <int KC>
+template <int BV, int KC>
 __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, int cq, float mx,
                                          const int* s_gid, TopkEntry* cand, TopkEntry* lbuf,
                                          TopkEntry* list, bool first) {
@@ -221,7 +226,7 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
     float bv = -INFINITY;
     int bc = 0, bid = INT_MAX;
 #pragma unroll
-    for (int j = 0; j < EV_BV / 8; ++j)
+    for (int j = 0; j < BV / 8; ++j)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const float v = acc[j * 4 + 2 * h + e];
@@ -241,7 +246,7 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
     if (q0) cand[m] = TopkEntry{wv, wid};
     if (bid == wid && bv == wv) {            // the lane that holds the winner takes it out
 #pragma unroll
-      for (int j = 0; j < EV_BV / 8; ++j)
+      for (int j = 0; j < BV / 8; ++j)
 #pragma unroll
         for (int e = 0; e < 2; ++e)
           if (j * 8 + cq + e == bc) acc[j * 4 + 2 * h + e] = -INFINITY;
@@ -266,13 +271,14 @@ __device__ __forceinline__ void topk_row(const TopkArgs& a, float* acc, int h, i
 // the lists rank Gumbel keys of the tempered logits instead of the logits.  GRAD (KC == 0): the
 // gradient epilogue over one gathered chunk instead of the (max, Σexp) pairs.  SAMPLE with KC == 0:
 // the pairs are of s = l/τ.  HIST = d (KC == 0, SAMPLE): the digit histogram of truncated sampling
-// instead of the pairs.  MASK (KC > 0, SAMPLE): keys below the row's threshold drop out
-template <typename BiasT, int KC, bool SAMPLE = false, bool GRAD = false, int HIST = 0,
+// instead of the pairs.  MASK (KC > 0, SAMPLE): keys below the row's threshold drop out.  BV:
+// the block height, ev_bv(K)
+template <typename BiasT, int BV, int KC, bool SAMPLE = false, bool GRAD = false, int HIST = 0,
           bool MASK = false>
 __global__ void __launch_bounds__(THREADS, 1)
 px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
                            EvalParams<KC, SAMPLE, GRAD, HIST, MASK> a) {
-  constexpr int BV = EV_BV, X_BYTES = BM * BK * 2;
+  constexpr int X_BYTES = BM * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sB = smem;                                        // [kb][BV rows][128 B]
@@ -532,7 +538,7 @@ px_full_softmax_lse_kernel(const __grid_constant__ CUtensorMap tmap_x,
             }
             if constexpr (KC > 0) {
               if (row < a.N)
-                topk_row<KC>(a, acc, h, cq, mx, s_gid, s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC,
+                topk_row<BV, KC>(a, acc, h, cq, mx, s_gid, s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC,
                              s_cand + ((threadIdx.x - 128) >> 2) * 2 * KC + KC,
                              a.tk + ((size_t)blockIdx.x * a.N + row) * a.k, first);
             }
@@ -729,20 +735,30 @@ px_full_softmax_select_kernel(const HistBin* __restrict__ hist, int grid, int N,
   }
 }
 
-// dynamic shared memory of px_full_softmax_lse_kernel<·, kc> at kb K-blocks: alignment slack,
-// table block, X ring, bias and barriers; the top-k kernels (kc > 0) add the block's global ids,
-// and a candidate list and a copy of the row's list per consumer quad; the gradient kernels
-// (grad) the block's column sums; the histogram kernels (bins = 2^d) the bins of one row per
-// consumer lane
-constexpr int ev_smem_bytes(int kb, int kc, bool grad = false, int bins = 0) {
-  return 1024 + kb * EV_BV * 128 + EV_STAGES * BM * BK * 2 + EV_BV * 4 + 2 * EV_STAGES * 8 +
-         (kc > 0 ? EV_BV * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0) +
-         (grad ? EV_BV * 4 : 0) + 2 * 128 * bins * (int)sizeof(HistBin);
+// dynamic shared memory of px_full_softmax_lse_kernel<·, bv, kc> at kb K-blocks: alignment
+// slack, table block, X ring, bias and barriers; the top-k kernels (kc > 0) add the block's
+// global ids, and a candidate list and a copy of the row's list per consumer quad; the gradient
+// kernels (grad) the block's column sums; the histogram kernels (bins = 2^d) the bins of one row
+// per consumer lane
+constexpr int ev_smem_bytes(int bv, int kb, int kc, bool grad = false, int bins = 0) {
+  return 1024 + kb * bv * 128 + EV_STAGES * BM * BK * 2 + bv * 4 + 2 * EV_STAGES * 8 +
+         (kc > 0 ? bv * 4 + (2 * 128 / 4) * 2 * kc * (int)sizeof(TopkEntry) : 0) +
+         (grad ? bv * 4 : 0) + 2 * 128 * bins * (int)sizeof(HistBin);
 }
-static_assert(ev_smem_bytes(EV_KMAX / BK, 0) == 198208, "log-sum-exp shared memory at K = 512");
-static_assert(ev_smem_bytes(EV_KMAX / BK, 32) <= 227 * 1024, "top-k shared memory");
-static_assert(ev_smem_bytes(EV_KMAX / BK, 0, false, 1 << EV_RADIX_BITS) <= 227 * 1024,
+static_assert(ev_kmax(128) == 512 && ev_kmax(64) == EV_KMAX, "block heights");
+static_assert(ev_smem_bytes(128, ev_kmax(128) / BK, 0) == 198208,
+              "log-sum-exp shared memory at K = 512");
+static_assert(ev_smem_bytes(128, ev_kmax(128) / BK, 32) <= 227 * 1024, "top-k shared memory");
+static_assert(ev_smem_bytes(128, ev_kmax(128) / BK, 0, false, 1 << EV_RADIX_BITS) <= 227 * 1024,
               "histogram shared memory");
+static_assert(ev_smem_bytes(64, ev_kmax(64) / BK, 0) == 197952,
+              "log-sum-exp shared memory at K = 1024");
+static_assert(ev_smem_bytes(64, ev_kmax(64) / BK, 32) <= 227 * 1024,
+              "top-k and masked sampling shared memory at K = 1024");
+static_assert(ev_smem_bytes(64, ev_kmax(64) / BK, 0, false, 1 << EV_RADIX_BITS) <= 227 * 1024,
+              "histogram shared memory at K = 1024");
+static_assert(ev_smem_bytes(64, ev_kmax(64) / BK, 0, true) == 198208,
+              "gradient shared memory at K = 1024");
 
 }  // namespace tc
 
@@ -767,7 +783,8 @@ int ev_setup(tc::EvalArgs& a, CUtensorMap& tx, int& grid, const void* X, int N, 
   a.w_pitch = w_pitch; a.b_pitch = b_pitch;
   a.W = G.W; a.rank = rank; a.replicated = G.replicated; a.owners = G.replicated ? 1 : G.W;
   a.slots = slots; a.rows_per_part = G.rows_per_part;
-  a.nblk = (slots * G.rows_per_part + EV_BV - 1) / EV_BV;
+  const int bv = ev_bv(K);
+  a.nblk = (slots * G.rows_per_part + bv - 1) / bv;
   a.wait = wait;
   const int items = a.owners * a.nblk;
   grid = items < ws_ctas ? items : ws_ctas;
@@ -785,15 +802,17 @@ void ev_launch(int grid, const CUtensorMap& tx,
                const tc::EvalParams<KC, SAMPLE, GRAD, HIST, MASK>& a, cudaStream_t stream) {
   using namespace tc;
   constexpr int bins = HIST ? 1 << HIST : 0;
-  static bool set = false;
-  if (!set) {
-    cudaFuncSetAttribute(px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD, HIST, MASK>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         ev_smem_bytes(EV_KMAX / BK, KC, GRAD, bins));
-    set = true;
+  // the block height of a.K; each height's shared memory limit is set at its own widest K
+  const int bv = ev_bv(a.K);
+  const auto kernel = bv == 128 ? px_full_softmax_lse_kernel<BiasT, 128, KC, SAMPLE, GRAD, HIST, MASK>
+                                : px_full_softmax_lse_kernel<BiasT, 64, KC, SAMPLE, GRAD, HIST, MASK>;
+  static bool set[2] = {false, false};
+  if (!set[bv == 64]) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         ev_smem_bytes(bv, ev_kmax(bv) / BK, KC, GRAD, bins));
+    set[bv == 64] = true;
   }
-  px_full_softmax_lse_kernel<BiasT, KC, SAMPLE, GRAD, HIST, MASK>
-      <<<grid, THREADS, ev_smem_bytes(a.kb, KC, GRAD, bins), stream>>>(tx, a);
+  kernel<<<grid, THREADS, ev_smem_bytes(bv, a.kb, KC, GRAD, bins), stream>>>(tx, a);
 }
 
 template <typename BiasT>
@@ -861,7 +880,8 @@ int ev_temp_setup(tc::TempArgs& a, CUtensorMap& tx, int& grid, const void* X, in
 
 extern "C" {
 
-// nll[N] (fp32) of X [N, K] (bf16, K-contiguous) against a (weight, bias) co-lookup group.
+// nll[N] (fp32) of X [N, K] (bf16, K-contiguous, K % 8 == 0, 8 <= K <= 1024) against a
+// (weight, bias) co-lookup group.
 //   w_ptrs / b_ptrs: device arrays of every rank's weight shadow (bf16, row pitch w_pitch) and
 //                    bias master rows (fp32, or bf16 when b_bf16; row pitch b_pitch elements,
 //                    16 bytes apart or a multiple of them);
@@ -1012,8 +1032,9 @@ int px_full_softmax_sample_masked(const void* X, int N, int K, const void* w_ptr
 //   db [rows] fp32       = Σ_i G[i][v]
 // X [N, K] bf16 as px_full_softmax_nll; wc / bc: the chunk's bf16 weight rows and bias rows (fp32,
 // or bf16 when b_bf16), row pitches w_pitch / b_pitch elements as px_full_softmax_nll; lse, g fp32
-// [N] and targets int64 [N].  Columns of G from rows to rows rounded up to 128 are written as zero,
-// later ones are not written; g_pitch >= rows rounded up to 128, even.  Grid <= ctas CTAs.
+// [N] and targets int64 [N].  Columns of G from rows to rows rounded up to the block height (128
+// rows for K <= 512, 64 for 512 < K <= 1024) are written as zero, later ones are not written;
+// g_pitch >= rows rounded up to the block height, even.  Grid <= ctas CTAs.
 // Returns 0, a negative argument error, or a CUDA error code.
 int px_full_softmax_grad(const void* X, int N, int K, const void* wc, int w_pitch, const void* bc,
                          int b_pitch, int b_bf16, int rows, long long v0, const float* lse,
@@ -1023,8 +1044,9 @@ int px_full_softmax_grad(const void* X, int N, int K, const void* wc, int w_pitc
   if (N <= 0 || rows <= 0) return 0;
   if (K < 8 || K % 8 || K > EV_KMAX || w_pitch < K || w_pitch % 8 || b_pitch % (b_bf16 ? 8 : 4))
     return -1;
-  const int nblk = (rows + EV_BV - 1) / EV_BV;
-  if (ctas < 1 || g_pitch % 2 || g_pitch < nblk * EV_BV) return -2;
+  const int bv = ev_bv(K);
+  const int nblk = (rows + bv - 1) / bv;
+  if (ctas < 1 || g_pitch % 2 || g_pitch < nblk * bv) return -2;
   GradArgs a{};
   a.N = N; a.K = K; a.kb = (K + BK - 1) / BK;
   a.w_pitch = w_pitch; a.b_pitch = b_pitch;

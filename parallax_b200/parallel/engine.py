@@ -127,13 +127,14 @@ def _fused_group(inputs, weight, bias):
     """The co-lookup group whose fused full-softmax kernels can take `inputs` against the
     (weight, bias) embedding modules, else None: the modules form a group on the NVLink fabric
     (protocol nvlink) whose weight table keeps a bf16 shadow, and `inputs` is bf16 on the group's
-    device with K % 8 == 0 and K <= 512."""
+    device with K % 8 == 0 and K <= 1024 (the kernels hold 128 table rows per block up to K = 512
+    and 64 rows beyond)."""
     tabs = [getattr(m, "table", None) for m in (weight, bias)]
     grp = getattr(tabs[0], "group", None) if tabs[0] is not None else None
     K = int(inputs.shape[-1])
     if grp is not None and list(grp.tables) == tabs and grp.protocol == "nvlink" and \
             tabs[0].use_shadow and inputs.dtype == torch.bfloat16 and \
-            inputs.device == grp.device and K % 8 == 0 and K <= 512:
+            inputs.device == grp.device and K % 8 == 0 and K <= 1024:
         return grp
     return None
 

@@ -55,6 +55,12 @@ def _sp(stream):
     return _vp(stream.cuda_stream)
 
 
+def full_softmax_block_rows(K):
+    """Table rows per work item of the fused full-softmax kernels at input width K (`ev_bv` in
+    `ops/csrc/kernels/softmax_eval.cu`): 128 up to K = 512, 64 up to K = 1024."""
+    return 128 if K <= 512 else 64
+
+
 class HPStage(object):
     """Device copy of an optimizer's hyper-parameter vector, refreshed once per step
     through a ring of pinned buffers (the host may run several CUDA-graph replays ahead
@@ -662,14 +668,16 @@ class NVSparseGroup(object):
     def full_softmax_train_chunk(self, n):
         """Rows of one vocabulary chunk of `full_softmax_nll_grad` for n input rows: the
         chunk's gathered rows and its bf16 [n, Vc] softmax gradient fit in
-        `consts.FULL_SOFTMAX_TRAIN_WS_BYTES`; a multiple of 128 · NUM_SMS where that fits
-        (whole waves of the gradient kernel's 128-row blocks), else of 128."""
+        `consts.FULL_SOFTMAX_TRAIN_WS_BYTES`; a multiple of BV · NUM_SMS where that fits
+        (whole waves of the gradient kernel's blocks of BV = `full_softmax_block_rows(K)`
+        rows), else of BV."""
         tw, tb = self.tables
         b_bytes = tb.Dps * 2 if tb.weight_dtype == torch.bfloat16 else tb.Dp * 4
         rows = consts.FULL_SOFTMAX_TRAIN_WS_BYTES // (2 * n + 2 * tw.Dps + b_bytes)
-        wave = 128 * consts.NUM_SMS
-        vc = rows // wave * wave if rows >= wave else max(128, rows // 128 * 128)
-        return min(vc, (tw.V + 127) // 128 * 128)
+        bv = full_softmax_block_rows(tw.D)
+        wave = bv * consts.NUM_SMS
+        vc = rows // wave * wave if rows >= wave else max(bv, rows // bv * bv)
+        return min(vc, (tw.V + bv - 1) // bv * bv)
 
     def full_softmax_nll_grad(self, x, targets, lse, g, want_x=True, want_tables=True,
                               chunk=None):
@@ -693,7 +701,8 @@ class NVSparseGroup(object):
             lse = lse.to(dev, torch.float32).contiguous()
             g = g.reshape(-1).to(dev, torch.float32).contiguous()
             vc = int(chunk) if chunk else self.full_softmax_train_chunk(n)
-            gp = (vc + 127) // 128 * 128
+            bv = full_softmax_block_rows(K)
+            gp = (vc + bv - 1) // bv * bv                  # >= the chunk's blocks · BV, even
             wc = torch.empty((vc, tw.Dps), dtype=torch.bfloat16, device=dev)
             bc = torch.empty((vc, b_pitch), dtype=tb.weight_dtype, device=dev)
             G = torch.empty((n, gp), dtype=torch.bfloat16, device=dev)

@@ -7,13 +7,15 @@ gather + matmul + log_softmax + noise + top-n composition against the fused samp
 
     python tools/bench_full_softmax.py [--n 640 2560] [--k 1 10 32] [--sample 1 10 32]
                                        [--trunc 1 10] [--top_k 40] [--top_p 0.9 0.95]
-                                       [--temperature 1.0] [--out result.json]
+                                       [--temperature 1.0] [--K 512] [--out result.json]
 
 Builds LM1B's (softmax_w, softmax_b) co-lookup group through the engine on the NVLink fabric,
-one GPU: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N:
+one GPU: V = 793 470, K = --K (LM1B's projected_size, default 512), bf16 shadow rows, 32
+partitions.  For each N:
 - NLL: the composition and the fused kernel alternate over --rounds rounds of --iters calls
   (median).  The records carry the largest |Δ| between the arms' NLL (the composition rounds
-  logits to bf16).
+  logits to bf16).  At K != 512 a second group 512 wide is built and its fused NLL
+  (`fused_nll_k512`) is timed in the same rounds.
 - top-k, for each k of --k (an empty list times the NLL only): the fused top-k and the fused NLL
   alternate over the rounds, and the composition is timed after them in each round over
   --comp_iters calls.  The fused ids are compared with the composition's where its consecutive
@@ -86,6 +88,39 @@ def alternate(arms, rounds):
     return {name: (ms[name], mem[name]) for name in ms}
 
 
+def output_layer(K, sess_config, **model_kw):
+    """(session, softmax_w, softmax_b) of an LM1B whose output layer is LM1B's with K columns,
+    built through the engine on the NVLink fabric, one GPU"""
+    model = LM1B(lazy=True, state_size=512, projected_size=K, **model_kw)
+    sess, *_ = parallax.parallel_run(
+        lm1b_graph(model, batch_size=128), "localhost:0",
+        parallax_config=parallax.Config(sess_config=dict({"fabric": "nvlink",
+                                                          "compute_dtype": "bf16"},
+                                                         **sess_config)))
+    m = sess.engine.model
+    w, b = m.softmax_w, m.softmax_b
+    assert w.table.group is b.table.group and w.table.use_shadow and w.embedding_dim == K
+    return sess, w, b
+
+
+def k512_nll(sess_config, n_list, **model_kw):
+    """{N: a call of the fused NLL on a second output layer 512 wide}, timed next to a wider
+    layer's arms, and its session"""
+    sess, w, b = output_layer(512, sess_config, **model_kw)
+    calls = {}
+    for n in n_list:
+        g = torch.Generator(device="cuda").manual_seed(n)
+        x = (torch.randn(n, 512, device="cuda", generator=g) * 0.5).bfloat16()
+        t = torch.randint(0, w.num_embeddings, (n,), device="cuda", generator=g)
+
+        def call(x=x, t=t):
+            with torch.no_grad():
+                return parallax.nn.full_softmax_nll(x, t, w, b)
+        call()
+        calls[n] = call
+    return sess, calls
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, nargs="+", default=[640, 2560])
@@ -98,6 +133,8 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--comp_iters", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--K", type=int, default=512,
+                    help="columns of the output layer (LM1B's projected_size)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -105,25 +142,21 @@ def main():
     info = card()
     print("card: %s" % info, flush=True)
     torch.manual_seed(0)
-    model = LM1B(lazy=True, state_size=512)          # the output layer is LM1B's exactly
-    sess, *_ = parallax.parallel_run(
-        lm1b_graph(model, batch_size=128), "localhost:0",
-        parallax_config=parallax.Config(sess_config={"fabric": "nvlink",
-                                                     "compute_dtype": "bf16"}))
-    m = sess.engine.model
-    w, b = m.softmax_w, m.softmax_b
-    assert w.table.group is b.table.group and w.table.use_shadow
+    # the output layer is LM1B's exactly, --K wide
+    sess, w, b = output_layer(a.K, {})
     V, K = w.num_embeddings, w.embedding_dim
+    sess512, nll512 = k512_nll({}, a.n) if K != 512 else (None, {})
     results = []
 
-    def report(arm, n, timing, k=None, extra=None):
+    def report(arm, n, timing, k=None, extra=None, Kx=None):
         ms, grow = timing
         med = statistics.median(ms)
-        r = {"arm": arm, "N": n, **({} if k is None else {"k": k}), "V": V, "K": K,
+        Kx = Kx or K
+        r = {"arm": arm, "N": n, **({} if k is None else {"k": k}), "V": V, "K": Kx,
              **({} if k is None or "sample" not in arm else {"temperature": a.temperature}),
              "ms": round(med, 3), "ms_all": [round(v, 3) for v in ms],
              "mem_growth_MB": round(grow / 2 ** 20, 1),
-             "tflops": round(2.0 * n * V * K / (med * 1e-3) / 1e12, 1), **(extra or {}),
+             "tflops": round(2.0 * n * V * Kx / (med * 1e-3) / 1e12, 1), **(extra or {}),
              "card": info}
         results.append(r)
         print(json.dumps(r), flush=True)
@@ -140,9 +173,14 @@ def main():
             comp(), nll()
             diff = {"max_abs_diff_nll": float((fused - ref).abs().max())}
             del ref, fused
-            res = alternate([("composition", comp, a.iters), ("fused", nll, a.iters)], a.rounds)
+            arms = [("composition", comp, a.iters), ("fused", nll, a.iters)]
+            if nll512:
+                arms.append(("fused_nll_k512", nll512[n], a.iters))
+            res = alternate(arms, a.rounds)
             for arm in ("composition", "fused"):
                 report(arm, n, res[arm], extra=diff)
+            if nll512:
+                report("fused_nll_k512", n, res["fused_nll_k512"], Kx=512)
             for k in a.k:
                 topk = lambda: parallax.nn.full_softmax_topk(x, w, b, k)    # noqa: E731
                 tcomp = lambda: full_softmax_topk_composition(x, w, b, k)   # noqa: E731
@@ -213,6 +251,8 @@ def main():
                                       "trunc_over_nll": round(tt / nl, 3),
                                       "composition_over_trunc": round(cm / tt, 2)}), flush=True)
     sess.close()
+    if sess512 is not None:
+        sess512.close()
     if a.out:
         with open(a.out, "w") as f:
             json.dump({"card": info, "results": results}, f, indent=1)

@@ -2,18 +2,20 @@
 composition against the fused forward and backward (``sess_config["full_softmax_train"] =
 "fused"``), and an LM1B(num_sampled=0) training step under each setting.
 
-    python tools/bench_full_softmax_train.py [--n 640 2560] [--steps 10] [--out result.json]
+    python tools/bench_full_softmax_train.py [--n 640 2560] [--steps 10] [--K 512]
+                                             [--out result.json]
 
 Head: LM1B's (softmax_w, softmax_b) co-lookup group built through the engine on the NVLink
-fabric: V = 793 470, K = 512, bf16 shadow rows, 32 partitions.  For each N the composition's
-forward plus backward, the fused forward plus backward and the fused NLL (no gradient) alternate
-over --rounds rounds of --iters calls (median).  The backward's table gradient rows are dropped
-after each call (no step is run).  Per arm: ms per call (CUDA events, after warm-up), the growth
+fabric: V = 793 470, K = --K (LM1B's projected_size, default 512), bf16 shadow rows, 32
+partitions.  For each N the composition's forward plus backward, the fused forward plus backward
+and the fused NLL (no gradient) alternate over --rounds rounds of --iters calls (median); at
+K != 512 so does the fused NLL of a second group 512 wide (`fused_nll_k512`).  The backward's
+table gradient rows are dropped after each call (no step is run).  Per arm: ms per call (CUDA events, after warm-up), the growth
 of `torch.cuda.max_memory_allocated` during one call, and TFLOP/s counted as 8·N·V·K for forward
 plus backward (2·N·V·K for the NLL alone).  The records carry the relative Frobenius difference
 of the two arms' input gradients.
 
-Step: LM1B(num_sampled=0) at the benchmark's shapes (batch 128, 20 steps, LSTM 2048 -> 512,
+Step: LM1B(num_sampled=0) at the benchmark's shapes (batch 128, 20 steps, LSTM 2048 -> --K,
 bf16, CUDA graph), each setting in a process of its own: ms per step over --steps steps after
 --warmup, and the peak allocation from the first step on.  The card name, power limit and max SM clock are read in the
 same run.
@@ -31,21 +33,16 @@ import torch  # noqa: E402
 import parallax_b200 as parallax  # noqa: E402
 from parallax_b200.models.lm1b import LM1B, lm1b_graph  # noqa: E402
 from parallax_b200.parallel.engine import full_softmax_composition  # noqa: E402
-from tools.bench_full_softmax import alternate, card  # noqa: E402
+from tools.bench_full_softmax import alternate, card, k512_nll, output_layer  # noqa: E402
 
 
 def head(a, info):
     torch.manual_seed(0)
-    model = LM1B(lazy=True, state_size=512, num_sampled=0)
-    sess, *_ = parallax.parallel_run(
-        lm1b_graph(model, batch_size=128), "localhost:0",
-        parallax_config=parallax.Config(sess_config={"fabric": "nvlink", "compute_dtype": "bf16",
-                                                     "full_softmax_train": "fused"}))
-    m = sess.engine.model
-    w, b = m.softmax_w, m.softmax_b
+    sess, w, b = output_layer(a.K, {"full_softmax_train": "fused"}, num_sampled=0)
     grp = w.table.group
-    assert b.table.group is grp and w.table.use_shadow
     V, K = w.num_embeddings, w.embedding_dim
+    sess512, nll512 = k512_nll({"full_softmax_train": "fused"}, a.n, num_sampled=0) \
+        if K != 512 else (None, {})
     out = []
     for n in a.n:
         gen = torch.Generator(device="cuda").manual_seed(n)
@@ -72,13 +69,17 @@ def head(a, info):
         nll()
         diff = float((df.float() - dc.float()).norm() / dc.float().norm())
         del dc, df
-        res = alternate([("composition", comp, a.iters), ("fused", fused, a.iters),
-                         ("fused_nll", nll, a.iters)], a.rounds)
+        arms = [("composition", comp, a.iters), ("fused", fused, a.iters),
+                ("fused_nll", nll, a.iters)]
+        if nll512:
+            arms.append(("fused_nll_k512", nll512[n], a.iters))
+        res = alternate(arms, a.rounds)
         med = {}
         for arm, (ms, grow) in res.items():
             med[arm] = statistics.median(ms)
-            flop = (2.0 if arm == "fused_nll" else 8.0) * n * V * K
-            r = {"part": "head", "arm": arm, "N": n, "V": V, "K": K,
+            Kx = 512 if arm == "fused_nll_k512" else K
+            flop = (8.0 if arm in ("composition", "fused") else 2.0) * n * V * Kx
+            r = {"part": "head", "arm": arm, "N": n, "V": V, "K": Kx,
                  "ms": round(med[arm], 3), "ms_all": [round(v, 3) for v in ms],
                  "mem_growth_MB": round(grow / 2 ** 20, 1),
                  "tflops": round(flop / (med[arm] * 1e-3) / 1e12, 1),
@@ -92,13 +93,15 @@ def head(a, info):
         out.append(r)
         print(json.dumps(r), flush=True)
     sess.close()
+    if sess512 is not None:
+        sess512.close()
     return out
 
 
 def step(a, setting, info):
     torch.manual_seed(0)
     model = LM1B(lazy=True, vocab_size=793470, emb_size=512, state_size=2048,
-                 projected_size=512, num_sampled=0, num_steps=20, num_shards=32)
+                 projected_size=a.K, num_sampled=0, num_steps=20, num_shards=32)
     sess, *_ = parallax.parallel_run(
         lm1b_graph(model, batch_size=128), "localhost:0",
         parallax_config=parallax.Config(sess_config={
@@ -120,6 +123,7 @@ def step(a, setting, info):
     e1.record()
     torch.cuda.synchronize()
     r = {"part": "lm1b_step", "full_softmax_train": setting, "num_sampled": 0,
+         **({} if a.K == 512 else {"K": a.K}),
          "ms_per_step": round(e0.elapsed_time(e1) / a.steps, 2),
          "peak_allocated_GB": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2),
          "loss": float(loss), "cuda_graph": bool(getattr(sess.engine, "graph_captured", False)),
@@ -137,6 +141,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--step_settings", nargs="*", default=["composition", "fused"])
+    ap.add_argument("--K", type=int, default=512,
+                    help="columns of the output layer (LM1B's projected_size)")
     ap.add_argument("--step_only", default=None, help=argparse.SUPPRESS)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -152,7 +158,8 @@ def main():
     for setting in a.step_settings:
         # each setting in its own process: peak allocation and allocator state of its own
         p = subprocess.run([sys.executable, os.path.abspath(__file__), "--step_only", setting,
-                            "--steps", str(a.steps), "--warmup", str(a.warmup)],
+                            "--steps", str(a.steps), "--warmup", str(a.warmup),
+                            "--K", str(a.K)],
                            capture_output=True, text=True)
         lines = [ln for ln in p.stdout.splitlines() if ln.startswith("{")]
         if p.returncode != 0 or not lines:
