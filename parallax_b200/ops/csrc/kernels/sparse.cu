@@ -796,9 +796,52 @@ __device__ __forceinline__ void owner_link(const OwnerArgs& a, const int* s_pre,
   if (stamp) ctl->t_dbg[7] = px_globaltimer();
 }
 
+// Sorts the list of ring entries that starts at `first` by ascending entry index (source, then
+// position in the source's ring), in place in next[], and returns the new first entry.  The links
+// come from atomics in whatever order they ran; in this order every owner of a replicated table
+// sums a row's entries alike, so the replicas stay bitwise identical (and a rerun of a step
+// gives the same bits).  Bottom-up merge sort, by one lane: O(L log L) for a list of L entries;
+// kept out of line so that it does not add to the owner kernels' register budget.
+__device__ __noinline__ int owner_sort_list(int32_t* next, int first) {
+  int len = 0;
+  for (int x = first; x != -1; x = __ldcg(next + x)) ++len;
+  for (int run = 1; run < len; run <<= 1) {
+    int cur = first, tail = -1;
+    first = -1;
+    while (cur != -1) {
+      // cut two runs of `run` entries off the front: [x ..] and [y ..]
+      const int x0 = cur;
+      int end = x0;
+      for (int k = 1; k < run && __ldcg(next + end) != -1; ++k) end = __ldcg(next + end);
+      const int y0 = __ldcg(next + end);
+      __stcg(next + end, -1);
+      cur = -1;
+      if (y0 != -1) {
+        end = y0;
+        for (int k = 1; k < run && __ldcg(next + end) != -1; ++k) end = __ldcg(next + end);
+        cur = __ldcg(next + end);
+        __stcg(next + end, -1);
+      }
+      // merge them onto the tail of the sorted list
+      int x = x0, y = y0;
+      while (x != -1 || y != -1) {
+        int pick;
+        if (y == -1 || (x != -1 && x < y)) { pick = x; x = __ldcg(next + x); }
+        else { pick = y; y = __ldcg(next + y); }
+        if (tail == -1) first = pick;
+        else __stcg(next + tail, pick);
+        tail = pick;
+      }
+    }
+    __stcg(next + tail, -1);
+  }
+  return first;
+}
+
 // 16 lanes per entry (two entries per warp in flight).  visit(i, s) runs for every entry i (of
-// source s); head(e, r) for every entry e that heads the list of its row r (without merge: every
-// entry of a row of mine), after which the half-warp resets slotmap[r] for the next step.
+// source s); head(e, r) for every row r with an entry of mine (without merge: for every such
+// entry e), e being the first entry of the row's list once it is sorted by entry index, after
+// which the half-warp resets slotmap[r] for the next step.
 template <typename Visit, typename Head>
 __device__ __forceinline__ void owner_walk(const OwnerArgs& a, const int* s_pre, int total,
                                            Visit visit, Head head) {
@@ -811,7 +854,13 @@ __device__ __forceinline__ void owner_walk(const OwnerArgs& a, const int* s_pre,
     visit(i, s);
     if (r < 0) continue;
     if (a.use_merge && __ldcg(a.slotmap + r) != e) continue;          // not the list head
-    head(e, r);
+    int first = e;
+    if (a.use_merge) {
+      if ((threadIdx.x & 15) == 0) first = owner_sort_list(a.next, e);
+      __syncwarp(hmask);                    // the sorted links are visible to the half-warp
+      first = __shfl_sync(hmask, first, threadIdx.x & 16);
+    }
+    head(first, r);
     __syncwarp(hmask);
     if (a.use_merge && (threadIdx.x & 15) == 0) a.slotmap[r] = -1;
   }

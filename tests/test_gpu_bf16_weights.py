@@ -9,6 +9,7 @@ import torch.nn.functional as F
 import parallax_b200 as parallax
 from parallax_b200 import optim
 from parallax_b200.models.simple import MLPWithEmbedding
+from tests import sparse_plane_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -44,25 +45,6 @@ def _gids(t):
     return gid
 
 
-def _merged(grp):
-    """fp32 merge of this owner's receive rings: [(local rows, rows [n, D])] per table."""
-    from parallax_b200 import ops
-    W, cap = grp.world, grp.cap
-    R = ops.sparse_abi()["hdr_words"] // 3
-    cnt = grp.hdr_buf.tensor(torch.int32, 3 * R).cpu()[2 * R:2 * R + W].tolist()
-    ring_ids = grp.ids_buf.tensor(torch.int32, W * cap).view(W, cap).cpu()
-    out = []
-    for t in grp.tables:
-        ring = t.ring_buf.tensor(grp.wire_dtype, W * cap * t.Dp).view(W, cap, t.Dp).cpu()
-        ids = torch.cat([ring_ids[s, :cnt[s]] for s in range(W)]).long()
-        vals = torch.cat([ring[s, :cnt[s]].double() for s in range(W)])
-        keep = ids >= 0
-        u, inv = torch.unique(ids[keep], return_inverse=True)
-        m = torch.zeros(u.numel(), t.Dp, dtype=torch.float64).index_add_(0, inv, vals[keep])
-        out.append((u, m[:, :t.D].float()))
-    return out
-
-
 def _step(groups, ids_per_rank, grads_per_rank, step):
     for grp, ids, gs in zip(groups, ids_per_rank, grads_per_rank):
         _, pend = grp.lookup(ids.cuda())
@@ -72,7 +54,8 @@ def _step(groups, ids_per_rank, grads_per_rank, step):
     for grp in groups:
         grp.stage_push(step)
     torch.cuda.synchronize()
-    merged = [_merged(grp) for grp in groups]
+    # each owner's receive rings merged per row (fp32 of the fp64 sum): [(local rows, rows)]
+    merged = [[(r.rows, r.sum.float()) for r in sparse_plane_ref.merged(grp)] for grp in groups]
     for grp in groups:
         grp.stage_apply(step)
     torch.cuda.synchronize()
