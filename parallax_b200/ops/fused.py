@@ -1,8 +1,9 @@
 """Fused model-side ops (autograd Functions) for the LM1B hot path.
 
 `lstm_layer`  — a whole unrolled LSTMP layer as ONE autograd node: the
-  sequential part per time step is 2 small GEMMs + 1 fused cell kernel
-  (forward) and 2 GEMMs, the first with the cell backward in its epilogue
+  sequential part is one persistent kernel for all T forward steps (bf16, batch
+  128; elsewhere 2 small GEMMs + 1 fused cell kernel per time step) and, per
+  backward step, 2 GEMMs, the first with the cell backward in its epilogue
   (backward, bf16; elsewhere 2 GEMMs + 1 fused kernel); every weight gradient is
   a single GEMM batched over all time steps (the reference's TF graph issues
   one small GEMM + ~25 elementwise kernels per step and direction:
@@ -25,6 +26,8 @@ register_signatures({
     "px_lstm_cell_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
     "px_lstm_cell_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_lstm_dm_cell_bwd": (_i, [_vp] * 7 + [_i, _i, _i, _i, _vp]),
+    "px_lstm_fwd_persistent_grid": (_i, [_i, _i, _i]),
+    "px_lstm_fwd_persistent": (_i, [_vp] * 8 + [_i, _i, _i, _i, _f, _vp]),
     "px_sampled_softmax": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_sampled_softmax_dot": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
                                     _vp]),
@@ -67,6 +70,22 @@ def _fused_bwd_ok(dt, Bsz, S, P, W_P):
     operand (the other operands are the layer's own 16-byte-aligned buffers)."""
     return (dt == torch.bfloat16 and Bsz % 128 == 0 and S % BWD_BN == 0 and P % 64 == 0 and
             W_P.is_contiguous() and W_P.data_ptr() % 16 == 0)
+
+
+_persistent_grid = {}
+
+
+def _fwd_persistent_ok(dt, Bsz, S, P, Wh, W_P):
+    """All T forward steps fit one `px_lstm_fwd_persistent` launch: bf16, one 128-row tile,
+    S in 128-unit and P in 64-column tiles with P <= 512, Wh and W_P contiguous and 16-byte
+    aligned, and the device keeps the whole grid (S/16 CTAs) resident."""
+    if not (dt == torch.bfloat16 and Wh.is_contiguous() and W_P.is_contiguous() and
+            Wh.data_ptr() % 16 == 0 and W_P.data_ptr() % 16 == 0):
+        return False
+    key = (torch.cuda.current_device(), Bsz, S, P)
+    if key not in _persistent_grid:
+        _persistent_grid[key] = _lib().px_lstm_fwd_persistent_grid(Bsz, S, P)
+    return _persistent_grid[key] > 0
 
 
 def lstm_layer_reference(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
@@ -126,16 +145,24 @@ class _LSTMLayerFn(torch.autograd.Function):
         c_all[0].copy_(c0)
         h_all[0].copy_(h0)
         st = _stream()
-        for t in range(T):
-            # accumulate straight into xw[t] (an `out=` different from the addend makes
-            # torch copy the 2 MB addend first — one more launch per step on the
-            # critical path)
-            gpre = xw[t].addmm_(h_all[t], Wh)
-            _check(L.px_lstm_cell_fwd(_p(gpre), _p(c_all[t]), _p(act[t]),
-                                      _p(c_all[t + 1]), _p(m_all[t]), Bsz, S,
-                                      float(forget_bias), _DT[dt], st), "lstm_cell_fwd")
-            torch.mm(m_all[t], W_P, out=h_all[t + 1])
-        _count(T)
+        if _fwd_persistent_ok(dt, Bsz, S, P, Wh, W_P):
+            # every time step in one cooperative launch, Wh and W_P resident in shared memory
+            ws = torch.empty(S // 128, Bsz, P, dtype=torch.float32, device=dev)
+            _check(L.px_lstm_fwd_persistent(_p(xw), _p(Wh), _p(W_P), _p(act), _p(c_all),
+                                            _p(m_all), _p(h_all), _p(ws), T, Bsz, S, P,
+                                            float(forget_bias), st), "lstm_fwd_persistent")
+            _count(1)
+        else:
+            for t in range(T):
+                # accumulate straight into xw[t] (an `out=` different from the addend makes
+                # torch copy the 2 MB addend first — one more launch per step on the
+                # critical path)
+                gpre = xw[t].addmm_(h_all[t], Wh)
+                _check(L.px_lstm_cell_fwd(_p(gpre), _p(c_all[t]), _p(act[t]),
+                                          _p(c_all[t + 1]), _p(m_all[t]), Bsz, S,
+                                          float(forget_bias), _DT[dt], st), "lstm_cell_fwd")
+                torch.mm(m_all[t], W_P, out=h_all[t + 1])
+            _count(T)
         ctx.save_for_backward(x, Wx, Wh, W_P, act, c_all, m_all, h_all)
         ctx.dims = (T, Bsz, E, S, P)
         return h_all[1:], c_all[T].clone(), h_all[T].clone()

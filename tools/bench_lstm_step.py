@@ -3,7 +3,8 @@ arm captured as a CUDA graph of T dependent time steps (the regime of the real s
 replayed alternately with the other arms:
   unfused: dm = dh·W_P^T (cuBLAS), cell kernel, dh' = dH + dgates·Wh^T (wgmma split-K 8)
   fused:   px_lstm_dm_cell_bwd (BN swept), the same split-K product
-The forward chain (xw[t] += h·Wh, cell kernel, h' = m·W_P) is timed alongside for scale.
+The forward chain is timed the same way, per step (xw[t] += h·Wh, cell kernel, h' = m·W_P) against
+the persistent kernel that runs all T steps in one cooperative launch (px_lstm_fwd_persistent).
 Usage: python tools/bench_lstm_step.py [--rounds R]"""
 import argparse
 import ctypes
@@ -69,6 +70,14 @@ def fwd_unfused():
         torch.mm(m_all[t], WP, out=h_all[t + 1])
 
 
+ws_fwd = torch.empty(S // 128, B, P, device=dev)
+
+
+def fwd_persistent():
+    check(L.px_lstm_fwd_persistent(p_(xw), p_(Wh), p_(WP), p_(act), p_(c_all), p_(m_all),
+                                   p_(h_all), p_(ws_fwd), T, B, S, P, 1.0, st()), "fwd_persistent")
+
+
 def dh_step(t):
     if t > 0:
         G.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=8, bn=64, out=dh_tot[t - 1])
@@ -103,7 +112,8 @@ def graph_of(fn):
     return g
 
 
-arms = [("fwd (addmm, cell, mm)", fwd_unfused), ("bwd unfused (mm, cell, gemm_tn)", bwd_unfused)]
+arms = [("fwd (addmm, cell, mm)", fwd_unfused), ("fwd persistent", fwd_persistent),
+        ("bwd unfused (mm, cell, gemm_tn)", bwd_unfused)]
 for bn in (16, 32, 64):
     arms.append(("bwd fused  BN %2d" % bn, bwd_fused(bn)))
 graphs = [(name, graph_of(fn)) for name, fn in arms]
