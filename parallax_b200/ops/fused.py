@@ -1,12 +1,13 @@
 """Fused model-side ops (autograd Functions) for the LM1B hot path.
 
 `lstm_layer`  — a whole unrolled LSTMP layer as ONE autograd node: the
-  sequential part is one persistent kernel for all T forward steps (bf16, batch
-  128; elsewhere 2 small GEMMs + 1 fused cell kernel per time step) and, per
-  backward step, 2 GEMMs, the first with the cell backward in its epilogue
-  (backward, bf16; elsewhere 2 GEMMs + 1 fused kernel); every weight gradient is
-  a single GEMM batched over all time steps (the reference's TF graph issues
-  one small GEMM + ~25 elementwise kernels per step and direction:
+  sequential part is one persistent kernel for all T forward steps and one for
+  all T backward steps (bf16, batch 128; elsewhere, forward, 2 small GEMMs + 1
+  fused cell kernel per time step and, backward, 2 GEMMs per step, the first
+  with the cell backward in its epilogue for bf16, else 2 GEMMs + 1 fused
+  kernel); every weight gradient is a single GEMM batched over all time steps
+  (the reference's TF graph issues one small GEMM + ~25 elementwise kernels per
+  step and direction:
   `examples/lm1b/language_model.py:76-87`).
 `sampled_softmax_loss` — logits GEMM + one fused kernel that produces the
   loss and the softmax probabilities in place (= gradient wrt logits), so the
@@ -28,6 +29,8 @@ register_signatures({
     "px_lstm_dm_cell_bwd": (_i, [_vp] * 7 + [_i, _i, _i, _i, _vp]),
     "px_lstm_fwd_persistent_grid": (_i, [_i, _i, _i]),
     "px_lstm_fwd_persistent": (_i, [_vp] * 8 + [_i, _i, _i, _i, _f, _vp]),
+    "px_lstm_bwd_persistent_grid": (_i, [_i, _i, _i]),
+    "px_lstm_bwd_persistent": (_i, [_vp] * 10 + [_i, _i, _i, _i, _vp]),
     "px_sampled_softmax": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "px_sampled_softmax_dot": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
                                     _vp]),
@@ -75,17 +78,29 @@ def _fused_bwd_ok(dt, Bsz, S, P, W_P):
 _persistent_grid = {}
 
 
+def _persistent_ok(entry, dt, Bsz, S, P, Wh, W_P):
+    """bf16, Wh and W_P contiguous and 16-byte aligned, and `entry` (a persistent kernel's grid
+    query: its shapes, and whether the device keeps the whole grid resident) takes the layer."""
+    if not (dt == torch.bfloat16 and Wh.is_contiguous() and W_P.is_contiguous() and
+            Wh.data_ptr() % 16 == 0 and W_P.data_ptr() % 16 == 0):
+        return False
+    key = (entry, torch.cuda.current_device(), Bsz, S, P)
+    if key not in _persistent_grid:
+        _persistent_grid[key] = getattr(_lib(), entry)(Bsz, S, P)
+    return _persistent_grid[key] > 0
+
+
 def _fwd_persistent_ok(dt, Bsz, S, P, Wh, W_P):
     """All T forward steps fit one `px_lstm_fwd_persistent` launch: bf16, one 128-row tile,
     S in 128-unit and P in 64-column tiles with P <= 512, Wh and W_P contiguous and 16-byte
     aligned, and the device keeps the whole grid (S/16 CTAs) resident."""
-    if not (dt == torch.bfloat16 and Wh.is_contiguous() and W_P.is_contiguous() and
-            Wh.data_ptr() % 16 == 0 and W_P.data_ptr() % 16 == 0):
-        return False
-    key = (torch.cuda.current_device(), Bsz, S, P)
-    if key not in _persistent_grid:
-        _persistent_grid[key] = _lib().px_lstm_fwd_persistent_grid(Bsz, S, P)
-    return _persistent_grid[key] > 0
+    return _persistent_ok("px_lstm_fwd_persistent_grid", dt, Bsz, S, P, Wh, W_P)
+
+
+def _bwd_persistent_ok(dt, Bsz, S, P, Wh, W_P):
+    """All T backward steps fit one `px_lstm_bwd_persistent` launch: the same conditions as
+    the forward kernel's."""
+    return _persistent_ok("px_lstm_bwd_persistent_grid", dt, Bsz, S, P, Wh, W_P)
 
 
 def lstm_layer_reference(x, Wx, Wh, bias, W_P, c0, h0, forget_bias=1.0):
@@ -222,26 +237,36 @@ class _LSTMLayerFn(torch.autograd.Function):
             dh_tot[T - 1].copy_(dH[T - 1])
         else:
             torch.add(dH[T - 1], dh_rec, out=dh_tot[T - 1])
-        for t in range(T - 1, -1, -1):
-            if fused:
-                _check(L.px_lstm_dm_cell_bwd(_p(dh_tot[t]), _p(W_P), _p(dc), _p(act[t]),
-                                             _p(c_all[t]), _p(c_all[t + 1]), _p(dgates[t]), Bsz,
-                                             S, P, BWD_BN, st), "lstm_dm_cell_bwd")
-            else:
-                torch.mm(dh_tot[t], WPT, out=dm)
-                _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
-                                          _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt], st),
-                       "lstm_cell_bwd")
-            if t > 0:
-                if use_tc:
-                    _gemm.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=8, bn=64,
-                                  out=dh_tot[t - 1])
+        if _bwd_persistent_ok(dt, Bsz, S, P, Wh, W_P) and dH.data_ptr() % 16 == 0:
+            # every time step in one cooperative launch, W_P's and Wh's tiles resident in
+            # shared memory; dh_rec = dgates[0]·Wh^T with no addend
+            dh_rec = torch.empty(Bsz, P, dtype=dt, device=dev)
+            ws_ = torch.empty(4 * S // 512, Bsz, P, dtype=torch.float32, device=dev)
+            _check(L.px_lstm_bwd_persistent(_p(dH), _p(act), _p(c_all), _p(Wh), _p(W_P), _p(dc),
+                                            _p(dgates), _p(dh_tot), _p(dh_rec), _p(ws_), T, Bsz,
+                                            S, P, st), "lstm_bwd_persistent")
+            _count(1)
+        else:
+            for t in range(T - 1, -1, -1):
+                if fused:
+                    _check(L.px_lstm_dm_cell_bwd(_p(dh_tot[t]), _p(W_P), _p(dc), _p(act[t]),
+                                                 _p(c_all[t]), _p(c_all[t + 1]), _p(dgates[t]),
+                                                 Bsz, S, P, BWD_BN, st), "lstm_dm_cell_bwd")
                 else:
-                    torch.addmm(dH[t - 1], dgates[t], WhT, out=dh_tot[t - 1])
-            else:
-                dh_rec = _gemm.gemm_tn(dgates[0], Wh, splits=8, bn=64) if use_tc \
-                    else torch.mm(dgates[0], WhT)
-        _count(T)
+                    torch.mm(dh_tot[t], WPT, out=dm)
+                    _check(L.px_lstm_cell_bwd(_p(dm), _p(dc), _p(act[t]), _p(c_all[t]),
+                                              _p(c_all[t + 1]), _p(dgates[t]), Bsz, S, _DT[dt],
+                                              st), "lstm_cell_bwd")
+                if t > 0:
+                    if use_tc:
+                        _gemm.gemm_tn(dgates[t], Wh, addend=dH[t - 1], splits=8, bn=64,
+                                      out=dh_tot[t - 1])
+                    else:
+                        torch.addmm(dH[t - 1], dgates[t], WhT, out=dh_tot[t - 1])
+                else:
+                    dh_rec = _gemm.gemm_tn(dgates[0], Wh, splits=8, bn=64) if use_tc \
+                        else torch.mm(dgates[0], WhT)
+            _count(T)
         dg2 = dgates.view(T * Bsz, 4 * S)
         # the bias gradient, a bandwidth-bound column sum, runs on a second side stream next
         # to the compute-bound weight-gradient GEMMs

@@ -3,6 +3,7 @@ arm captured as a CUDA graph of T dependent time steps (the regime of the real s
 replayed alternately with the other arms:
   unfused: dm = dh·W_P^T (cuBLAS), cell kernel, dh' = dH + dgates·Wh^T (wgmma split-K 8)
   fused:   px_lstm_dm_cell_bwd (BN swept), the same split-K product
+  persistent: px_lstm_bwd_persistent, all T steps in one cooperative launch
 The forward chain is timed the same way, per step (xw[t] += h·Wh, cell kernel, h' = m·W_P) against
 the persistent kernel that runs all T steps in one cooperative launch (px_lstm_fwd_persistent).
 Usage: python tools/bench_lstm_step.py [--rounds R]"""
@@ -101,6 +102,16 @@ def bwd_fused(bn):
     return run
 
 
+ws_bwd = torch.empty(4 * S // 512, B, P, device=dev)
+dh_rec = torch.empty(B, P, dtype=bf, device=dev)
+
+
+def bwd_persistent():
+    check(L.px_lstm_bwd_persistent(p_(dH), p_(act), p_(c_all), p_(Wh), p_(WP), p_(dc),
+                                   p_(dgates), p_(dh_tot), p_(dh_rec), p_(ws_bwd), T, B, S, P,
+                                   st()), "bwd_persistent")
+
+
 def graph_of(fn):
     for _ in range(2):
         xw.copy_(xw0)
@@ -116,6 +127,7 @@ arms = [("fwd (addmm, cell, mm)", fwd_unfused), ("fwd persistent", fwd_persisten
         ("bwd unfused (mm, cell, gemm_tn)", bwd_unfused)]
 for bn in (16, 32, 64):
     arms.append(("bwd fused  BN %2d" % bn, bwd_fused(bn)))
+arms.append(("bwd persistent", bwd_persistent))
 graphs = [(name, graph_of(fn)) for name, fn in arms]
 times = {name: [] for name, _ in graphs}
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
