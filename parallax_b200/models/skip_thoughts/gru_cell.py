@@ -12,10 +12,13 @@ recurrent matrices start as random orthonormal blocks, input matrices uniform
 There is no cuDNN kernel for a layer-normalised GRU, so the layer is arranged
 for the GPU rather than as a cell: both input projections and their layer norms
 are computed for ALL time steps with two GEMMs before the recurrence, and each
-step does a single fused ``h @ [W_h | U]`` GEMM.
+step does a single fused ``h @ [W_h | U]`` GEMM.  On the GPU the recurrence is one autograd
+node with one cell kernel per step each way (`ops/fused.py: ln_gru_layer`).
 """
 import torch
 import torch.nn as nn
+
+from ...ops import fused
 
 
 def random_orthonormal_(w):
@@ -54,12 +57,28 @@ class LayerNormGRU(nn.Module):
         cand = torch.tanh(r * self.ln_u(hh[:, 2 * n:]) + cx_t)
         return (1.0 - z) * h + z * cand
 
+    def _input_side(self, x):
+        """both input projections and their layer norms, for all steps at once"""
+        return self.ln_wx(x @ self.w_x), self.ln_w(x @ self.w)
+
     def forward(self, x, lengths=None, initial_state=None, reverse=False):
         """x [B,T,I] → (outputs [B,T,U] zero past each length, final state [B,U]).
-        `reverse=True` runs each sequence back to front (inside its own length)."""
+        `reverse=True` runs each sequence back to front (inside its own length).
+
+        On CUDA in bf16 or fp32, with n % 8 == 0 and n <= 4096, the recurrence is one fused
+        autograd node (`ops.fused.ln_gru_layer`: a product and one cell kernel per step each
+        way); otherwise (CPU, fp64, other shapes) it is `_composition`."""
+        if fused.ln_gru_applies(x, self.w_hu, self.ln_wh, self.ln_u, initial_state):
+            gx, cx = self._input_side(x)
+            return fused.ln_gru_layer(gx, cx, self.w_hu, self.ln_wh, self.ln_u, initial_state,
+                                      lengths, reverse)
+        return self._composition(x, lengths, initial_state, reverse)
+
+    def _composition(self, x, lengths=None, initial_state=None, reverse=False):
+        """The layer as plain PyTorch ops, one time step at a time: the fallback of `forward`
+        and the oracle of the fused node."""
         B, T, _ = x.shape
-        gx = self.ln_wx(x @ self.w_x)            # all steps at once
-        cx = self.ln_w(x @ self.w)
+        gx, cx = self._input_side(x)
         h = initial_state if initial_state is not None else \
             torch.zeros(B, self.num_units, device=x.device, dtype=x.dtype)
         outs = [None] * T

@@ -15,6 +15,10 @@
 
 Both have a pure-PyTorch implementation (`*_reference`) which is the numerics
 oracle in the tests and the path used on the host fabric.
+`ln_gru_layer` — the skip-thoughts layer-normalised GRU recurrence as ONE autograd node: per
+  time step a cuBLAS product in fp32 and one cell kernel forward, one cell kernel and a cuBLAS
+  product backward (`kernels/ln_gru.cu`); `w_hu`'s gradient is one GEMM over all steps.  Its
+  oracle is the composition in `LayerNormGRU._composition`.
 """
 import ctypes
 
@@ -36,6 +40,12 @@ register_signatures({
                                     _vp]),
     "px_ssm_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _f, _vp, _vp, _vp, _i, _vp, _i, _i, _i,
                         _vp]),
+    "px_ln_gru_max_units": (_i, []),
+    "px_ln_gru_fwd": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp,
+                           _i, _i, _i, _f, _f, _i, _vp]),
+    "px_ln_gru_bwd": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp,
+                           _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "px_ln_gru_param_grad": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp]),
 })
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 
@@ -322,6 +332,142 @@ def lstm_layer_stacked(x, W, bias, W_P, c0, h0, forget_bias=1.0):
     if x.is_cuda and x.dtype in _DT:
         return _LSTMLayerFn.apply(x, W, None, bias, W_P, c0, h0, forget_bias)
     return lstm_layer_reference(x, W[:E], W[E:], bias, W_P, c0, h0, forget_bias)
+
+
+# ===========================================================================
+# layer-normalised GRU layer (skip-thoughts)
+# ===========================================================================
+def _addr(t, offset):
+    """Device address of element `offset` of tensor `t`."""
+    return _vp(t.data_ptr() + offset * t.element_size())
+
+
+def _mm_f32(a, b, out):
+    """out (fp32) = a·b on cuBLAS, with an fp32 output for bf16 operands too."""
+    if a.dtype == torch.float32:
+        return torch.mm(a, b, out=out)
+    return torch.mm(a, b, out_dtype=torch.float32, out=out)
+
+
+def ln_gru_applies(x, w_hu, ln_wh, ln_u, h0=None):
+    """The fused node takes the layer: a CUDA tensor in bf16 or fp32 with w_hu and both
+    LayerNorms' γ/β in the same dtype, w_hu contiguous and 16-byte aligned, n % 8 == 0 and
+    n <= `px_ln_gru_max_units()` (4096: 8 units per thread, 2 groups per thread, one 256-thread
+    CTA per row), and an initial state, if any, of the same dtype."""
+    dt = x.dtype
+    if not (x.is_cuda and dt in _DT and w_hu.dtype == dt):
+        return False
+    n = w_hu.shape[0]
+    params = (ln_wh.weight, ln_wh.bias, ln_u.weight, ln_u.bias)
+    if any(p is None or p.dtype != dt or not p.is_contiguous() for p in params):
+        return False
+    if h0 is not None and h0.dtype != dt:
+        return False
+    return (n % 8 == 0 and n <= _lib().px_ln_gru_max_units() and w_hu.is_contiguous() and
+            w_hu.data_ptr() % 16 == 0)
+
+
+def _ln_gru_forward(gx, cx, w_hu, lnp, h0, lengths, reverse, eps, save):
+    """All T steps -> (out [B, T, n], hs, hh, stats).  hs [T+1, B, n] holds the state before
+    each step in processing order, hh [T, B, 3n] (fp32) each step's h·w_hu and stats [T, B, 4]
+    its LayerNorm (mean, rstd) pairs; without `save`, hs and hh are ping-pong / scratch buffers
+    and stats is None."""
+    L = _lib()
+    B, T, n2 = gx.shape
+    n = n2 // 2
+    dt, dev = gx.dtype, gx.device
+    hs = torch.empty(T + 1 if save else 2, B, n, dtype=dt, device=dev)
+    if h0 is None:
+        hs[0].zero_()
+    else:
+        hs[0].copy_(h0)
+    hh = torch.empty(T if save else 1, B, 3 * n, dtype=torch.float32, device=dev)
+    stats = torch.empty(T, B, 4, dtype=torch.float32, device=dev) if save else None
+    out = torch.empty(B, T, n, dtype=dt, device=dev)
+    st = _stream()
+    for s in range(T):
+        t = T - 1 - s if reverse else s
+        i, o = (s, s + 1) if save else (s % 2, (s + 1) % 2)
+        hh_s = hh[s] if save else hh[0]
+        _mm_f32(hs[i], w_hu, hh_s)
+        _check(L.px_ln_gru_fwd(_p(hh_s), _addr(gx, t * 2 * n), T * 2 * n, _addr(cx, t * n), T * n,
+                               _p(hs[i]), _p(hs[o]), _addr(out, t * n), T * n,
+                               _p(stats[s]) if save else None, *[_p(p) for p in lnp],
+                               None if lengths is None else _p(lengths), t, B, n, eps[0], eps[1],
+                               _DT[dt], st), "ln_gru_fwd")
+    _count(T)
+    return out, hs[T] if save else hs[T % 2], hs, hh, stats
+
+
+class _LNGRULayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, gx, cx, w_hu, g_wh, b_wh, g_u, b_u, h0, lengths, reverse, eps_wh, eps_u):
+        out, hT, hs, hh, stats = _ln_gru_forward(gx, cx, w_hu, (g_wh, b_wh, g_u, b_u), h0, lengths,
+                                                 reverse, (eps_wh, eps_u), True)
+        ctx.save_for_backward(gx, cx, w_hu, g_wh, b_wh, g_u, b_u, hs, hh, stats, lengths)
+        ctx.reverse = reverse
+        ctx.set_materialize_grads(False)
+        return out, hT.clone()
+
+    @staticmethod
+    def backward(ctx, d_out, d_final):
+        L = _lib()
+        gx, cx, w_hu, g_wh, b_wh, g_u, b_u, hs, hh, stats, lengths = ctx.saved_tensors
+        B, T, n2 = gx.shape
+        n = n2 // 2
+        dt, dev = gx.dtype, gx.device
+        if d_out is not None:
+            d_out = d_out.contiguous()
+            if d_out.data_ptr() % 16:
+                d_out = d_out.clone()
+        carry = torch.zeros(B, n, dtype=torch.float32, device=dev) if d_final is None \
+            else d_final.float().clone()
+        drec = torch.empty(B, n, dtype=torch.float32, device=dev)
+        dhh = torch.empty(T, B, 3 * n, dtype=dt, device=dev)
+        dgx = torch.empty(B, T, 2 * n, dtype=dt, device=dev)
+        dcx = torch.empty(B, T, n, dtype=dt, device=dev)
+        acc = torch.empty(B, 6 * n, dtype=torch.float32, device=dev)
+        lnp = [_p(p) for p in (g_wh, b_wh, g_u, b_u)]
+        lp = None if lengths is None else _p(lengths)
+        need_h0 = ctx.needs_input_grad[7]
+        w_t = w_hu.t()
+        st = _stream()
+        for k in range(T):
+            s = T - 1 - k
+            t = T - 1 - s if ctx.reverse else s
+            _check(L.px_ln_gru_bwd(_p(hh[s]), _p(stats[s]), _addr(gx, t * 2 * n), T * 2 * n,
+                                   _addr(cx, t * n), T * n, _p(hs[s]),
+                                   None if d_out is None else _addr(d_out, t * n), T * n,
+                                   None if k == 0 else _p(drec), _p(carry), _p(dhh[s]),
+                                   _addr(dgx, t * 2 * n), T * 2 * n, _addr(dcx, t * n), T * n,
+                                   _p(acc), int(k == 0), *lnp, lp, t, B, n, _DT[dt], st),
+                   "ln_gru_bwd")
+            if s > 0 or need_h0:
+                _mm_f32(dhh[s], w_t, drec)
+        dh0 = drec.add_(carry).to(dt) if need_h0 else None
+        dw_hu = torch.mm(hs[:T].reshape(T * B, n).t(), dhh.view(T * B, 3 * n))
+        dln = [torch.empty_like(p) for p in (g_wh, b_wh, g_u, b_u)]
+        _check(L.px_ln_gru_param_grad(_p(acc), B, n, *[_p(d) for d in dln], _DT[dt], st),
+               "ln_gru_param_grad")
+        _count(T + 1)
+        return (dgx, dcx, dw_hu, *dln, dh0, None, None, None, None)
+
+
+def ln_gru_layer(gx, cx, w_hu, ln_wh, ln_u, h0=None, lengths=None, reverse=False):
+    """The recurrence of `LayerNormGRU` from its input-side terms gx = LN_wx(x·w_x) [B, T, 2n]
+    and cx = LN_w(x·w) [B, T, n] -> (outputs [B, T, n], zero past each length; final state
+    [B, n]).  `lengths` [B] masks each row as the composition does; `reverse` walks t from T−1
+    down to 0.  Callers check `ln_gru_applies` first.  Without autograd (no_grad, or nothing
+    requiring a gradient) nothing is kept for a backward pass."""
+    gx, cx = gx.contiguous(), cx.contiguous()
+    if lengths is not None:
+        lengths = lengths.to(device=gx.device, dtype=torch.int64).contiguous()
+    args = (gx, cx, w_hu, ln_wh.weight, ln_wh.bias, ln_u.weight, ln_u.bias, h0)
+    eps = (float(ln_wh.eps), float(ln_u.eps))
+    if torch.is_grad_enabled() and any(a is not None and a.requires_grad for a in args):
+        return _LNGRULayerFn.apply(*args, lengths, bool(reverse), *eps)
+    out, hT, _, _, _ = _ln_gru_forward(gx, cx, w_hu, args[3:7], h0, lengths, reverse, eps, False)
+    return out, hT
 
 
 # ===========================================================================
