@@ -25,7 +25,8 @@ stacks (packed by length), and in the GNMT decoder every layer above the
 attention layer (those depend on the *contexts*, which the bottom layer
 produces for all steps first); only the layers that feed attention back into
 their own input run step by step.  The same modules serve the step API used by
-greedy/sampling/beam decoding (`inference.py`).
+greedy/sampling/beam decoding (`inference.py`).  On the GPU, with LSTM cells, those step-by-step
+layers and the attention are one fused autograd node (`ops/fused.py: nmt_attention_decoder`).
 """
 import math
 
@@ -37,6 +38,7 @@ from torch.nn.utils.rnn import pack_padded_sequence, pad_packed_sequence
 from ... import nn as pnn
 from ... import optim
 from ...graph import Graph, ClipByGlobalNorm
+from ...ops import fused
 from ...partitions import get_partitioner
 from .attention import AttentionMechanism
 
@@ -314,9 +316,103 @@ class Decoder(nn.Module):
             out["attention"] = sel(state["attention"])
         return out
 
+    # -- the fused node ---------------------------------------------------------------
+    def node_arguments(self):
+        """(layers, keyword arguments) of `fused.nmt_attention_decoder` (and of its reference)
+        for this decoder's parameters: the layers that feed attention back into their input,
+        every layer for standard and the bottom one for gnmt / gnmt_v2."""
+        layers = self.layers if self.architecture == "standard" else self.layers[:1]
+        rnn = [l.rnn for l in layers]
+        a = self.attention
+        kw = dict(w_ih=[r.weight_ih_l0 for r in rnn], w_hh=[r.weight_hh_l0 for r in rnn],
+                  b_ih=[r.bias_ih_l0 for r in rnn], b_hh=[r.bias_hh_l0 for r in rnn],
+                  residual=[l.residual for l in layers])
+        extra = []
+        if a.option in ("bahdanau", "normed_bahdanau"):
+            kw["w_q"] = a.query_layer.weight
+            extra = [a.v]
+            if a.option == "normed_bahdanau":
+                kw["b"] = a.b
+                extra.append(a.g)
+        elif a.option == "scaled_luong":
+            kw["g"] = a.g
+        if self.architecture == "standard":
+            kw["w_a"] = self.attention_layer.weight
+        if a.option in ("bahdanau", "normed_bahdanau"):
+            v = a.g * a.v / a.v.norm() if a.option == "normed_bahdanau" else a.v
+            kw["v"] = v if v.dtype == torch.float64 else v.float().contiguous()
+        return layers, kw, extra
+
+    def _node(self, emb, state, memory):
+        """`node_arguments` when the fused node takes this decoder, else None (no attention,
+        other cells, CPU, fp64, shapes outside the kernels' limits)."""
+        if self.architecture == "none":
+            return None
+        layers = self.layers if self.architecture == "standard" else self.layers[:1]
+        if any(l.unit_type != "lstm" for l in layers) or not emb.is_cuda:
+            return None
+        layers, kw, extra = self.node_arguments()
+        keys, values, _ = memory
+        cells = state["cells"][:len(layers)]
+        weights = kw["w_ih"] + kw["w_hh"] + kw["b_ih"] + kw["b_hh"] + extra + \
+            [kw.get(k) for k in ("w_q", "g", "b", "w_a")]
+        states = [x for c in cells for x in c] + [state["attention"]]
+        if not fused.nmt_decoder_applies(emb, keys, values, weights, states, layers[0].unit_type):
+            return None
+        return layers, kw
+
+    def _dropout_masks(self, layers, T, emb):
+        """Per layer [T, B, I_l] input masks (0 or 1/(1−p), in emb's dtype) when training with
+        dropout, else None: the same distribution as the composition's `F.dropout`, drawn
+        here because the fused node takes its masks as tensors."""
+        if not (self.training and any(l.dropout > 0 for l in layers)):
+            return None
+        B = emb.shape[0]
+        masks = []
+        for l in layers:
+            keep = 1.0 - l.dropout
+            m = torch.empty(T, B, l.input_size, dtype=emb.dtype, device=emb.device)
+            masks.append(m.bernoulli_(keep).div_(keep) if l.dropout > 0 else m.fill_(1.0))
+        return masks
+
+    def _gnmt_upper(self, x, ctx, state):
+        """GNMT layers above the bottom one, as whole-sequence calls over (h⁰_t, context)"""
+        if self.architecture == "gnmt":          # upper layers use the previous context
+            ctx = torch.cat([state["attention"][:, None, :], ctx[:, :-1]], 1)
+        for layer, st in zip(self.layers[1:], state["cells"][1:]):
+            x, _ = layer(torch.cat([x, ctx], -1), st)
+        return x
+
     # -- one step (inference; also the inner loop of the attention layers) --------
     def step(self, emb_t, state, memory):
-        """emb_t [B,U] → (output [B,U], new state).  `memory` = attention.prepare(…)"""
+        """emb_t [B,U] → (output [B,U], new state).  `memory` = attention.prepare(…)
+
+        Without gradients and when the fused node applies, the attention layers run as one
+        step of it (nothing saved); otherwise as `_step`."""
+        grad = torch.is_grad_enabled() and (emb_t.requires_grad or
+                                            any(p.requires_grad for p in self.parameters()))
+        node = None if grad else self._node(emb_t, state, memory)
+        if node is None:
+            return self._step(emb_t, state, memory)
+        layers, kw = node
+        keys, values, pad = memory
+        cells = state["cells"]
+        n = len(layers)
+        q, att, hs, cs = fused.nmt_attention_decoder_step(
+            emb_t, [c[0] for c in cells[:n]], [c[1] for c in cells[:n]], state["attention"],
+            keys, values, pad, masks=self._dropout_masks(layers, 1, emb_t), **kw)
+        new_cells = list(zip(hs, cs))
+        if self.architecture == "standard":
+            return (att if self.output_attention else q), {"cells": new_cells, "attention": att}
+        x, fed = q, (att if self.architecture == "gnmt_v2" else state["attention"])
+        for layer, st in zip(self.layers[1:], cells[1:]):
+            x, s2 = layer.step(torch.cat([x, fed], -1), st)
+            new_cells.append(s2)
+        return x, {"cells": new_cells, "attention": att}
+
+    def _step(self, emb_t, state, memory):
+        """One step of the composition: each layer's `RNNLayer.step`, the attention and the
+        attention layer as separate PyTorch ops."""
         cells, new_cells = state["cells"], []
         if self.architecture == "none":
             x = emb_t
@@ -346,7 +442,30 @@ class Decoder(nn.Module):
 
     # -- teacher-forced training pass ------------------------------------------------
     def forward(self, emb, state, memory):
-        """emb [B,T,U] → outputs [B,T,U]"""
+        """emb [B,T,U] → outputs [B,T,U].
+
+        With LSTM cells on CUDA in bf16 or fp32 and shapes within the kernels' limits, the
+        attention recurrence is one fused autograd node (`fused.nmt_attention_decoder`); every
+        other case runs `_composition`.  With dropout the node's masks come from the same
+        distribution as the composition's but not from the same random stream."""
+        node = self._node(emb, state, memory)
+        if node is None:
+            return self._composition(emb, state, memory)
+        layers, kw = node
+        keys, values, pad = memory
+        n = len(layers)
+        cells = state["cells"][:n]
+        out = fused.nmt_attention_decoder(
+            emb, [c[0] for c in cells], [c[1] for c in cells], state["attention"], keys, values,
+            pad, masks=self._dropout_masks(layers, emb.shape[1], emb),
+            output_attention=self.output_attention, **kw)
+        if self.architecture == "standard":
+            return out
+        return self._gnmt_upper(*out, state)
+
+    def _composition(self, emb, state, memory):
+        """The decoder as plain PyTorch ops, one time step at a time: the fallback of `forward`
+        and the oracle of the fused node."""
         if self.architecture == "none":
             out, _ = run_stack(self.layers, emb, None, state["cells"])
             return out
@@ -355,7 +474,7 @@ class Decoder(nn.Module):
         if self.architecture == "standard":
             outs = []
             for t in range(T):
-                o, state = self.step(emb[:, t], state, memory)
+                o, state = self._step(emb[:, t], state, memory)
                 outs.append(o)
             return torch.stack(outs, 1)
         # GNMT: only the bottom layer is recurrent through attention; the layers
@@ -367,12 +486,7 @@ class Decoder(nn.Module):
             prev, _ = self.attention(h, keys, values, pad)
             hs.append(h)
             ctxs.append(prev)
-        x, ctx = torch.stack(hs, 1), torch.stack(ctxs, 1)
-        if self.architecture == "gnmt":          # upper layers use the previous context
-            ctx = torch.cat([state["attention"][:, None, :], ctx[:, :-1]], 1)
-        for layer, st in zip(self.layers[1:], state["cells"][1:]):
-            x, _ = layer(torch.cat([x, ctx], -1), st)
-        return x
+        return self._gnmt_upper(torch.stack(hs, 1), torch.stack(ctxs, 1), state)
 
 
 # --------------------------------------------------------------------- model

@@ -19,6 +19,11 @@ oracle in the tests and the path used on the host fabric.
   time step a cuBLAS product in fp32 and one cell kernel forward, one cell kernel and a cuBLAS
   product backward (`kernels/ln_gru.cu`); `w_hu`'s gradient is one GEMM over all steps.  Its
   oracle is the composition in `LayerNormGRU._composition`.
+`nmt_attention_decoder` — the NMT decoder's attention recurrence (standard: every layer; gnmt:
+  the bottom layer) as ONE autograd node: per time step a cuBLAS product and one cell kernel per
+  layer and one attention kernel (`kernels/nmt_decoder.cu`) each way; every weight gradient is one
+  GEMM over all steps.  Its oracle is `nmt_attention_decoder_reference`, which equals
+  `Decoder._composition`.
 """
 import ctypes
 
@@ -46,6 +51,18 @@ register_signatures({
     "px_ln_gru_bwd": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp,
                            _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "px_ln_gru_param_grad": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp]),
+    "px_nmt_max_units": (_i, []),
+    "px_nmt_max_memory": (_i, []),
+    "px_nmt_max_source": (_i, []),
+    "px_nmt_attn_fwd": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp,
+                             _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "px_nmt_attn_bwd": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i] + [_vp] * 13 +
+                        [_i, _i, _i, _i, _i, _i, _vp]),
+    "px_nmt_attn_param_grad": (_i, [_vp, _i, _i, _vp, _vp]),
+    "px_nmt_lstm_cell_fwd": (_i, [_vp] * 6 + [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i,
+                                              _i, _i, _i, _vp]),
+    "px_nmt_lstm_cell_bwd": (_i, [_vp] * 6 + [_vp, _i, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp,
+                                              _vp, _i, _i, _i, _vp]),
 })
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 
@@ -468,6 +485,441 @@ def ln_gru_layer(gx, cx, w_hu, ln_wh, ln_u, h0=None, lengths=None, reverse=False
         return _LNGRULayerFn.apply(*args, lengths, bool(reverse), *eps)
     out, hT, _, _, _ = _ln_gru_forward(gx, cx, w_hu, args[3:7], h0, lengths, reverse, eps, False)
     return out, hT
+
+
+# ===========================================================================
+# NMT attention decoder
+# ===========================================================================
+def nmt_decoder_applies(emb, keys, values, weights, states, unit_type="lstm"):
+    """The fused node takes the decoder: LSTM cells, a CUDA tensor in bf16 or fp32 with every
+    weight and state in the same dtype, the matrices contiguous and 16-byte aligned, keys
+    [B, S, U] and values [B, S, M] contiguous and 16-byte aligned, U % 8 == 0 and M % 8 == 0,
+    and U, M and S within `px_nmt_max_units` / `px_nmt_max_memory` / `px_nmt_max_source`
+    (1024 / 2048 / 1024)."""
+    dt = emb.dtype
+    if unit_type != "lstm" or not (emb.is_cuda and dt in _DT):
+        return False
+    if any(t is not None and t.dtype != dt for t in list(weights) + list(states) + [keys, values]):
+        return False
+    for w in weights:
+        if w is not None and w.dim() == 2 and not (w.is_contiguous() and w.data_ptr() % 16 == 0):
+            return False
+    for t in (keys, values):
+        if not (t.is_contiguous() and t.data_ptr() % 16 == 0):
+            return False
+    B, S, U = keys.shape
+    M = values.shape[2]
+    L = _lib()
+    return (U % 8 == 0 and M % 8 == 0 and emb.shape[-1] == U and U <= L.px_nmt_max_units() and
+            M <= L.px_nmt_max_memory() and S <= L.px_nmt_max_source())
+
+
+def _mask_mul(x, m):
+    return x if m is None else x * m
+
+
+def nmt_attention_decoder_reference(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh,
+                                    residual, w_q=None, g=None, v=None, b=None, w_a=None,
+                                    masks=None, output_attention=True):
+    """Pure-PyTorch version of `nmt_attention_decoder` (same arguments, same masks): the fp64
+    oracle of the node's tests.  State and gates are kept in the accumulation type (fp32 for
+    bf16/fp32 inputs)."""
+    B, T, U = emb.shape
+    L = len(w_ih)
+    dt = emb.dtype
+    h, c = list(h0), [_acc(x) for x in c0]
+    feed = att0
+    outs, qs, ctxs = [], [], []
+    for t in range(T):
+        x = torch.cat([emb[:, t], feed], -1)
+        for l in range(L):
+            inp = _mask_mul(x, None if masks is None else masks[l][t])
+            gates = _acc(torch.nn.functional.linear(inp, w_ih[l], b_ih[l]) +
+                         torch.nn.functional.linear(h[l], w_hh[l], b_hh[l]))
+            i, f, gg, o = gates.chunk(4, -1)
+            c[l] = torch.sigmoid(f) * c[l] + torch.sigmoid(i) * torch.tanh(gg)
+            h[l] = (torch.sigmoid(o) * torch.tanh(c[l])).to(dt)
+            x = h[l] + x[..., :U] if residual[l] else h[l]
+        q = x
+        if v is not None:
+            hid = keys + (q @ w_q.t())[:, None, :]
+            if b is not None:
+                hid = hid + b
+            s = (torch.tanh(hid) * v.to(hid.dtype)).sum(-1)
+        else:
+            s = torch.bmm(q[:, None, :], keys.transpose(1, 2))[:, 0]
+            if g is not None:
+                s = s * g.to(s.dtype)
+        a = torch.softmax(_acc(s).masked_fill(pad, float("-inf")), -1)
+        ctx = torch.bmm(a[:, None, :].to(values.dtype), values)[:, 0]
+        if w_a is not None:
+            feed = torch.cat([q, ctx], -1) @ w_a.t()
+            outs.append(feed if output_attention else q)
+        else:
+            feed = ctx
+            qs.append(q)
+            ctxs.append(ctx)
+    if w_a is not None:
+        return torch.stack(outs, 1)
+    return torch.stack(qs, 1), torch.stack(ctxs, 1)
+
+
+def _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, save):
+    """All T steps of the decoder -> dict of buffers (module docstring of
+    `kernels/nmt_decoder.cu`; DESIGN.md §5).  Time-major per-step buffers:
+    xh[l] [T+1, B, K_l] = [input ⊙ mask | h_{t-1}] (layer 0: [emb ⊙ mask | feed ⊙ mask | h]),
+    P[l] [T, B, 4U] fp32 products, C[l] [T+1, B, U] fp32 cell states, qc [T, B, U+M] = [q | ctx],
+    align [T, B, S] fp32, pq [T, B, U] fp32.  Without `save` the recurrent buffers are ping-pong
+    pairs and only what the outputs need is kept."""
+    Lb = _lib()
+    L, std, bah, res = cfg["L"], cfg["standard"], cfg["bahdanau"], cfg["residual"]
+    w_ih, w_hh, b_ih, b_hh = W["w_ih"], W["w_hh"], W["b_ih"], W["b_hh"]
+    B, T, U = emb.shape
+    S, M = keys.shape[1], values.shape[2]
+    A = att0.shape[1]
+    dt, dev = emb.dtype, emb.device
+    nT = T + 1 if save else 2
+    sl = (lambda t: t) if save else (lambda t: t % 2)
+    I = [U + A] + [U] * (L - 1)
+    K = [I[0] + U] + [I[l] + U for l in range(1, L)]
+    xh = [torch.empty(nT, B, K[l], dtype=dt, device=dev) for l in range(L)]
+    C = [torch.empty(nT, B, U, dtype=torch.float32, device=dev) for _ in range(L)]
+    P = [torch.empty(T if save else 1, B, 4 * U, dtype=torch.float32, device=dev)
+         for _ in range(L)]
+    qc = torch.empty(T, B, U + M, dtype=dt, device=dev)
+    align = torch.empty(T if save else 1, B, S, dtype=torch.float32, device=dev)
+    pq = torch.empty(T if save else 1, B, U, dtype=torch.float32, device=dev) if bah else None
+    att = torch.empty(T, B, U, dtype=dt, device=dev) if std else None
+    ybuf = [torch.empty(B, U, dtype=dt, device=dev) for _ in range(L - 1)]
+    # W_step[l]: the columns a step multiplies (layer 0: feed and h; the embedding part is one
+    # product over all T before the loop)
+    w_step = [torch.cat([w_ih[0][:, U:], w_hh[0]], 1)] + \
+        [torch.cat([w_ih[l], w_hh[l]], 1) for l in range(1, L)]
+    m0 = None if masks is None else masks[0]
+    embT = emb.transpose(0, 1)
+    e_part = xh[0][:T, :, :U] if save else torch.empty(T, B, U, dtype=dt, device=dev)
+    if m0 is None:
+        e_part.copy_(embT)
+    else:
+        torch.mul(embT, m0[:, :, :U], out=e_part)
+    gx0 = torch.empty(T, B, 4 * U, dtype=torch.float32, device=dev)
+    _mm_f32(e_part.reshape(T * B, U), w_ih[0][:, :U].t(), gx0.view(T * B, 4 * U))
+    if m0 is None:
+        xh[0][0, :, U:U + A].copy_(att0)
+    else:
+        torch.mul(att0, m0[0, :, U:], out=xh[0][0, :, U:U + A])
+    for l in range(L):
+        xh[l][0, :, I[l]:].copy_(h0[l])
+        C[l][0].copy_(c0[l])
+    kind = 1 if bah else 0
+    g_p = _p(attn["g"]) if attn["g"] is not None else None
+    v_p = _p(attn["v"]) if bah else None
+    b_p = _p(attn["b"]) if attn["b"] is not None else None
+    emb_ld = T * U
+    st = _stream()
+    for t in range(T):
+        i0, i1 = sl(t), sl(t + 1)
+        for l in range(L):
+            Pt = P[l][t] if save else P[l][0]
+            _mm_f32(xh[l][i0, :, U if l == 0 else 0:], w_step[l].t(), Pt)
+            top = l == L - 1
+            if res[l]:
+                resid, r_ld = ((_addr(emb, t * U), emb_ld) if l == 0 else (_p(ybuf[l - 1]), U))
+            else:
+                resid, r_ld = None, 0
+            y, y_ld = (_p(qc[t]), U + M) if top else (_p(ybuf[l]), U)
+            if top:
+                xn, xn_ld, mk, mk_ld = None, 0, None, 0
+            else:
+                xn, xn_ld = _p(xh[l + 1][i0]), K[l + 1]
+                mk, mk_ld = (None, 0) if masks is None else (_p(masks[l + 1][t]), I[l + 1])
+            _check(Lb.px_nmt_lstm_cell_fwd(
+                _p(Pt), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]), _p(C[l][i0]),
+                _p(C[l][i1]), _addr(xh[l][i1], I[l]), K[l], resid, r_ld, y, y_ld, mk, mk_ld, xn,
+                xn_ld, B, U, _DT[dt], st), "nmt_lstm_cell_fwd")
+        q = qc[t][:, :U]
+        pq_t = None
+        if bah:
+            pq_t = pq[t] if save else pq[0]
+            _mm_f32(q, attn["w_q"].t(), pq_t)
+        feed, feed_ld, fm, fm_ld = None, 0, None, 0
+        if not std and t + 1 < T:
+            feed, feed_ld = _addr(xh[0][i1], U), K[0]
+            if m0 is not None:
+                fm, fm_ld = _addr(m0[t + 1], U), I[0]
+        _check(Lb.px_nmt_attn_fwd(
+            _p(qc[t]), U + M, _p(pq_t) if bah else None, _p(keys), _p(values), _p(pad), g_p,
+            v_p, b_p, _addr(qc[t], U), U + M, fm, fm_ld, feed, feed_ld,
+            _p(align[t] if save else align[0]), B, S, U, M, kind, _DT[dt], st), "nmt_attn_fwd")
+        if std:
+            torch.mm(qc[t], W["w_a"].t(), out=att[t])
+            if t + 1 < T:
+                dst = xh[0][i1, :, U:U + A]
+                if m0 is None:
+                    dst.copy_(att[t])
+                else:
+                    torch.mul(att[t], m0[t + 1, :, U:], out=dst)
+    _count(T * (L + 1))
+    return dict(xh=xh, C=C, P=P, qc=qc, align=align, pq=pq, att=att, gx0=gx0, w_step=w_step,
+                e_part=e_part, last=sl(T))
+
+
+def _nmt_outputs(cfg, F, U, output_attention):
+    if cfg["standard"]:
+        if output_attention:
+            return F["att"].transpose(0, 1)
+        return F["qc"][:, :, :U].transpose(0, 1).contiguous()
+    return (F["qc"][:, :, :U].transpose(0, 1).contiguous(),
+            F["qc"][:, :, U:].transpose(0, 1).contiguous())
+
+
+class _NMTDecoderFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, cfg, n_in, emb, att0, keys, values, pad, *rest):
+        L = cfg["L"]
+        h0, c0 = rest[:L], rest[L:2 * L]
+        W = dict(w_ih=rest[2 * L:3 * L], w_hh=rest[3 * L:4 * L], b_ih=rest[4 * L:5 * L],
+                 b_hh=rest[5 * L:6 * L], w_q=rest[6 * L], w_a=rest[6 * L + 4])
+        attn = dict(w_q=rest[6 * L], g=rest[6 * L + 1], v=rest[6 * L + 2], b=rest[6 * L + 3])
+        masks = None if rest[6 * L + 5] is None else rest[6 * L + 5:6 * L + 5 + L]
+        F = _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, True)
+        ctx.cfg, ctx.n_in = cfg, n_in
+        ctx.F = F
+        ctx.save_for_backward(emb, att0, keys, values, pad, *rest)
+        ctx.set_materialize_grads(False)
+        return _nmt_outputs(cfg, F, emb.shape[2], cfg["output_attention"])
+
+    @staticmethod
+    def backward(ctx, *douts):
+        cfg, F = ctx.cfg, ctx.F
+        Lb = _lib()
+        emb, att0, keys, values, pad, *rest = ctx.saved_tensors
+        L, std, bah, res = cfg["L"], cfg["standard"], cfg["bahdanau"], cfg["residual"]
+        w_ih, w_hh, b_ih, b_hh = rest[2 * L:3 * L], rest[3 * L:4 * L], rest[4 * L:5 * L], \
+            rest[5 * L:6 * L]
+        w_q, g, vp, bb, w_a = rest[6 * L:6 * L + 5]
+        masks = None if rest[6 * L + 5] is None else rest[6 * L + 5:6 * L + 5 + L]
+        B, T, U = emb.shape
+        S, M = keys.shape[1], values.shape[2]
+        A = att0.shape[1]
+        dt, dev = emb.dtype, emb.device
+        xh, C, P, qc, align, pq, gx0, w_step = (F[k] for k in ("xh", "C", "P", "qc", "align",
+                                                                "pq", "gx0", "w_step"))
+        I = [U + A] + [U] * (L - 1)
+        K = [I[0] + U] + [I[l] + U for l in range(1, L)]
+        m0 = None if masks is None else masks[0]
+
+        def _prep(d):
+            if d is None:
+                return None
+            d = d.contiguous()
+            return d if d.data_ptr() % 16 == 0 else d.clone()
+        if std:
+            d_main, d_ctx_out = _prep(douts[0]), None
+        else:
+            d_main, d_ctx_out = _prep(douts[0]), _prep(douts[1])
+        f32 = dict(dtype=torch.float32, device=dev)
+        dG = [torch.empty(T, B, 4 * U, dtype=dt, device=dev) for _ in range(L)]
+        dXH = [torch.empty(B, K[l] - (U if l == 0 else 0), **f32) for l in range(L)]
+        dc = [torch.zeros(B, U, **f32) for _ in range(L)]
+        dY = [torch.empty(B, U, **f32) for _ in range(L)]
+        dY0 = torch.empty(T, B, U, **f32) if res[0] else None
+        dkeys = torch.zeros(B, S, U, **f32)
+        dvalues = torch.zeros(B, S, M, **f32)
+        part_g = torch.zeros(B, 1, **f32) if (not bah and g is not None) else None
+        part_v = torch.zeros(B, U, **f32) if bah else None
+        part_b = torch.zeros(B, U, **f32) if (bah and bb is not None) else None
+        dq = torch.empty(B, U, **f32)
+        dpq = torch.empty(T, B, U, dtype=dt, device=dev) if bah else None
+        datt = torch.empty(T, B, U, dtype=dt, device=dev) if std else None
+        dqc = torch.empty(B, U + M, **f32) if std else None
+        g_p = _p(g) if g is not None else None
+        kind = 1 if bah else 0
+        st = _stream()
+        for t in range(T - 1, -1, -1):
+            last = t == T - 1
+            if std:
+                # d att_t = d_out_t (output_attention) + the feed's gradient from step t+1
+                dst = datt[t]
+                d_o = d_main[:, t] if (cfg["output_attention"] and d_main is not None) else None
+                if last:
+                    if d_o is None:
+                        dst.zero_()
+                    else:
+                        dst.copy_(d_o)
+                else:
+                    dF = dXH[0][:, :A]
+                    mf = None if m0 is None else m0[t + 1, :, U:]
+                    if d_o is None:
+                        dst.copy_(dF if mf is None else dF * mf)
+                    elif mf is None:
+                        torch.add(d_o, dF, out=dst)
+                    else:
+                        torch.addcmul(d_o, dF, mf, out=dst)
+                _mm_f32(datt[t], w_a, dqc)
+                dA, dA_ld, dAm, dAm_ld = _addr(dqc, U), U + M, None, 0
+                dO, dO_ld = None, 0
+            else:
+                dA, dA_ld, dAm, dAm_ld = (None, 0, None, 0) if last else \
+                    (_p(dXH[0]), K[0] - U, None if m0 is None else _addr(m0[t + 1], U), I[0])
+                dO, dO_ld = (None, 0) if d_ctx_out is None else (_addr(d_ctx_out, t * M), T * M)
+            _check(Lb.px_nmt_attn_bwd(
+                dA, dA_ld, dAm, dAm_ld, dO, dO_ld, _p(align[t]), _p(qc[t]), U + M,
+                _p(pq[t]) if bah else None, _p(keys), _p(values), g_p,
+                _p(vp) if bah else None, _p(bb) if bb is not None else None,
+                None if bah else _p(dq), _p(dpq[t]) if bah else None, _p(dkeys), _p(dvalues),
+                _p(part_g) if part_g is not None else None,
+                _p(part_v) if bah else None, _p(part_b) if part_b is not None else None,
+                B, S, U, M, kind, _DT[dt], st), "nmt_attn_bwd")
+            if bah:
+                _mm_f32(dpq[t], w_q, dq)
+            for l in range(L - 1, -1, -1):
+                top = l == L - 1
+                if top:
+                    a_, a_ld, am, am_ld = (_p(dqc), U + M, None, 0) if std else (None, 0, None, 0)
+                    dR = _p(dq)
+                    if std:
+                        o_ = None if (cfg["output_attention"] or d_main is None) else \
+                            _addr(d_main, t * U)
+                    else:
+                        o_ = None if d_main is None else _addr(d_main, t * U)
+                    o_ld = T * U
+                else:
+                    a_, a_ld = _p(dXH[l + 1]), K[l + 1]
+                    am, am_ld = (None, 0) if masks is None else (_p(masks[l + 1][t]), I[l + 1])
+                    dR = _p(dY[l + 1]) if res[l + 1] else None
+                    o_, o_ld = None, 0
+                off = A if l == 0 else I[l]
+                drec, drec_ld = (None, 0) if last else (_addr(dXH[l], off), dXH[l].shape[1])
+                dYp = _p(dY0[t]) if (l == 0 and res[0]) else (_p(dY[l]) if l > 0 and res[l]
+                                                              else None)
+                _check(Lb.px_nmt_lstm_cell_bwd(
+                    _p(P[l][t]), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]),
+                    _p(C[l][t]), _p(C[l][t + 1]), a_, a_ld, am, am_ld, dR, o_, o_ld, drec,
+                    drec_ld, _p(dc[l]), _p(dG[l][t]), dYp, B, U, _DT[dt], st),
+                    "nmt_lstm_cell_bwd")
+                _mm_f32(dG[l][t], w_step[l], dXH[l])
+        _count(T * (L + 1))
+        nd = ctx.needs_input_grad
+        # gradients of the inputs: (cfg, n_in, emb, att0, keys, values, pad, *rest)
+        dG2 = [d.view(T * B, 4 * U) for d in dG]
+        gl = [None] * len(rest)
+        demb = None
+        if nd[2]:
+            de = torch.empty(T * B, U, **f32)
+            _mm_f32(dG2[0], w_ih[0][:, :U], de)
+            de = de.view(T, B, U)
+            if m0 is not None:
+                de = de * m0[:, :, :U]
+            if dY0 is not None:
+                de = de + dY0
+            demb = de.transpose(0, 1).to(dt)
+        datt0 = None
+        if nd[3]:
+            d = dXH[0][:, :A]
+            datt0 = (d if m0 is None else d * m0[0, :, U:]).to(dt)
+        dk = dkeys.to(dt) if nd[4] else None
+        dv = dvalues.to(dt) if nd[5] else None
+        for l in range(L):
+            off = A if l == 0 else I[l]
+            gl[l] = dXH[l][:, off:].to(dt)                         # h0
+            gl[L + l] = dc[l].to(rest[L + l].dtype)                # c0
+            if l == 0:
+                gl[2 * L] = torch.mm(dG2[0].t(), xh[0][:T, :, :U + A].reshape(T * B, U + A))
+            else:
+                gl[2 * L + l] = torch.mm(dG2[l].t(), xh[l][:T, :, :I[l]].reshape(T * B, I[l]))
+            gl[3 * L + l] = torch.mm(dG2[l].t(), xh[l][:T, :, I[l]:].reshape(T * B, U))
+            db = torch.sum(dG2[l], 0, dtype=torch.float32)
+            gl[4 * L + l] = db.to(rest[4 * L + l].dtype)
+            gl[5 * L + l] = db.to(rest[5 * L + l].dtype)
+        qrows = qc[:, :, :U].reshape(T * B, U)
+        if bah:
+            gl[6 * L] = torch.mm(dpq.view(T * B, U).t(), qrows)
+            out = torch.empty(U, **f32)
+            _check(Lb.px_nmt_attn_param_grad(_p(part_v), B, U, _p(out), st), "nmt_attn_param_grad")
+            gl[6 * L + 2] = out.to(vp.dtype)
+            if part_b is not None:
+                out = torch.empty(U, **f32)
+                _check(Lb.px_nmt_attn_param_grad(_p(part_b), B, U, _p(out), st),
+                       "nmt_attn_param_grad")
+                gl[6 * L + 3] = out.to(bb.dtype)
+        elif part_g is not None:
+            out = torch.empty(1, **f32)
+            _check(Lb.px_nmt_attn_param_grad(_p(part_g), B, 1, _p(out), st), "nmt_attn_param_grad")
+            gl[6 * L + 1] = out.view(()).to(g.dtype)
+        if std:
+            gl[6 * L + 4] = torch.mm(datt.view(T * B, U).t(), qc.view(T * B, U + M))
+        ctx.F = None
+        return (None, None, demb, datt0, dk, dv, None, *gl)
+
+
+def _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks):
+    L = len(w_ih)
+    return (list(h0) + list(c0) + list(w_ih) + list(w_hh) + list(b_ih) + list(b_hh) +
+            [w_q, g, v, b, w_a] + (list(masks) if masks is not None else [None] * L))
+
+
+def _nmt_cfg(L, residual, v, w_a, output_attention):
+    return {"L": L, "standard": w_a is not None, "bahdanau": v is not None,
+            "residual": tuple(bool(r) for r in residual),
+            "output_attention": bool(output_attention)}
+
+
+def nmt_attention_decoder(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh, residual,
+                          w_q=None, g=None, v=None, b=None, w_a=None, masks=None,
+                          output_attention=True):
+    """All T steps of the NMT attention decoder's recurrence as ONE autograd node
+    (`kernels/nmt_decoder.cu`).
+
+    emb [B, T, U] (the decoder inputs), h0/c0 (per layer [B, U]), att0 [B, A] (the fed-back
+    attention state), keys [B, S, U], values [B, S, M], pad [B, S] bool (True past each source
+    length); per layer w_ih [4U, I_l], w_hh [4U, U], b_ih, b_hh (torch.nn.LSTM, gates i, f, g,
+    o) and `residual` flags.  The attention: luong (`g`: scaled_luong's scale or None) or, with
+    `v` = v′ (g·v/‖v‖ for normed_bahdanau, else v) and `w_q`, bahdanau (`b`: normed's bias).
+    With `w_a` the architecture is *standard*: the L layers feed att_t = W_a·[q_t, ctx_t] back
+    and the output is att_t or q_t (`output_attention`) -> [B, T, U].  Without it, *gnmt*: the
+    layers (the bottom layer only) feed ctx_t back -> (h [B, T, U], ctx [B, T, M]).
+
+    `masks` (per layer [T, B, I_l] in emb's dtype, or None) multiply each layer's input: the
+    caller draws dropout there, from the same distribution as `F.dropout` but not from its
+    random stream.  Callers check `nmt_decoder_applies` first.  Without autograd nothing is
+    kept for a backward pass; the node never synchronises with the host."""
+    L = len(w_ih)
+    cfg = _nmt_cfg(L, residual, v, w_a, output_attention)
+    emb, att0 = emb.contiguous(), att0.contiguous()
+    pad = pad.to(torch.bool).contiguous()
+    if masks is not None:
+        masks = [m.contiguous() for m in masks]
+    args = _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks)
+    ins = [emb, att0, keys, values] + args
+    if torch.is_grad_enabled() and any(a is not None and a.requires_grad for a in ins):
+        return _NMTDecoderFn.apply(cfg, len(args), emb, att0, keys, values, pad, *args)
+    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a)
+    attn = dict(w_q=w_q, g=g, v=v, b=b)
+    F = _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, False)
+    return _nmt_outputs(cfg, F, emb.shape[2], output_attention)
+
+
+@torch.no_grad()
+def nmt_attention_decoder_step(emb_t, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh,
+                               residual, w_q=None, g=None, v=None, b=None, w_a=None, masks=None):
+    """One decoding step (T = 1, nothing saved) of `nmt_attention_decoder` from emb_t [B, U] ->
+    (q [B, U] the top layer's output, att [B, A] the new fed-back state: W_a·[q, ctx] for
+    standard, ctx for gnmt, h per layer, c per layer in c0's dtype)."""
+    L = len(w_ih)
+    cfg = _nmt_cfg(L, residual, v, w_a, True)
+    U = emb_t.shape[1]
+    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a)
+    attn = dict(w_q=w_q, g=g, v=v, b=b)
+    F = _nmt_forward(cfg, emb_t[:, None, :].contiguous(), h0, c0, att0, keys, values,
+                     pad.to(torch.bool).contiguous(), W, attn, masks, False)
+    last = F["last"]
+    I = [U + att0.shape[1]] + [U] * (L - 1)
+    hs = [F["xh"][l][last, :, I[l]:].clone() for l in range(L)]
+    cs = [F["C"][l][last].to(c0[l].dtype) for l in range(L)]
+    q = F["qc"][0, :, :U]
+    att = F["att"][0] if w_a is not None else F["qc"][0, :, U:]
+    return q, att, hs, cs
 
 
 # ===========================================================================
