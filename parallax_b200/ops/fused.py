@@ -236,10 +236,11 @@ class _LSTMLayerFn(torch.autograd.Function):
         # dh_{t-1} = dH_{t-1} + dgates_t @ Wh^T : Wh [P, 4S] is already the
         # K-contiguous "B^T" operand, so this skinny product (M=B, N=P, K=4S)
         # goes to our wgmma split-K kernel with the +dH addend fused in, its 8 K-splits
-        # per tile reducing through DSMEM in a cluster.
+        # per tile reducing through DSMEM in a cluster.  The reduction reads the addend 4 bf16 at
+        # a time, so dH must be 8-byte aligned (an incoming gradient may be a view at any offset).
         from . import gemm as _gemm
         use_tc = (dt == torch.bfloat16 and Bsz % 128 == 0 and P % 64 == 0 and
-                  (4 * S) % 1024 == 0 and Wh.is_contiguous())
+                  (4 * S) % 1024 == 0 and Wh.is_contiguous() and dH.data_ptr() % 8 == 0)
         WhT = None if use_tc else Wh.t().contiguous()
         st = _stream()
 

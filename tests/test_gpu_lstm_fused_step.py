@@ -120,12 +120,16 @@ def _small_inputs(T, Bsz, E, S_, P_):
 ])
 def test_layer_fused_and_fallback_shapes(monkeypatch, Bsz, E, S_, P_, fused_bwd):
     """The stacked layer (T 3) against fp64 on both sides of the fused path's conditions, with
-    the layer's own input width patched into the numerics module's helpers."""
+    the layer's own input width patched into the numerics module's helpers.  Both persistent
+    kernels are switched off, so the per-step kernels run even where the persistent ones would
+    take the layer ((128, 256, 64) is in `test_gpu_lstm_persistent_shapes`)."""
     import tests.test_gpu_lm1b_numerics as N
     from parallax_b200.ops import fused
     WP = torch.empty(S_, P_, dtype=BF, device="cuda")
     assert fused._fused_bwd_ok(BF, Bsz, S_, P_, WP) == fused_bwd
     monkeypatch.setattr(N, "E_", E)
+    monkeypatch.setattr(fused, "_fwd_persistent_ok", lambda *a: False)
+    monkeypatch.setattr(fused, "_bwd_persistent_ok", lambda *a: False)
     inp = _small_inputs(3, Bsz, E, S_, P_)
     ref = _run_layer("reference", inp, torch.float64)
     low = _run_layer("reference", inp, BF)
