@@ -116,6 +116,10 @@ SAMPLE_RADIX_BITS = 4
 # ["full_softmax_train"] = "fused"): the gathered rows and the bf16 [N, Vc] softmax gradient of
 # one vocabulary chunk of Vc rows
 FULL_SOFTMAX_TRAIN_WS_BYTES = 256 << 20
+# bound on the chunk scratch of the fused dense linear cross-entropy (`nn.linear_cross_entropy`):
+# the fp32 logits and the bf16 softmax gradient of one chunk of rows, [n, V] each; a chunk never
+# has fewer than 128 rows, so a vocabulary above ~350k rows may exceed it
+LINEAR_XENT_WS_BYTES = 256 << 20
 
 RUN_OPTIONS = ("PS", "MPI", "HYBRID")
 # "AR" is accepted as a modern alias of the reference's "MPI" run option.

@@ -600,16 +600,21 @@ class Seq2Seq(nn.Module):
 
     def forward(self, source, target_input, target_output, source_sequence_length,
                 target_sequence_length):
-        logits = self.logits(source, target_input, source_sequence_length)
-        B, T, V = logits.shape
-        xent = F.cross_entropy(logits.reshape(B * T, V), target_output.reshape(-1),
-                               reduction="none").view(B, T)
-        tl = target_sequence_length.to(xent.device)
-        mask = (torch.arange(T, device=xent.device)[None, :] < tl[:, None]).to(xent.dtype)
-        loss = (xent * mask).sum() / B
-        return {"loss": loss, "predict_count": tl.sum(),
+        """Training loss: the masked cross entropy of the output layer summed over the batch
+        and divided by B, through `parallax.nn.linear_cross_entropy` (fused where it applies,
+        so no [B·T, V] logits are kept)."""
+        memory, state = self.encode(source, source_sequence_length)
+        emb = self._embed(self.embedding_decoder, target_input)
+        out = self.decoder(emb, state, memory)
+        B, T, U = out.shape
+        tl = target_sequence_length.to(out.device)
+        mask = (torch.arange(T, device=out.device)[None, :] < tl[:, None]).to(torch.float32)
+        loss, _ = pnn.linear_cross_entropy(out.reshape(B * T, U), target_output.reshape(-1),
+                                           self.output_layer.weight, None,
+                                           row_weights=mask.reshape(-1))
+        return {"loss": loss / B, "predict_count": tl.sum(),
                 "word_count": tl.sum() + source_sequence_length.to(tl.device).sum(),
-                "batch_size": torch.tensor(B, device=xent.device)}
+                "batch_size": torch.tensor(B, device=out.device)}
 
 
 # --------------------------------------------------------- training "graph"

@@ -70,23 +70,30 @@ class SkipThoughtsModel(nn.Module):
 
     # -- decoders ------------------------------------------------------------------
     def _decode(self, gru, thought, ids, mask):
+        """The decoder GRU's outputs [B, T, encoder_dim] for target `ids`."""
         emb = self.word_embedding(ids).to(self.compute_dtype)
         inp = F.pad(emb[:, :-1, :], (0, 0, 1, 0))           # shift right, zero first step
-        mask = mask.to(emb.device)
-        out, _ = gru(inp, mask.sum(1), initial_state=thought)
-        logits = self.logits(out).float()
-        losses = F.cross_entropy(logits.view(-1, logits.shape[-1]), ids.reshape(-1),
-                                 reduction="none")
-        weights = mask.reshape(-1).to(losses.dtype)
-        return losses, weights
+        out, _ = gru(inp, mask.to(emb.device).sum(1), initial_state=thought)
+        return out
+
+    def _decoder_loss(self, gru, thought, ids, mask):
+        """(Σ masked cross entropy, Σ weights) of one decoder, through
+        `parallax.nn.linear_cross_entropy` with the shared logits layer (fused where it
+        applies, so no [B·T, vocab] logits are kept)."""
+        out = self._decode(gru, thought, ids, mask)
+        weights = mask.to(out.device).reshape(-1).to(torch.float32)
+        loss, _ = pnn.linear_cross_entropy(out.reshape(-1, out.shape[-1]), ids.reshape(-1),
+                                           self.logits.weight, self.logits.bias,
+                                           row_weights=weights)
+        return loss, weights
 
     def forward(self, encode_ids, encode_mask, decode_pre_ids, decode_pre_mask,
                 decode_post_ids, decode_post_mask):
         thought = self.encode(encode_ids, encode_mask)
-        l_pre, w_pre = self._decode(self.decoder_pre, thought, decode_pre_ids, decode_pre_mask)
-        l_post, w_post = self._decode(self.decoder_post, thought, decode_post_ids,
-                                      decode_post_mask)
-        pre, post = (l_pre * w_pre).sum(), (l_post * w_post).sum()
+        pre, w_pre = self._decoder_loss(self.decoder_pre, thought, decode_pre_ids,
+                                        decode_pre_mask)
+        post, w_post = self._decoder_loss(self.decoder_post, thought, decode_post_ids,
+                                          decode_post_mask)
         return {"loss": pre + post, "loss_pre": pre.detach(), "loss_post": post.detach(),
                 "sum_weights": (w_pre.sum() + w_post.sum()).detach(),
                 "thought_vectors": thought.detach()}

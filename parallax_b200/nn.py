@@ -259,6 +259,65 @@ def full_softmax_sample(inputs, weight, bias, num_samples=1, temperature=1.0, se
     return _fsm(inputs, weight, bias, num_samples, inv_tau, int(seed), top_k, top_p)
 
 
+def linear_cross_entropy(inputs, targets, weight, bias=None, row_weights=None):
+    """Cross entropy of a dense output layer, without the ``[N, V]`` logits: ``(loss, nll)``
+    with ``nll`` the per-row fp32 cross entropy (``reduction="none"``) of ::
+
+        cross_entropy(linear(inputs, weight, bias).float(), targets)
+
+    and ``loss`` the scalar ``Σ_i row_weights_i · nll_i`` (every weight 1 when `row_weights` is
+    None), which carries the gradient; ``nll`` is detached, for statistics.  `inputs` is
+    ``[N, K]``, `targets` ``[N]`` integer ids, `weight` ``[V, K]`` (an ``nn.Linear.weight``),
+    `bias` ``[V]`` or None, `row_weights` ``[N]`` real numbers (zeros and negatives allowed; they
+    are constants and get no gradient).
+
+    For CUDA tensors with bf16 inputs and weight, a bf16 or fp32 bias, K % 8 == 0 and
+    8 <= K <= 8192, and a contiguous 16-byte-aligned weight, fused kernels compute the fp32
+    logits a chunk of rows at a time with their log-sum-exp in the GEMM's epilogue
+    (`ops/csrc/kernels/linear_xent.cu`); the scratch stays within
+    `consts.LINEAR_XENT_WS_BYTES` (chunks of at least 128 rows).  When a gradient is wanted it is
+    formed in the forward, as a bf16 softmax gradient per chunk, and the backward scales it.
+    Everywhere else the composition above runs.  A target outside [0, V) gives NaN in its
+    ``nll`` row, and so in ``loss``, on either path.
+
+    `ValueError` for inputs that are not 2-D, a weight that is not ``[V, K]`` of the inputs'
+    dtype, targets that are not ``[N]`` integer ids, a bias that is not ``[V]``, row weights
+    that are not ``[N]`` real numbers, and tensors on different devices."""
+    if inputs.dim() != 2:
+        raise ValueError("inputs must be [N, K], got shape %s" % (tuple(inputs.shape),))
+    N, K = inputs.shape
+    if weight.dim() != 2 or weight.shape[1] != K:
+        raise ValueError("weight must be [V, %d], got shape %s" % (K, tuple(weight.shape)))
+    if not inputs.dtype.is_floating_point or weight.dtype != inputs.dtype:
+        raise ValueError("inputs and weight must share one floating dtype, got %s and %s"
+                         % (inputs.dtype, weight.dtype))
+    V = weight.shape[0]
+    if targets.dim() != 1 or targets.shape[0] != N:
+        raise ValueError("targets must be [N] = [%d], got shape %s" % (N, tuple(targets.shape)))
+    if targets.dtype.is_floating_point or targets.dtype.is_complex or targets.dtype == torch.bool:
+        raise ValueError("targets must be integer ids, got %s" % targets.dtype)
+    if bias is not None and (tuple(bias.shape) != (V,) or not bias.dtype.is_floating_point):
+        raise ValueError("bias must be a floating [%d] or None, got %s %s"
+                         % (V, tuple(bias.shape), bias.dtype))
+    if row_weights is not None and (tuple(row_weights.shape) != (N,) or
+                                    row_weights.dtype.is_complex or
+                                    row_weights.dtype == torch.bool):
+        raise ValueError("row_weights must be [N] = [%d] real numbers or None, got %s %s"
+                         % (N, tuple(row_weights.shape), row_weights.dtype))
+    devs = {t.device for t in (inputs, targets, weight, bias, row_weights) if t is not None}
+    if len(devs) > 1:
+        raise ValueError("all tensors must be on one device, got %s" % sorted(map(str, devs)))
+    from .ops import fused
+    if fused.linear_xent_applies(inputs, weight, bias):
+        loss, nll = fused.linear_cross_entropy(inputs, targets, weight,
+                                               None if bias is None else bias.contiguous(),
+                                               row_weights)
+    else:
+        loss, nll = fused.linear_cross_entropy_reference(inputs, targets, weight, bias,
+                                                         row_weights)
+    return loss, nll.detach()
+
+
 def _check_full_softmax(inputs, weight, bias):
     if weight.embedding_dim != inputs.shape[1]:
         raise ValueError("weight rows have %d columns, inputs have %d"

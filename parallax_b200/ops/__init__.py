@@ -135,6 +135,11 @@ _SIGS = {
                                      c_void_p, c_void_p, c_void_p, c_int,
                                      ctypes.POINTER(GroupGeom), c_void_p, c_int, c_int,
                                      c_void_p, c_void_p]),
+    "px_linear_xent_tile_cols": (c_int, []),
+    "px_linear_xent_logits": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                      c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "px_linear_xent_rows": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "px_clip_hp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "px_stamp": (c_int, [c_void_p, c_void_p]),
 }

@@ -24,10 +24,15 @@ oracle in the tests and the path used on the host fabric.
   layer and one attention kernel (`kernels/nmt_decoder.cu`) each way; every weight gradient is one
   GEMM over all steps.  Its oracle is `nmt_attention_decoder_reference`, which equals
   `Decoder._composition`.
+`linear_cross_entropy` — a dense output layer and its softmax cross entropy without the [N, V]
+  logits: per chunk of rows one wgmma logits kernel with a log-sum-exp epilogue and one row
+  kernel (`kernels/linear_xent.cu`), the gradient formed in the forward.  Its oracle is
+  `linear_cross_entropy_reference`.
 """
 import ctypes
 
 import torch
+import torch.nn.functional as F
 
 from . import lib as _lib, check as _check, register_signatures
 
@@ -1115,3 +1120,152 @@ def sampled_softmax_head(inputs, w_all, b_all, logq, targets, sampled, row_w=Non
     sm = sampled.to(torch.int64).contiguous()
     rw = None if row_w is None else row_w.detach().float().contiguous()
     return _SampledSoftmaxHeadFn.apply(inputs, w_all, b_all, adj, tg, sm, rw)
+
+
+# ===========================================================================
+# dense linear cross-entropy (output layer + softmax loss)
+# ===========================================================================
+_LX_K_MAX = 8192
+
+
+def linear_xent_applies(inputs, weight, bias):
+    """The fused kernels take the head: CUDA tensors, bf16 inputs and weight, a bias that is None
+    or bf16/fp32 [V], 8 <= K <= 8192 with K % 8 == 0 (the TMA row pitch is a multiple of 16
+    bytes), and a contiguous, 16-byte-aligned weight (it is read in place)."""
+    if not (inputs.is_cuda and weight.is_cuda and inputs.dtype == torch.bfloat16 and
+            weight.dtype == torch.bfloat16 and inputs.dim() == 2 and weight.dim() == 2):
+        return False
+    V, K = weight.shape
+    if bias is not None and not (bias.is_cuda and bias.dtype in (torch.bfloat16, torch.float32)
+                                 and tuple(bias.shape) == (V,)):
+        return False
+    return (K % 8 == 0 and 8 <= K <= _LX_K_MAX and V >= 1 and weight.is_contiguous() and
+            weight.data_ptr() % 16 == 0)
+
+
+def linear_xent_chunk_rows(N, V):
+    """Rows per chunk: the most whole 128-row tiles whose fp32 logits and bf16 softmax gradient
+    ([n, V] each, rows padded to 8 columns) fit `consts.LINEAR_XENT_WS_BYTES`, never fewer than
+    128, never more than N."""
+    from .. import consts
+    vp = (V + 7) // 8 * 8
+    return min(N, max(128, consts.LINEAR_XENT_WS_BYTES // (vp * 6) // 128 * 128))
+
+
+def linear_cross_entropy_reference(inputs, targets, weight, bias=None, row_weights=None):
+    """The composition: ``(cross_entropy(linear(x, W, b).float(), t, reduction="none") * w).sum()``
+    -> (loss, nll), with NaN in the nll of a target outside [0, V).  The oracle of the fused path
+    and the path taken wherever `linear_xent_applies` is false."""
+    if bias is not None and bias.dtype != inputs.dtype:
+        bias = bias.to(inputs.dtype)
+    V = weight.shape[0]
+    valid = (targets >= 0) & (targets < V)
+    nll = F.cross_entropy(F.linear(inputs, weight, bias).float(), targets.clamp(0, V - 1),
+                          reduction="none")
+    nll = torch.where(valid, nll, torch.full_like(nll, float("nan")))
+    if row_weights is None:
+        return nll.sum(), nll
+    return (nll * row_weights.detach().to(nll.dtype)).sum(), nll
+
+
+def _linear_xent(x, targets, weight, bias, row_w, want, chunk=None):
+    """Chunked fused forward -> (nll [N] fp32, dX, fp32 dW, fp32 db), each gradient of the
+    unscaled loss Σ w_i · nll_i or None as `want` (x, weight, bias) asks.  Per chunk of n rows:
+    the logits kernel, the rows kernel (writing the bf16 gradient G when anything is wanted),
+    then dX_c = G·W, dW += Gᵀ·X_c and db += Σ_rows G on cuBLAS."""
+    L = _lib()
+    N, K = x.shape
+    V = weight.shape[0]
+    dev = x.device
+    grad = any(want)
+    vp = (V + 7) // 8 * 8
+    n = min(N, int(chunk)) if chunk else linear_xent_chunk_rows(N, V)
+    nvt = (V + L.px_linear_xent_tile_cols() - 1) // L.px_linear_xent_tile_cols()
+    nll = torch.empty(N, dtype=torch.float32, device=dev)
+    dx = torch.empty(N, K, dtype=x.dtype, device=dev) if want[0] else None
+    dw = torch.zeros(V, K, dtype=torch.float32, device=dev) if want[1] and N == 0 else None
+    db = torch.zeros(1, V, dtype=torch.float32, device=dev) if want[2] and N == 0 else None
+    if N == 0:
+        return nll, dx, dw, db
+    S = torch.empty(n, vp, dtype=torch.float32, device=dev)
+    part = torch.empty(n, nvt, 2, dtype=torch.float32, device=dev)
+    tgt = torch.empty(n, dtype=torch.float32, device=dev)
+    G = torch.empty(n, vp, dtype=torch.bfloat16, device=dev) if grad else None
+    ones = torch.ones(1, n, dtype=torch.bfloat16, device=dev) if want[2] else None
+    kind = 0 if bias is None else (1 if bias.dtype == torch.bfloat16 else 2)
+    st = _stream()
+    for c0 in range(0, N, n):
+        m = min(n, N - c0)
+        _check(L.px_linear_xent_logits(_addr(x, c0 * K), m, K, _p(weight), V,
+                                       None if bias is None else _p(bias), kind,
+                                       _addr(targets, c0), _p(S), vp, _p(part), _p(tgt), st),
+               "linear_xent_logits")
+        _check(L.px_linear_xent_rows(_p(S), vp, _p(part), _p(tgt), _addr(targets, c0),
+                                     None if row_w is None else _addr(row_w, c0), _addr(nll, c0),
+                                     None if G is None else _p(G), m, V, st),
+               "linear_xent_rows")
+        _count(2)
+        if not grad:
+            continue
+        Gc = G[:m, :V]
+        if want[0]:
+            torch.mm(Gc, weight, out=dx[c0:c0 + m])
+        if want[1]:
+            if c0 == 0:
+                dw = torch.mm(Gc.t(), x[:m], out_dtype=torch.float32)
+            else:
+                torch.addmm(dw, Gc.t(), x[c0:c0 + m], out_dtype=torch.float32, out=dw)
+        if want[2]:
+            if c0 == 0:
+                db = torch.mm(ones[:, :m], Gc, out_dtype=torch.float32)
+            else:
+                torch.addmm(db, ones[:, :m], Gc, out_dtype=torch.float32, out=db)
+    return nll, dx, dw, db
+
+
+def _weighted_sum(nll, row_w):
+    return nll.sum() if row_w is None else (nll * row_w).sum()
+
+
+class _LinearXentFn(torch.autograd.Function):
+    """Forms the gradient of the loss during the forward (the row weights are known then), so
+    the backward only scales the saved dX, dW and db by the incoming scalar."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, targets, row_w, chunk):
+        want = tuple(bool(w) for w in ctx.needs_input_grad[:3])
+        nll, dx, dw, db = _linear_xent(x, targets, weight, bias, row_w, want, chunk)
+        ctx.grads = (dx, dw, db)
+        ctx.out_dtypes = (weight.dtype, None if bias is None else bias.dtype)
+        ctx.mark_non_differentiable(nll)
+        return _weighted_sum(nll, row_w), nll
+
+    @staticmethod
+    def backward(ctx, g, _):
+        dx, dw, db = ctx.grads
+        w_dt, b_dt = ctx.out_dtypes
+        g = g.float()
+        gx = None if dx is None else dx * g
+        gw = None if dw is None else torch.mul(dw, g, out=torch.empty(dw.shape, dtype=w_dt,
+                                                                      device=dw.device))
+        gb = None if db is None else (db.view(-1) * g).to(b_dt)
+        return gx, gw, gb, None, None, None
+
+
+def linear_cross_entropy(inputs, targets, weight, bias=None, row_weights=None, chunk=None):
+    """The fused head: (loss = Σ_i w_i · nll_i, nll [N] fp32) for bf16 inputs [N, K] against a
+    dense output layer `weight` [V, K] (+ `bias` [V]), without an [N, V] logits tensor beyond
+    one chunk of `chunk` rows (default `linear_xent_chunk_rows`).  Callers check
+    `linear_xent_applies` first.  With autograd the gradient is formed during the forward; without
+    it (no_grad, or nothing requiring a gradient) only the logits and rows kernels run."""
+    x = inputs.contiguous()
+    if x.data_ptr() % 16:
+        x = x.clone()
+    t = targets.to(device=x.device, dtype=torch.int64).contiguous()
+    rw = None if row_weights is None else \
+        row_weights.detach().to(device=x.device, dtype=torch.float32).contiguous()
+    if torch.is_grad_enabled() and any(a is not None and a.requires_grad
+                                       for a in (inputs, weight, bias)):
+        return _LinearXentFn.apply(x, weight, bias, t, rw, chunk)
+    nll = _linear_xent(x, t, weight, bias, rw, (False, False, False), chunk)[0]
+    return _weighted_sum(nll, rw), nll
