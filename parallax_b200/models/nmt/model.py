@@ -25,8 +25,10 @@ stacks (packed by length), and in the GNMT decoder every layer above the
 attention layer (those depend on the *contexts*, which the bottom layer
 produces for all steps first); only the layers that feed attention back into
 their own input run step by step.  The same modules serve the step API used by
-greedy/sampling/beam decoding (`inference.py`).  On the GPU, with LSTM cells, those step-by-step
-layers and the attention are one fused autograd node (`ops/fused.py: nmt_attention_decoder`).
+greedy/sampling/beam decoding (`inference.py`).  On the GPU, with lstm or layer_norm_lstm cells,
+those step-by-step layers and the attention are one fused autograd node (`ops/fused.py:
+nmt_attention_decoder`), and every other layer_norm_lstm layer call is one fused autograd node
+(`ops/fused.py: ln_lstm_layer`).
 """
 import math
 
@@ -48,7 +50,8 @@ UNIT_TYPES = ("lstm", "gru", "layer_norm_lstm")
 # --------------------------------------------------------------------- cells
 class LayerNormLSTM(nn.Module):
     """`tf.contrib.rnn.LayerNormBasicLSTMCell`: layer-normalised gate
-    pre-activations and cell state.  Python time loop (no cuDNN equivalent)."""
+    pre-activations and cell state.  On the GPU the whole layer is one fused autograd node
+    (`fused.ln_lstm_layer`); elsewhere a Python time loop (no cuDNN equivalent)."""
 
     def __init__(self, input_size, num_units, forget_bias=1.0):
         super().__init__()
@@ -65,6 +68,18 @@ class LayerNormLSTM(nn.Module):
         return h2, c2
 
     def forward(self, x, state, lengths=None):
+        """x [B, T, I], state (h, c) -> (outputs [B, T, U], (h_T, c_T)).  The fused node when
+        `fused.ln_lstm_applies` (CUDA, bf16/fp32, U % 8 == 0 and within the kernels' limit),
+        else `_composition`."""
+        h, c = state
+        if fused.ln_lstm_applies(x, self.kernel.weight, self.ln, self.ln_c, h, c):
+            return fused.ln_lstm_layer(x, self.kernel.weight, self.ln, self.ln_c, self.forget_bias,
+                                       h, c, lengths)
+        return self._composition(x, state, lengths)
+
+    def _composition(self, x, state, lengths=None):
+        """The layer as plain PyTorch ops, one time step at a time: the fallback of `forward`
+        and the oracle of the fused node."""
         h, c = state
         outs = []
         for t in range(x.shape[1]):
@@ -324,9 +339,18 @@ class Decoder(nn.Module):
         layers = self.layers if self.architecture == "standard" else self.layers[:1]
         rnn = [l.rnn for l in layers]
         a = self.attention
-        kw = dict(w_ih=[r.weight_ih_l0 for r in rnn], w_hh=[r.weight_hh_l0 for r in rnn],
-                  b_ih=[r.bias_ih_l0 for r in rnn], b_hh=[r.bias_hh_l0 for r in rnn],
-                  residual=[l.residual for l in layers])
+        if layers[0].unit_type == "layer_norm_lstm":
+            # the bias-free kernel over [input | h]: its two column blocks, and the LayerNorms
+            kw = dict(w_ih=[r.kernel.weight[:, :l.input_size] for l, r in zip(layers, rnn)],
+                      w_hh=[r.kernel.weight[:, l.input_size:] for l, r in zip(layers, rnn)],
+                      b_ih=None, b_hh=None, residual=[l.residual for l in layers],
+                      ln=[([n.weight for n in list(r.ln) + [r.ln_c]] +
+                           [n.bias for n in list(r.ln) + [r.ln_c]],
+                           [n.eps for n in list(r.ln) + [r.ln_c]], r.forget_bias) for r in rnn])
+        else:
+            kw = dict(w_ih=[r.weight_ih_l0 for r in rnn], w_hh=[r.weight_hh_l0 for r in rnn],
+                      b_ih=[r.bias_ih_l0 for r in rnn], b_hh=[r.bias_hh_l0 for r in rnn],
+                      residual=[l.residual for l in layers])
         extra = []
         if a.option in ("bahdanau", "normed_bahdanau"):
             kw["w_q"] = a.query_layer.weight
@@ -345,19 +369,24 @@ class Decoder(nn.Module):
 
     def _node(self, emb, state, memory):
         """`node_arguments` when the fused node takes this decoder, else None (no attention,
-        other cells, CPU, fp64, shapes outside the kernels' limits)."""
+        GRU cells, CPU, fp64, shapes outside the kernels' limits)."""
         if self.architecture == "none":
             return None
         layers = self.layers if self.architecture == "standard" else self.layers[:1]
-        if any(l.unit_type != "lstm" for l in layers) or not emb.is_cuda:
+        unit = layers[0].unit_type
+        if unit not in ("lstm", "layer_norm_lstm") or any(l.unit_type != unit for l in layers) \
+                or not emb.is_cuda:
             return None
         layers, kw, extra = self.node_arguments()
         keys, values, _ = memory
         cells = state["cells"][:len(layers)]
-        weights = kw["w_ih"] + kw["w_hh"] + kw["b_ih"] + kw["b_hh"] + extra + \
-            [kw.get(k) for k in ("w_q", "g", "b", "w_a")]
+        if unit == "lstm":
+            weights = kw["w_ih"] + kw["w_hh"] + kw["b_ih"] + kw["b_hh"]
+        else:
+            weights = [l.rnn.kernel.weight for l in layers] + [p for x in kw["ln"] for p in x[0]]
+        weights = weights + extra + [kw.get(k) for k in ("w_q", "g", "b", "w_a")]
         states = [x for c in cells for x in c] + [state["attention"]]
-        if not fused.nmt_decoder_applies(emb, keys, values, weights, states, layers[0].unit_type):
+        if not fused.nmt_decoder_applies(emb, keys, values, weights, states, unit):
             return None
         return layers, kw
 
@@ -444,10 +473,11 @@ class Decoder(nn.Module):
     def forward(self, emb, state, memory):
         """emb [B,T,U] → outputs [B,T,U].
 
-        With LSTM cells on CUDA in bf16 or fp32 and shapes within the kernels' limits, the
-        attention recurrence is one fused autograd node (`fused.nmt_attention_decoder`); every
-        other case runs `_composition`.  With dropout the node's masks come from the same
-        distribution as the composition's but not from the same random stream."""
+        With lstm or layer_norm_lstm cells on CUDA in bf16 or fp32 and shapes within the
+        kernels' limits, the attention recurrence is one fused autograd node
+        (`fused.nmt_attention_decoder`); every other case runs `_composition`.  With dropout the
+        node's masks come from the same distribution as the composition's but not from the same
+        random stream."""
         node = self._node(emb, state, memory)
         if node is None:
             return self._composition(emb, state, memory)

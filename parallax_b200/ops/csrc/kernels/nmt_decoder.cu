@@ -4,7 +4,8 @@
 // Per time step and layer the node runs one cuBLAS product with an fp32 output (the gate
 // pre-activations of [x_t | h_{t-1}]) and `px_nmt_lstm_cell_fwd`; per step the attention is
 // `px_nmt_attn_fwd` (after the cuBLAS query projection for the Bahdanau kinds).  Backward mirrors
-// it with `px_nmt_lstm_cell_bwd` and `px_nmt_attn_bwd`.
+// it with `px_nmt_lstm_cell_bwd` and `px_nmt_attn_bwd`.  With layer-normalised LSTM cells the cell
+// kernels are `px_nmt_ln_lstm_cell_fwd` / `bwd`, built on the row code of `ln_lstm_cell.cuh`.
 //
 // Every kernel runs one CTA of NA_THREADS threads per batch row.  All math is fp32; what is
 // stored is bf16 or fp32 (the compute dtype) or fp32 where the backward pass consumes it.
@@ -16,12 +17,14 @@
 // `px_nmt_attn_param_grad`: no atomics anywhere.
 #include "common.cuh"
 #include "lstm_cell.cuh"   // lstm_cell_fwd_elem / lstm_cell_bwd_elem, sigmoidf_, tanhf_
+#include "ln_lstm_cell.cuh"   // ln_lstm_cell_fwd_row / ln_lstm_cell_bwd_row
 
 #define NA_THREADS 256
 #define NA_WARPS (NA_THREADS / 32)
 #define NA_MAX_U 1024   // units (keys and query width)
 #define NA_MAX_M 2048   // memory width (values and context)
 #define NA_MAX_S 1024   // source positions
+static_assert(NA_THREADS == LN_ROW_THREADS, "the LN-LSTM cell kernels run the shared row code");
 
 namespace {
 
@@ -413,6 +416,91 @@ px_nmt_lstm_cell_bwd_kernel(const float* __restrict__ P, const float* __restrict
   }
 }
 
+// Layer-normalised LSTM cell (`LayerNormLSTM.cell`, gates i, j, f, o; ln_lstm_cell.cuh) of one
+// step for row blockIdx.x: pre = P + gx (nullable), both fp32 [B, 4U].  Writes c' (fp32, the
+// carried state), h, y and xn exactly as px_nmt_lstm_cell_fwd_kernel does, and, when `stats` is
+// set, the row's LL_NSTAT LayerNorm statistics.
+template <typename T>
+__global__ void __launch_bounds__(NA_THREADS)
+px_nmt_ln_lstm_cell_fwd_kernel(const float* __restrict__ P, const float* __restrict__ gx,
+                               const float* __restrict__ c_prev, float* __restrict__ c_new,
+                               T* __restrict__ h_out, int h_ld, const T* __restrict__ resid,
+                               int resid_ld, T* __restrict__ y, int y_ld,
+                               const T* __restrict__ mask, int mask_ld, T* __restrict__ xn,
+                               int xn_ld, float* __restrict__ stats, LnLstmParams<T> p, int U) {
+  __shared__ float s_red[4 * NA_WARPS];
+  const int b = blockIdx.x, j = threadIdx.x * 8;
+  float hv[8], c2[8], st[LL_NSTAT];
+  ln_lstm_cell_fwd_row<T>(P + (size_t)b * 4 * U, gx != nullptr ? gx + (size_t)b * 4 * U : nullptr,
+                          c_prev + (size_t)b * U, p, U, s_red, hv, c2, st);
+  if (stats != nullptr && threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < LL_NSTAT; ++k) stats[(size_t)b * LL_NSTAT + k] = st[k];
+  }
+  if (j >= U) return;
+  st8(c_new + (size_t)b * U + j, c2);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int u = j + i;
+    const T h = from_f<T>(hv[i]);
+    h_out[(size_t)b * h_ld + u] = h;
+    float yv = to_f<T>(h);
+    if (resid != nullptr) yv = round_t<T>(yv + to_f<T>(resid[(size_t)b * resid_ld + u]));
+    y[(size_t)b * y_ld + u] = from_f<T>(yv);
+    if (xn != nullptr)
+      xn[(size_t)b * xn_ld + u] =
+          from_f<T>(mask != nullptr ? yv * to_f<T>(mask[(size_t)b * mask_ld + u]) : yv);
+  }
+}
+
+// Backward of the cell above for row blockIdx.x, with the layer-output gradient dy, dY, drec and
+// the in-place fp32 carry dc as in px_nmt_lstm_cell_bwd_kernel.  Recomputes the cell from P, gx
+// and the saved statistics, writes the pre-LayerNorm gate gradients dG (T, [B, 4U], gate order
+// i, j, f, o) and adds the row's dy·x̂ and dy of the five LayerNorms to acc[b] = [Σ dy·x̂ (5U) |
+// Σ dy (5U)] (set instead of added when `first`).
+template <typename T>
+__global__ void __launch_bounds__(NA_THREADS)
+px_nmt_ln_lstm_cell_bwd_kernel(const float* __restrict__ P, const float* __restrict__ gx,
+                               const float* __restrict__ stats, const float* __restrict__ c_prev,
+                               const float* __restrict__ dA, int dA_ld,
+                               const T* __restrict__ dA_mask, int dA_mask_ld,
+                               const float* __restrict__ dR, const T* __restrict__ dO, int dO_ld,
+                               const float* __restrict__ drec, int drec_ld,
+                               float* __restrict__ dc, T* __restrict__ dG, float* __restrict__ dY,
+                               float* __restrict__ acc, int first, LnLstmParams<T> p, int U) {
+  __shared__ float s_red[8 * NA_WARPS];
+  const int b = blockIdx.x, j = threadIdx.x * 8;
+  const bool on = j < U;
+  float st[LL_NSTAT];
+#pragma unroll
+  for (int k = 0; k < LL_NSTAT; ++k) st[k] = stats[(size_t)b * LL_NSTAT + k];
+  float dh[8], dcv[8];
+  if (on) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int u = j + i;
+      float dy = 0.f;
+      if (dA != nullptr)
+        dy = dA[(size_t)b * dA_ld + u] *
+             (dA_mask != nullptr ? to_f<T>(dA_mask[(size_t)b * dA_mask_ld + u]) : 1.f);
+      if (dR != nullptr) dy += dR[(size_t)b * U + u];
+      if (dO != nullptr) dy += to_f<T>(dO[(size_t)b * dO_ld + u]);
+      if (dY != nullptr) dY[(size_t)b * U + u] = dy;
+      dh[i] = dy + (drec != nullptr ? drec[(size_t)b * drec_ld + u] : 0.f);
+    }
+    ld8(dc + (size_t)b * U + j, dcv);
+  }
+  float dp[4][8], dcp[8];
+  ln_lstm_cell_bwd_row<T>(P + (size_t)b * 4 * U, gx != nullptr ? gx + (size_t)b * 4 * U : nullptr,
+                          st, c_prev + (size_t)b * U, p, U, dh, dcv, s_red, dp, dcp,
+                          acc + (size_t)b * 10 * U, first);
+  if (!on) return;
+  st8(dc + (size_t)b * U + j, dcp);
+  T* o = dG + (size_t)b * 4 * U + j;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) st8(o + k * U, dp[k]);
+}
+
 // Vector loads need U and M in whole 16-byte vectors and 4-column groups, and every row start
 // (row strides included) on a 16-byte boundary.
 inline bool attn_shape_ok(int B, int S, int U, int M, int dtype) {
@@ -516,6 +604,39 @@ int px_nmt_lstm_cell_bwd(const float* P, const float* gx, const void* b_ih, cons
   px_nmt_lstm_cell_bwd_kernel<T><<<B, NA_THREADS, 0, stream>>>(                                 \
       P, gx, (const T*)b_ih, (const T*)b_hh, c_prev, c_new, dA, dA_ld, (const T*)dA_mask,       \
       dA_mask_ld, dR, (const T*)dO, dO_ld, drec, drec_ld, dc, (T*)dG, dY, U)
+  if (dtype == 0) NL_BWD(float); else NL_BWD(__nv_bfloat16);
+#undef NL_BWD
+  return (int)cudaGetLastError();
+}
+
+// ln: host array of 10 device pointers (γ of LN_i, LN_j, LN_f, LN_o, LN_c, then their β);
+// eps: host array of the 5 LayerNorms' eps.
+int px_nmt_ln_lstm_cell_fwd(const float* P, const float* gx, const float* c_prev, float* c_new,
+                            void* h_out, int h_ld, const void* resid, int resid_ld, void* y,
+                            int y_ld, const void* mask, int mask_ld, void* xn, int xn_ld,
+                            float* stats, const void* const* ln, const float* eps,
+                            float forget_bias, int B, int U, int dtype, cudaStream_t stream) {
+  if (B <= 0 || U <= 0 || U % 8 || U > LL_MAX_UNITS) return -2;
+#define NL_FWD(T)                                                                             \
+  px_nmt_ln_lstm_cell_fwd_kernel<T><<<B, NA_THREADS, 0, stream>>>(                            \
+      P, gx, c_prev, c_new, (T*)h_out, h_ld, (const T*)resid, resid_ld, (T*)y, y_ld,          \
+      (const T*)mask, mask_ld, (T*)xn, xn_ld, stats, ln_lstm_params<T>(ln, eps, forget_bias), U)
+  if (dtype == 0) NL_FWD(float); else NL_FWD(__nv_bfloat16);
+#undef NL_FWD
+  return (int)cudaGetLastError();
+}
+
+int px_nmt_ln_lstm_cell_bwd(const float* P, const float* gx, const float* stats,
+                            const float* c_prev, const float* dA, int dA_ld, const void* dA_mask,
+                            int dA_mask_ld, const float* dR, const void* dO, int dO_ld,
+                            const float* drec, int drec_ld, float* dc, void* dG, float* dY,
+                            float* acc, int first, const void* const* ln, const float* eps,
+                            float forget_bias, int B, int U, int dtype, cudaStream_t stream) {
+  if (B <= 0 || U <= 0 || U % 8 || U > LL_MAX_UNITS) return -2;
+#define NL_BWD(T)                                                                               \
+  px_nmt_ln_lstm_cell_bwd_kernel<T><<<B, NA_THREADS, 0, stream>>>(                              \
+      P, gx, stats, c_prev, dA, dA_ld, (const T*)dA_mask, dA_mask_ld, dR, (const T*)dO, dO_ld,  \
+      drec, drec_ld, dc, (T*)dG, dY, acc, first, ln_lstm_params<T>(ln, eps, forget_bias), U)
   if (dtype == 0) NL_BWD(float); else NL_BWD(__nv_bfloat16);
 #undef NL_BWD
   return (int)cudaGetLastError();

@@ -19,10 +19,16 @@ oracle in the tests and the path used on the host fabric.
   time step a cuBLAS product in fp32 and one cell kernel forward, one cell kernel and a cuBLAS
   product backward (`kernels/ln_gru.cu`); `w_hu`'s gradient is one GEMM over all steps.  Its
   oracle is the composition in `LayerNormGRU._composition`.
+`ln_lstm_layer` — the NMT layer-normalised LSTM layer as ONE autograd node: the input side as
+  one cuBLAS product before the loop, then per time step a cuBLAS product in fp32 and one cell
+  kernel forward, one cell kernel and a cuBLAS product backward (`kernels/ln_lstm.cu`); the
+  kernel weight's gradient and the input gradient are one GEMM each over all steps.  Its oracle
+  is `LayerNormLSTM._composition`.
 `nmt_attention_decoder` — the NMT decoder's attention recurrence (standard: every layer; gnmt:
   the bottom layer) as ONE autograd node: per time step a cuBLAS product and one cell kernel per
   layer and one attention kernel (`kernels/nmt_decoder.cu`) each way; every weight gradient is one
-  GEMM over all steps.  Its oracle is `nmt_attention_decoder_reference`, which equals
+  GEMM over all steps; with `ln` the cells are layer-normalised LSTMs (`LayerNormLSTM.cell`).
+  Its oracle is `nmt_attention_decoder_reference`, which equals
   `Decoder._composition`.
 `linear_cross_entropy` — a dense output layer and its softmax cross entropy without the [N, V]
   logits: per chunk of rows one wgmma logits kernel with a log-sum-exp epilogue and one row
@@ -56,6 +62,12 @@ register_signatures({
     "px_ln_gru_bwd": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp,
                            _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "px_ln_gru_param_grad": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp]),
+    "px_ln_lstm_max_units": (_i, []),
+    "px_ln_lstm_fwd": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _f,
+                            _vp, _i, _i, _i, _i, _vp]),
+    "px_ln_lstm_bwd": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp,
+                            _vp, _f, _vp, _i, _i, _i, _i, _vp]),
+    "px_ln_lstm_param_grad": (_i, [_vp, _i, _i, _vp, _i, _vp]),
     "px_nmt_max_units": (_i, []),
     "px_nmt_max_memory": (_i, []),
     "px_nmt_max_source": (_i, []),
@@ -68,6 +80,10 @@ register_signatures({
                                               _i, _i, _i, _vp]),
     "px_nmt_lstm_cell_bwd": (_i, [_vp] * 6 + [_vp, _i, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp,
                                               _vp, _i, _i, _i, _vp]),
+    "px_nmt_ln_lstm_cell_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp,
+                                     _i, _vp, _vp, _vp, _f, _i, _i, _i, _vp]),
+    "px_nmt_ln_lstm_cell_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _i,
+                                     _vp, _vp, _vp, _vp, _i, _vp, _vp, _f, _i, _i, _i, _vp]),
 })
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 
@@ -494,16 +510,171 @@ def ln_gru_layer(gx, cx, w_hu, ln_wh, ln_u, h0=None, lengths=None, reverse=False
 
 
 # ===========================================================================
+# layer-normalised LSTM layer (NMT)
+# ===========================================================================
+def _ln_lstm_params(ln_gates, ln_c):
+    """γ of LN_i, LN_j, LN_f, LN_o, LN_c, then their β"""
+    lns = list(ln_gates) + [ln_c]
+    return [ln.weight for ln in lns] + [ln.bias for ln in lns], [float(ln.eps) for ln in lns]
+
+
+def ln_lstm_applies(x, kernel_weight, ln_gates, ln_c, h0=None, c0=None):
+    """The fused node takes the layer: a CUDA tensor [B, T, I] in bf16 or fp32 with the kernel
+    weight [4U, I + U], the five LayerNorms' γ/β and any initial state in the same dtype, the
+    kernel weight contiguous and 16-byte aligned, U % 8 == 0 and U <= `px_ln_lstm_max_units()`
+    (2048: 8 units per thread, one 256-thread CTA per row)."""
+    dt = x.dtype
+    if not (x.is_cuda and x.dim() == 3 and dt in _DT and kernel_weight.dtype == dt):
+        return False
+    params, _ = _ln_lstm_params(ln_gates, ln_c)
+    if any(p is None or p.dtype != dt or not p.is_contiguous() for p in params):
+        return False
+    if any(s is not None and s.dtype != dt for s in (h0, c0)):
+        return False
+    U = kernel_weight.shape[0] // 4
+    return (U % 8 == 0 and U <= _lib().px_ln_lstm_max_units() and
+            kernel_weight.shape == (4 * U, x.shape[2] + U) and kernel_weight.is_contiguous() and
+            kernel_weight.data_ptr() % 16 == 0)
+
+
+def _ln_lstm_ptrs(params, eps):
+    return (_vp * 10)(*[p.data_ptr() for p in params]), (_f * 5)(*eps)
+
+
+def _ln_lstm_forward(x, w, params, eps, fb, h0, c0, lengths, save):
+    """All T steps -> (out [B, T, U], h_T, c_T (fp32), hs, C, P, gx, stats).  gx [B, T, 4U] (fp32)
+    is x·W_xᵀ, hs [B, T, U] the state h before each step, C [T+1, B, U] (fp32) the cell states,
+    P [T, B, 4U] (fp32) each step's h·W_hᵀ and stats [T, B, 10] its LayerNorm statistics;
+    without `save`, hs, C and P are ping-pong / scratch buffers and stats is None."""
+    L = _lib()
+    B, T, I = x.shape
+    U = w.shape[0] // 4
+    dt, dev = x.dtype, x.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    gx = torch.empty(B, T, 4 * U, **f32)
+    _mm_f32(x.reshape(B * T, I), w[:, :I].t(), gx.view(B * T, 4 * U))
+    w_h = w[:, I:].t()
+    if save:
+        hs = torch.empty(B, T, U, dtype=dt, device=dev)
+        hT = torch.empty(B, U, dtype=dt, device=dev)
+        h_at = lambda s: (hs[:, s], T * U) if s < T else (hT, U)
+    else:
+        hs = torch.empty(2, B, U, dtype=dt, device=dev)
+        h_at = lambda s: (hs[s % 2], U)
+    C = torch.empty(T + 1 if save else 2, B, U, **f32)
+    h_at(0)[0].copy_(h0)
+    C[0].copy_(c0)
+    P = torch.empty(T if save else 1, B, 4 * U, **f32)
+    stats = torch.empty(T, B, 10, **f32) if save else None
+    out = torch.empty(B, T, U, dtype=dt, device=dev)
+    ln, ep = _ln_lstm_ptrs(params, eps)
+    lp = None if lengths is None else _p(lengths)
+    st = _stream()
+    for t in range(T):
+        (h, h_ld), (hn, hn_ld) = h_at(t), h_at(t + 1)
+        c_i, c_o = (t, t + 1) if save else (t % 2, (t + 1) % 2)
+        Pt = P[t] if save else P[0]
+        _mm_f32(h, w_h, Pt)
+        _check(L.px_ln_lstm_fwd(_p(Pt), _addr(gx, t * 4 * U), T * 4 * U, _p(C[c_i]), _p(C[c_o]),
+                                _p(h), h_ld, _p(hn), hn_ld, _addr(out, t * U), T * U,
+                                _p(stats[t]) if save else None, ln, ep, fb, lp, t, B, U, _DT[dt],
+                                st), "ln_lstm_fwd")
+    _count(T)
+    return out, h_at(T)[0], C[T if save else T % 2], hs, C, P, gx, stats
+
+
+class _LNLSTMLayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, h0, c0, lengths, eps, fb, *params):
+        out, hT, cT, hs, C, P, gx, stats = _ln_lstm_forward(x, w, params, eps, fb, h0, c0, lengths,
+                                                            True)
+        ctx.save_for_backward(x, w, hs, C, P, gx, stats, lengths, *params)
+        ctx.eps, ctx.fb = eps, fb
+        ctx.set_materialize_grads(False)
+        return out, hT, cT.to(x.dtype, copy=True)
+
+    @staticmethod
+    def backward(ctx, d_out, d_hT, d_cT):
+        L = _lib()
+        x, w, hs, C, P, gx, stats, lengths, *params = ctx.saved_tensors
+        B, T, I = x.shape
+        U = w.shape[0] // 4
+        dt, dev = x.dtype, x.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        if d_out is not None:
+            d_out = d_out.contiguous()
+            if d_out.data_ptr() % 16:
+                d_out = d_out.clone()
+        carry_h, carry_c = (torch.zeros(B, U, **f32) if d is None else
+                            torch.empty(B, U, **f32).copy_(d) for d in (d_hT, d_cT))
+        drec = torch.empty(B, U, **f32)
+        dpre = torch.empty(B, T, 4 * U, dtype=dt, device=dev)
+        acc = torch.empty(B, 10 * U, **f32)
+        ln, ep = _ln_lstm_ptrs(params, ctx.eps)
+        lp = None if lengths is None else _p(lengths)
+        need_h0 = ctx.needs_input_grad[2]
+        w_h = w[:, I:]
+        st = _stream()
+        for k in range(T):
+            t = T - 1 - k
+            _check(L.px_ln_lstm_bwd(_p(P[t]), _addr(gx, t * 4 * U), T * 4 * U, _p(stats[t]),
+                                    _p(C[t]), None if d_out is None else _addr(d_out, t * U),
+                                    T * U, None if k == 0 else _p(drec), _p(carry_h),
+                                    _p(carry_c), _addr(dpre, t * 4 * U), T * 4 * U, _p(acc),
+                                    int(k == 0), ln, ep, ctx.fb, lp, t, B, U, _DT[dt], st),
+                   "ln_lstm_bwd")
+            if t > 0 or need_h0:
+                _mm_f32(dpre[:, t], w_h, drec)
+        dh0 = drec.add_(carry_h).to(dt) if need_h0 else None
+        dc0 = carry_c.to(dt) if ctx.needs_input_grad[3] else None
+        d2 = dpre.view(B * T, 4 * U)
+        dx = torch.mm(d2, w[:, :I]).view(B, T, I) if ctx.needs_input_grad[0] else None
+        dw = torch.cat([torch.mm(d2.t(), x.reshape(B * T, I)),
+                        torch.mm(d2.t(), hs.view(B * T, U))], 1)
+        dln = torch.empty(10, U, dtype=dt, device=dev)
+        _check(L.px_ln_lstm_param_grad(_p(acc), B, U, _p(dln), _DT[dt], st), "ln_lstm_param_grad")
+        _count(T + 1)
+        return (dx, dw, dh0, dc0, None, None, None, *dln.unbind(0))
+
+
+def ln_lstm_layer(x, kernel_weight, ln_gates, ln_c, forget_bias, h0, c0, lengths=None):
+    """`LayerNormLSTM` over x [B, T, I] -> (outputs [B, T, U], zero past each length; (h_T, c_T)
+    in x's dtype).  kernel_weight [4U, I + U] is the bias-free `nn.Linear` over [x | h] (gate
+    order i, j, f, o), ln_gates the gates' four `nn.LayerNorm(U)`, ln_c the cell state's; c' is
+    carried un-normalised, in fp32 between steps.  `lengths` [B] freezes each row's state past
+    its length.  Callers check `ln_lstm_applies` first.  Without autograd (no_grad, or nothing
+    requiring a gradient) nothing is kept for a backward pass."""
+    B, T, _ = x.shape
+    U = kernel_weight.shape[0] // 4
+    if h0 is None:
+        h0 = x.new_zeros(B, U)
+    if c0 is None:
+        c0 = x.new_zeros(B, U)
+    if lengths is not None:
+        lengths = lengths.to(device=x.device, dtype=torch.int64).contiguous()
+    params, eps = _ln_lstm_params(ln_gates, ln_c)
+    fb = float(forget_bias)
+    args = [x, kernel_weight, h0, c0] + params
+    if torch.is_grad_enabled() and any(a.requires_grad for a in args):
+        out, hT, cT = _LNLSTMLayerFn.apply(x, kernel_weight, h0, c0, lengths, tuple(eps), fb,
+                                           *params)
+        return out, (hT, cT)
+    out, hT, cT, *_ = _ln_lstm_forward(x, kernel_weight, params, eps, fb, h0, c0, lengths, False)
+    return out, (hT.clone(), cT.to(x.dtype, copy=True))
+
+
+# ===========================================================================
 # NMT attention decoder
 # ===========================================================================
 def nmt_decoder_applies(emb, keys, values, weights, states, unit_type="lstm"):
-    """The fused node takes the decoder: LSTM cells, a CUDA tensor in bf16 or fp32 with every
-    weight and state in the same dtype, the matrices contiguous and 16-byte aligned, keys
+    """The fused node takes the decoder: LSTM or layer_norm_lstm cells, a CUDA tensor in bf16 or
+    fp32 with every weight and state in the same dtype, the matrices contiguous and 16-byte
+    aligned (for layer_norm_lstm, each layer's whole kernel weight), keys
     [B, S, U] and values [B, S, M] contiguous and 16-byte aligned, U % 8 == 0 and M % 8 == 0,
     and U, M and S within `px_nmt_max_units` / `px_nmt_max_memory` / `px_nmt_max_source`
     (1024 / 2048 / 1024)."""
     dt = emb.dtype
-    if unit_type != "lstm" or not (emb.is_cuda and dt in _DT):
+    if unit_type not in ("lstm", "layer_norm_lstm") or not (emb.is_cuda and dt in _DT):
         return False
     if any(t is not None and t.dtype != dt for t in list(weights) + list(states) + [keys, values]):
         return False
@@ -524,9 +695,22 @@ def _mask_mul(x, m):
     return x if m is None else x * m
 
 
+def _ln_cell_reference(gates, c, ln, dt):
+    """`LayerNormLSTM.cell` from its pre-LayerNorm gate terms, in the accumulation type"""
+    params, eps, fb = ln
+    U = c.shape[1]
+    F_ = torch.nn.functional
+    a = [F_.layer_norm(x, (U,), _acc(params[k]), _acc(params[5 + k]), eps[k])
+         for k, x in enumerate(gates.chunk(4, -1))]
+    c = c * torch.sigmoid(a[2] + fb) + torch.sigmoid(a[0]) * torch.tanh(a[1])
+    h = (torch.tanh(F_.layer_norm(c, (U,), _acc(params[4]), _acc(params[9]), eps[4])) *
+         torch.sigmoid(a[3])).to(dt)
+    return h, c
+
+
 def nmt_attention_decoder_reference(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh,
                                     residual, w_q=None, g=None, v=None, b=None, w_a=None,
-                                    masks=None, output_attention=True):
+                                    masks=None, output_attention=True, ln=None):
     """Pure-PyTorch version of `nmt_attention_decoder` (same arguments, same masks): the fp64
     oracle of the node's tests.  State and gates are kept in the accumulation type (fp32 for
     bf16/fp32 inputs)."""
@@ -540,11 +724,15 @@ def nmt_attention_decoder_reference(emb, h0, c0, att0, keys, values, pad, w_ih, 
         x = torch.cat([emb[:, t], feed], -1)
         for l in range(L):
             inp = _mask_mul(x, None if masks is None else masks[l][t])
-            gates = _acc(torch.nn.functional.linear(inp, w_ih[l], b_ih[l]) +
-                         torch.nn.functional.linear(h[l], w_hh[l], b_hh[l]))
-            i, f, gg, o = gates.chunk(4, -1)
-            c[l] = torch.sigmoid(f) * c[l] + torch.sigmoid(i) * torch.tanh(gg)
-            h[l] = (torch.sigmoid(o) * torch.tanh(c[l])).to(dt)
+            bi, bh = (None, None) if b_ih is None else (b_ih[l], b_hh[l])
+            gates = _acc(torch.nn.functional.linear(inp, w_ih[l], bi) +
+                         torch.nn.functional.linear(h[l], w_hh[l], bh))
+            if ln is not None:
+                h[l], c[l] = _ln_cell_reference(gates, c[l], ln[l], dt)
+            else:
+                i, f, gg, o = gates.chunk(4, -1)
+                c[l] = torch.sigmoid(f) * c[l] + torch.sigmoid(i) * torch.tanh(gg)
+                h[l] = (torch.sigmoid(o) * torch.tanh(c[l])).to(dt)
             x = h[l] + x[..., :U] if residual[l] else h[l]
         q = x
         if v is not None:
@@ -593,6 +781,10 @@ def _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, save
     P = [torch.empty(T if save else 1, B, 4 * U, dtype=torch.float32, device=dev)
          for _ in range(L)]
     qc = torch.empty(T, B, U + M, dtype=dt, device=dev)
+    lnc = cfg["ln"]
+    stats = [torch.empty(T, B, 10, dtype=torch.float32, device=dev) if save else None
+             for _ in range(L)] if lnc is not None else None
+    lnp = [_ln_lstm_ptrs(W["ln"][l], lnc[l][0]) for l in range(L)] if lnc is not None else None
     align = torch.empty(T if save else 1, B, S, dtype=torch.float32, device=dev)
     pq = torch.empty(T if save else 1, B, U, dtype=torch.float32, device=dev) if bah else None
     att = torch.empty(T, B, U, dtype=dt, device=dev) if std else None
@@ -639,10 +831,17 @@ def _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, save
             else:
                 xn, xn_ld = _p(xh[l + 1][i0]), K[l + 1]
                 mk, mk_ld = (None, 0) if masks is None else (_p(masks[l + 1][t]), I[l + 1])
-            _check(Lb.px_nmt_lstm_cell_fwd(
-                _p(Pt), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]), _p(C[l][i0]),
-                _p(C[l][i1]), _addr(xh[l][i1], I[l]), K[l], resid, r_ld, y, y_ld, mk, mk_ld, xn,
-                xn_ld, B, U, _DT[dt], st), "nmt_lstm_cell_fwd")
+            if lnc is not None:
+                _check(Lb.px_nmt_ln_lstm_cell_fwd(
+                    _p(Pt), _p(gx0[t]) if l == 0 else None, _p(C[l][i0]), _p(C[l][i1]),
+                    _addr(xh[l][i1], I[l]), K[l], resid, r_ld, y, y_ld, mk, mk_ld, xn, xn_ld,
+                    _p(stats[l][t]) if save else None, *lnp[l], lnc[l][1], B, U, _DT[dt], st),
+                    "nmt_ln_lstm_cell_fwd")
+            else:
+                _check(Lb.px_nmt_lstm_cell_fwd(
+                    _p(Pt), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]),
+                    _p(C[l][i0]), _p(C[l][i1]), _addr(xh[l][i1], I[l]), K[l], resid, r_ld, y,
+                    y_ld, mk, mk_ld, xn, xn_ld, B, U, _DT[dt], st), "nmt_lstm_cell_fwd")
         q = qc[t][:, :U]
         pq_t = None
         if bah:
@@ -667,7 +866,7 @@ def _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, save
                     torch.mul(att[t], m0[t + 1, :, U:], out=dst)
     _count(T * (L + 1))
     return dict(xh=xh, C=C, P=P, qc=qc, align=align, pq=pq, att=att, gx0=gx0, w_step=w_step,
-                e_part=e_part, last=sl(T))
+                e_part=e_part, last=sl(T), stats=stats)
 
 
 def _nmt_outputs(cfg, F, U, output_attention):
@@ -688,6 +887,7 @@ class _NMTDecoderFn(torch.autograd.Function):
                  b_hh=rest[5 * L:6 * L], w_q=rest[6 * L], w_a=rest[6 * L + 4])
         attn = dict(w_q=rest[6 * L], g=rest[6 * L + 1], v=rest[6 * L + 2], b=rest[6 * L + 3])
         masks = None if rest[6 * L + 5] is None else rest[6 * L + 5:6 * L + 5 + L]
+        W["ln"] = _nmt_ln_params(cfg, rest)
         F = _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, True)
         ctx.cfg, ctx.n_in = cfg, n_in
         ctx.F = F
@@ -711,6 +911,11 @@ class _NMTDecoderFn(torch.autograd.Function):
         dt, dev = emb.dtype, emb.device
         xh, C, P, qc, align, pq, gx0, w_step = (F[k] for k in ("xh", "C", "P", "qc", "align",
                                                                 "pq", "gx0", "w_step"))
+        lnc, stats = cfg["ln"], F["stats"]
+        if lnc is not None:
+            lnw = _nmt_ln_params(cfg, rest)
+            lnp = [_ln_lstm_ptrs(lnw[l], lnc[l][0]) for l in range(L)]
+            acc = [torch.empty(B, 10 * U, dtype=torch.float32, device=dev) for _ in range(L)]
         I = [U + A] + [U] * (L - 1)
         K = [I[0] + U] + [I[l] + U for l in range(1, L)]
         m0 = None if masks is None else masks[0]
@@ -799,11 +1004,18 @@ class _NMTDecoderFn(torch.autograd.Function):
                 drec, drec_ld = (None, 0) if last else (_addr(dXH[l], off), dXH[l].shape[1])
                 dYp = _p(dY0[t]) if (l == 0 and res[0]) else (_p(dY[l]) if l > 0 and res[l]
                                                               else None)
-                _check(Lb.px_nmt_lstm_cell_bwd(
-                    _p(P[l][t]), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]),
-                    _p(C[l][t]), _p(C[l][t + 1]), a_, a_ld, am, am_ld, dR, o_, o_ld, drec,
-                    drec_ld, _p(dc[l]), _p(dG[l][t]), dYp, B, U, _DT[dt], st),
-                    "nmt_lstm_cell_bwd")
+                if lnc is not None:
+                    _check(Lb.px_nmt_ln_lstm_cell_bwd(
+                        _p(P[l][t]), _p(gx0[t]) if l == 0 else None, _p(stats[l][t]),
+                        _p(C[l][t]), a_, a_ld, am, am_ld, dR, o_, o_ld, drec, drec_ld,
+                        _p(dc[l]), _p(dG[l][t]), dYp, _p(acc[l]), int(last), *lnp[l],
+                        lnc[l][1], B, U, _DT[dt], st), "nmt_ln_lstm_cell_bwd")
+                else:
+                    _check(Lb.px_nmt_lstm_cell_bwd(
+                        _p(P[l][t]), _p(gx0[t]) if l == 0 else None, _p(b_ih[l]), _p(b_hh[l]),
+                        _p(C[l][t]), _p(C[l][t + 1]), a_, a_ld, am, am_ld, dR, o_, o_ld, drec,
+                        drec_ld, _p(dc[l]), _p(dG[l][t]), dYp, B, U, _DT[dt], st),
+                        "nmt_lstm_cell_bwd")
                 _mm_f32(dG[l][t], w_step[l], dXH[l])
         _count(T * (L + 1))
         nd = ctx.needs_input_grad
@@ -835,6 +1047,13 @@ class _NMTDecoderFn(torch.autograd.Function):
             else:
                 gl[2 * L + l] = torch.mm(dG2[l].t(), xh[l][:T, :, :I[l]].reshape(T * B, I[l]))
             gl[3 * L + l] = torch.mm(dG2[l].t(), xh[l][:T, :, I[l]:].reshape(T * B, U))
+            if lnc is not None:
+                dln = torch.empty(10, U, dtype=dt, device=dev)
+                _check(Lb.px_ln_lstm_param_grad(_p(acc[l]), B, U, _p(dln), _DT[dt], st),
+                       "ln_lstm_param_grad")
+                o = 7 * L + 5 + 10 * l
+                gl[o:o + 10] = list(dln.unbind(0))
+                continue
             db = torch.sum(dG2[l], 0, dtype=torch.float32)
             gl[4 * L + l] = db.to(rest[4 * L + l].dtype)
             gl[5 * L + l] = db.to(rest[5 * L + l].dtype)
@@ -859,21 +1078,35 @@ class _NMTDecoderFn(torch.autograd.Function):
         return (None, None, demb, datt0, dk, dv, None, *gl)
 
 
-def _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks):
+def _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks, ln=None):
+    """the node's tensor arguments; with LN-LSTM cells the 10 γ/β of each layer come last"""
     L = len(w_ih)
+    if b_ih is None:
+        b_ih = b_hh = [None] * L
     return (list(h0) + list(c0) + list(w_ih) + list(w_hh) + list(b_ih) + list(b_hh) +
-            [w_q, g, v, b, w_a] + (list(masks) if masks is not None else [None] * L))
+            [w_q, g, v, b, w_a] + (list(masks) if masks is not None else [None] * L) +
+            ([p for x in ln for p in x[0]] if ln is not None else []))
 
 
-def _nmt_cfg(L, residual, v, w_a, output_attention):
+def _nmt_ln_params(cfg, rest):
+    """per layer the 10 γ/β tensors from the node's tensor arguments (None for LSTM cells)"""
+    if cfg["ln"] is None:
+        return None
+    L = cfg["L"]
+    return [rest[7 * L + 5 + 10 * l:7 * L + 15 + 10 * l] for l in range(L)]
+
+
+def _nmt_cfg(L, residual, v, w_a, output_attention, ln=None):
     return {"L": L, "standard": w_a is not None, "bahdanau": v is not None,
             "residual": tuple(bool(r) for r in residual),
-            "output_attention": bool(output_attention)}
+            "output_attention": bool(output_attention),
+            "ln": None if ln is None else tuple((tuple(float(e) for e in x[1]), float(x[2]))
+                                                for x in ln)}
 
 
 def nmt_attention_decoder(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh, residual,
                           w_q=None, g=None, v=None, b=None, w_a=None, masks=None,
-                          output_attention=True):
+                          output_attention=True, ln=None):
     """All T steps of the NMT attention decoder's recurrence as ONE autograd node
     (`kernels/nmt_decoder.cu`).
 
@@ -888,19 +1121,25 @@ def nmt_attention_decoder(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih
 
     `masks` (per layer [T, B, I_l] in emb's dtype, or None) multiply each layer's input: the
     caller draws dropout there, from the same distribution as `F.dropout` but not from its
-    random stream.  Callers check `nmt_decoder_applies` first.  Without autograd nothing is
+    random stream.
+
+    `ln` (or None) makes every layer a layer-normalised LSTM (`LayerNormLSTM.cell`, gates i, j,
+    f, o): per layer (the 10 γ/β of LN_i, LN_j, LN_f, LN_o, LN_c then their β, the 5 eps, the
+    forget bias), with w_ih / w_hh the input and h columns of the bias-free kernel weight and
+    b_ih = b_hh = None.  Callers check `nmt_decoder_applies` first.  Without autograd nothing is
     kept for a backward pass; the node never synchronises with the host."""
     L = len(w_ih)
-    cfg = _nmt_cfg(L, residual, v, w_a, output_attention)
+    cfg = _nmt_cfg(L, residual, v, w_a, output_attention, ln)
     emb, att0 = emb.contiguous(), att0.contiguous()
     pad = pad.to(torch.bool).contiguous()
     if masks is not None:
         masks = [m.contiguous() for m in masks]
-    args = _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks)
+    args = _nmt_args(h0, c0, w_ih, w_hh, b_ih, b_hh, w_q, g, v, b, w_a, masks, ln)
     ins = [emb, att0, keys, values] + args
     if torch.is_grad_enabled() and any(a is not None and a.requires_grad for a in ins):
         return _NMTDecoderFn.apply(cfg, len(args), emb, att0, keys, values, pad, *args)
-    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a)
+    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a,
+             ln=None if ln is None else [x[0] for x in ln])
     attn = dict(w_q=w_q, g=g, v=v, b=b)
     F = _nmt_forward(cfg, emb, h0, c0, att0, keys, values, pad, W, attn, masks, False)
     return _nmt_outputs(cfg, F, emb.shape[2], output_attention)
@@ -908,14 +1147,16 @@ def nmt_attention_decoder(emb, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih
 
 @torch.no_grad()
 def nmt_attention_decoder_step(emb_t, h0, c0, att0, keys, values, pad, w_ih, w_hh, b_ih, b_hh,
-                               residual, w_q=None, g=None, v=None, b=None, w_a=None, masks=None):
+                               residual, w_q=None, g=None, v=None, b=None, w_a=None, masks=None,
+                               ln=None):
     """One decoding step (T = 1, nothing saved) of `nmt_attention_decoder` from emb_t [B, U] ->
     (q [B, U] the top layer's output, att [B, A] the new fed-back state: W_a·[q, ctx] for
     standard, ctx for gnmt, h per layer, c per layer in c0's dtype)."""
     L = len(w_ih)
-    cfg = _nmt_cfg(L, residual, v, w_a, True)
+    cfg = _nmt_cfg(L, residual, v, w_a, True, ln)
     U = emb_t.shape[1]
-    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a)
+    W = dict(w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh, w_q=w_q, w_a=w_a,
+             ln=None if ln is None else [x[0] for x in ln])
     attn = dict(w_q=w_q, g=g, v=v, b=b)
     F = _nmt_forward(cfg, emb_t[:, None, :].contiguous(), h0, c0, att0, keys, values,
                      pad.to(torch.bool).contiguous(), W, attn, masks, False)
