@@ -111,7 +111,8 @@ def _cell_grads(ops, n, live, dt):
             "dgx": leaves[1].grad, "dcx": leaves[2].grad, "carry": leaves[3].grad}
 
 
-@pytest.mark.parametrize("B,n", [(128, 2400), (128, 1200), (3, 16)])
+@pytest.mark.parametrize("B,n", [(128, 2400), (128, 1200), (3, 16), (4, 8), (4, 2048), (4, 2056),
+                                 (4, 4096)])
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float32])
 def test_cell_kernels_vs_fp64(B, n, dt):
     ops = _cell_operands(B, n, dt, seed=B + n)
@@ -136,7 +137,8 @@ def test_cell_kernels_vs_fp64(B, n, dt):
 def _module(I, n, seed):
     from parallax_b200.models.skip_thoughts.gru_cell import LayerNormGRU
     torch.manual_seed(seed)
-    m = LayerNormGRU(I, n).cuda()
+    with torch.device("cuda"):      # the orthonormal init's SVDs, on the device at large n
+        m = LayerNormGRU(I, n)
     with torch.no_grad():     # non-trivial LayerNorm parameters
         for ln in (m.ln_wx, m.ln_w, m.ln_wh, m.ln_u):
             ln.weight.add_(0.2 * torch.randn_like(ln.weight))
@@ -181,7 +183,13 @@ _LAYER_CASES = [
     (128, 620, 31, 1200, True, True, torch.bfloat16),
     (128, 620, 31, 1200, True, False, torch.float32),
 ] + [(5, 20, 7, 16, rev, h0, dt) for rev in (False, True) for h0 in (False, True)
-     for dt in (torch.bfloat16, torch.float32)] + [(3, 12, 4, 40, True, True, torch.bfloat16)]
+     for dt in (torch.bfloat16, torch.float32)] + [(3, 12, 4, 40, True, True, torch.bfloat16)] + [
+    # the largest n (two full groups per thread) and one thread with a second group
+    (4, 24, 3, 4096, False, True, torch.bfloat16),
+    (4, 24, 3, 4096, True, False, torch.float32),
+    (4, 20, 4, 2056, True, True, torch.bfloat16),
+    (3, 20, 1, 2056, False, False, torch.float32),
+]
 
 
 @pytest.mark.parametrize("B,I,T,n,rev,with_h0,dt", _LAYER_CASES)

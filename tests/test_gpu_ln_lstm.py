@@ -70,7 +70,7 @@ def _close(name, got, ref, dt):
     assert err <= tol * max(scale, 1e-3), (name, err, scale)
 
 
-@pytest.mark.parametrize("B,U", [(128, 512), (128, 1024), (3, 16)])
+@pytest.mark.parametrize("B,U", [(128, 512), (128, 1024), (3, 16), (4, 8), (4, 1032), (4, 2048)])
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float32])
 def test_cell_kernels_vs_fp64(B, U, dt):
     L = _lib()
@@ -193,7 +193,15 @@ _LAYER_CASES = [
     (128, 50, 1024, 1024, True, torch.bfloat16),
     (128, 50, 1024, 512, False, torch.float32),
 ] + [(5, 7, 20, 16, s, dt) for s in (False, True) for dt in (torch.bfloat16, torch.float32)] + \
-    [(3, 4, 12, 40, True, torch.bfloat16)]
+    [(3, 4, 12, 40, True, torch.bfloat16)] + [
+    # every thread on (U 2048), one thread past 1024, T 1, and odd I: W_h = w[:, I:] is then a
+    # view at a 2-byte offset in bf16
+    (4, 3, 24, 2048, True, torch.bfloat16),
+    (4, 2, 16, 1032, False, torch.float32),
+    (3, 1, 20, 1032, True, torch.bfloat16),
+    (4, 3, 13, 40, True, torch.bfloat16),
+    (4, 3, 1, 64, False, torch.bfloat16),
+]
 
 
 @pytest.mark.parametrize("B,T,I,U,with_state,dt", _LAYER_CASES)
@@ -387,7 +395,11 @@ _NODE_CASES = [
      for opt in ("luong", "scaled_luong", "bahdanau", "normed_bahdanau")
      for dt in (torch.bfloat16, torch.float32)] + \
     [(5, 6, 7, 16, 16, 1, opt, "gnmt_v2", True, torch.float32)
-     for opt in ("luong", "scaled_luong", "bahdanau", "normed_bahdanau")]
+     for opt in ("luong", "scaled_luong", "bahdanau", "normed_bahdanau")] + [
+    # the largest shape the gate accepts, and S past one softmax pass of 256 threads
+    (2, 2, 1024, 1024, 2048, 1, "scaled_luong", "standard", False, torch.float32),
+    (3, 3, 300, 64, 128, 1, "normed_bahdanau", "gnmt_v2", True, torch.bfloat16),
+]
 
 
 @pytest.mark.parametrize("B,T,S,U,M,L,option,arch,residual,dt", _NODE_CASES)
@@ -408,14 +420,17 @@ def test_decoder_node_vs_fp64(B, T, S, U, M, L, option, arch, residual, dt):
                            low[k].to(torch.float64), dt, factor=4.0 if ref[k].dim() == 0 else 2.0)
 
 
-@pytest.mark.parametrize("option,arch", [("luong", "standard"), ("normed_bahdanau", "standard"),
-                                         ("normed_bahdanau", "gnmt_v2"),
-                                         ("scaled_luong", "gnmt")])
-def test_decode_step_reproduces_teacher_forced_logits(option, arch, monkeypatch):
+@pytest.mark.parametrize("option,arch,S", [
+    pytest.param(o, a, 9, id="%s-%s" % (o, a))
+    for o, a in (("luong", "standard"), ("normed_bahdanau", "standard"),
+                 ("normed_bahdanau", "gnmt_v2"), ("scaled_luong", "gnmt"))] + [
+    # a source of the longest accepted length: every softmax loop runs four passes per thread
+    pytest.param("bahdanau", "standard", 1024, id="bahdanau-standard-S1024")])
+def test_decode_step_reproduces_teacher_forced_logits(option, arch, S, monkeypatch):
     from parallax_b200.ops import fused
     from tests.test_gpu_nmt_decoder import _batch, _model
     m = _model(option, arch, unit_type="layer_norm_lstm", dt=torch.float32).eval()
-    src, tgt, sl = _batch()
+    src, tgt, sl = _batch(S=S)
     calls = {"n": 0, "train": 0}
     real, real_train = fused.nmt_attention_decoder_step, fused.nmt_attention_decoder
 

@@ -79,7 +79,12 @@ def _attn64(q_or_pq, keys, values, pad, prm, bah):
 
 
 @pytest.mark.parametrize("B,S,U,M", [(128, 50, 512, 1024), (128, 50, 1024, 2048),
-                                     (128, 50, 1024, 1024), (3, 7, 16, 24)])
+                                     (128, 50, 1024, 1024), (3, 7, 16, 24),
+                                     # the largest accepted shape; S around one pass of the
+                                     # 256-thread softmax loops; one lane per score (U 8); M 8
+                                     (2, 1024, 1024, 2048), (3, 255, 32, 48), (3, 256, 32, 48),
+                                     (3, 257, 32, 48), (3, 1000, 64, 128), (3, 9, 8, 24),
+                                     (3, 9, 16, 8)])
 @pytest.mark.parametrize("option", OPTIONS)
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float32])
 def test_attention_kernels_vs_fp64(B, S, U, M, option, dt):
@@ -150,7 +155,7 @@ def test_attention_kernels_vs_fp64(B, S, U, M, option, dt):
                            got[k], ref[k], low[k].to(ref[k].dtype), dt)
 
 
-@pytest.mark.parametrize("B,U", [(128, 512), (128, 1024), (3, 24)])
+@pytest.mark.parametrize("B,U", [(128, 512), (128, 1024), (3, 24), (4, 8), (4, 1032)])
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float32])
 def test_cell_kernels_vs_fp64(B, U, dt):
     L = _lib()
@@ -276,7 +281,11 @@ _NODE_CASES = [
 ] + [(5, 6, 7, 16, 24, 3, opt, "standard", True, dt) for opt in OPTIONS
      for dt in (torch.bfloat16, torch.float32)] + \
     [(5, 6, 7, 16, 16, 1, opt, "gnmt", opt in ("luong", "bahdanau"), torch.float32)
-     for opt in OPTIONS]
+     for opt in OPTIONS] + [
+    # the largest shape the gate accepts, and S past one softmax pass of 256 threads
+    (2, 2, 1024, 1024, 2048, 1, "scaled_luong", "standard", False, torch.float32),
+    (3, 3, 300, 64, 128, 1, "normed_bahdanau", "gnmt_v2", True, torch.bfloat16),
+]
 
 
 @pytest.mark.parametrize("B,T,S,U,M,L,option,arch,residual,dt", _NODE_CASES)
@@ -346,13 +355,16 @@ def test_no_grad_forward_equals_training_forward(option, arch):
     assert torch.equal(a, b.detach())
 
 
-@pytest.mark.parametrize("option,arch", [("luong", "standard"), ("normed_bahdanau", "standard"),
-                                         ("normed_bahdanau", "gnmt_v2"),
-                                         ("scaled_luong", "gnmt")])
-def test_decode_step_reproduces_teacher_forced_logits(option, arch, monkeypatch):
+@pytest.mark.parametrize("option,arch,S", [
+    pytest.param(o, a, 9, id="%s-%s" % (o, a))
+    for o, a in (("luong", "standard"), ("normed_bahdanau", "standard"),
+                 ("normed_bahdanau", "gnmt_v2"), ("scaled_luong", "gnmt"))] + [
+    # a source of the longest accepted length: every softmax loop runs four passes per thread
+    pytest.param("scaled_luong", "standard", 1024, id="scaled_luong-standard-S1024")])
+def test_decode_step_reproduces_teacher_forced_logits(option, arch, S, monkeypatch):
     from parallax_b200.ops import fused
     m = _model(option, arch, dt=torch.float32).eval()
-    src, tgt, sl = _batch()
+    src, tgt, sl = _batch(S=S)
     calls = {"n": 0}
     real = fused.nmt_attention_decoder_step
 
